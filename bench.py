@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BN254 G1 MSM points/s (+ Fr NTT elements/s) at 2^24 on B200, one process per GPU.
+"""bench.py -- BN254 G1 MSM points/s (+ Fr NTT elements/s) at 2^24 on an H100, one process per GPU.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -88,6 +88,26 @@ def ntt_products_per_element(log_n: int, full_table_max_log: int = 26) -> float:
     return total
 
 
+def gpu_identity(index: int) -> dict:
+    """name and power limit of the card the numbers were measured on (a rate means little without them)"""
+    try:
+        r = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        name, watts, mhz = [x.strip() for x in r.stdout.strip().split(",")]
+        return {"name": name, "power_limit_w": float(watts), "sm_max_mhz": float(mhz)}
+    except Exception:  # noqa: BLE001
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(out_dir: str, arrays: dict):
+    """--dump-outputs: one float64 .npy per output (254-bit values as 32-bit limbs, which float64 holds exactly)"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 def emit_result(line: dict):
     out = _RESULT_OUT or sys.stdout
     out.write(json.dumps(line) + "\n")
@@ -130,7 +150,7 @@ def _peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback: H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -325,6 +345,20 @@ def run_gpu(args):
     elif args.window:
         ctx.set_msm_window(args.window)
     result = {}
+    # what the timed paths returned in their last step (--dump-outputs): points and proofs as the caller receives them
+    # (big-endian bytes, as 32-bit words), the NTT as a fixed seeded sample of 2^16 elements (8 Montgomery limbs each).
+    # The NTT loops transform ONE buffer in place, warmup + steps times, so the forward sample is NTT^(warmup+steps) of
+    # the seeded input x and the inverse sample INTT^(warmup+steps)(NTT(x)): fixed for fixed arguments, and a restore
+    # of the input per step would put a 512 MiB copy into the timed region.
+    dumps = {}
+
+    def words(b: bytes):
+        return np.frombuffer(b, dtype=">u4").astype(np.float64)
+
+    ntt_rows = np.sort(np.random.default_rng(0).choice(n, min(n, 1 << 16), replace=False))
+
+    def ntt_sample(d):
+        return d.view(n, 4)[torch.from_numpy(ntt_rows).cuda()].cpu().numpy().view(np.uint32).astype(np.float64)
 
     from ethrex_b200.dist import msm_sharded, shard_range
 
@@ -369,6 +403,7 @@ def run_gpu(args):
     msm_step_stats = {}
     ms_step, launches, clocks = timed_loop(msm_step, args.steps, args.warmup, msm_step_stats)
     value = world * n / (ms_step / 1e3)
+    dumps["g1_msm"] = words(result["out"])
 
     # ---- correctness of what was timed: closed form of the chain MSM (rank 0, outside the timed region)
     import cpu_oracle as orc  # the checker (and the cpu_baseline leg): never inside a timed GPU region
@@ -427,7 +462,7 @@ def run_gpu(args):
         ctx.set_profiling(False)
         return sum(acc) / len(acc), ph
 
-    acc, phases = phase_times(lambda: ctx.g1_msm_partial_resident_device(handle, d_scalars, n, d_partial), max(2, min(args.steps, 5)))
+    acc, phases = phase_times(lambda: ctx.g1_msm_partial_resident_device(handle, d_scalars, n, d_partial), args.steps)
     peak, peak_src = _peaks()
     algo_bytes = n * 96 + 64  # SURVEY.md 8(d): n x (32 B scalar + 64 B affine base) read + 64 B written
     achieved = algo_bytes / (acc / 1e3) / 1e9
@@ -454,7 +489,7 @@ def run_gpu(args):
     if not args.no_plain and world == 1 and not args.no_precompute:
         hp = ctx.g1_bases_from_device(d_points, n)
         st = {}
-        pms, _, _ = timed_loop(lambda: result.__setitem__("plain", ctx.g1_msm_resident_device(hp, d_scalars, n)), max(3, args.steps // 2), 2, st)
+        pms, _, _ = timed_loop(lambda: result.__setitem__("plain", ctx.g1_msm_resident_device(hp, d_scalars, n)), args.steps, 2, st)
         ctx.bases_free(hp)
         assert result["plain"] == result["out"]
         plain = {"value": n / (pms / 1e3), "unit": "points/s", "ms_per_step": pms,
@@ -497,15 +532,15 @@ def run_gpu(args):
         ctx.synchronize()
         g2_setup = time.perf_counter() - t0
         st2 = {}
-        g2_steps = max(3, args.steps // 2)
-        g2ms, g2l, _ = timed_loop(lambda: result.__setitem__("g2", ctx.g2_msm_resident_device(h2, d_scalars, g2n)), g2_steps, 2, st2)
+        g2ms, g2l, _ = timed_loop(lambda: result.__setitem__("g2", ctx.g2_msm_resident_device(h2, d_scalars, g2n)), args.steps, 2, st2)
+        dumps["g2_msm"] = words(result["g2"])
         g2_ok = None
         if not args.no_verify:
             g2_ok = bool(closed_form(g2n, SEED_SCALARS, g2=True) == result["g2"])
             if not g2_ok:
                 raise SystemExit("bench.py: GPU G2 MSM result differs from the oracle's closed form")
         d_partial2 = torch.zeros(32, dtype=torch.int64, device="cuda")
-        acc2, ph2 = phase_times(lambda: ctx.g2_msm_partial_resident_device(h2, d_scalars, g2n, d_partial2), 2)
+        acc2, ph2 = phase_times(lambda: ctx.g2_msm_partial_resident_device(h2, d_scalars, g2n, d_partial2), args.steps)
         g2_bytes = g2n * 160 + 128
         prof2 = ncu_profile("msm_accumulate_g2") if default_cfg else None
         # multiply instructions of one G2 mixed addition in units of one Fq product (136 instructions):
@@ -515,7 +550,7 @@ def run_gpu(args):
         if not args.no_e2e:
             hs = torch.empty(4 * g2n, dtype=torch.int64).pin_memory()
             hs.copy_(d_scalars)
-            wall = wall_loop(lambda: result.__setitem__("g2e", ctx.g2_msm_resident(h2, hs, g2n)), g2_steps, 1)
+            wall = wall_loop(lambda: result.__setitem__("g2e", ctx.g2_msm_resident(h2, hs, g2n)), args.steps, 1)
             assert result["g2e"] == result["g2"]
             g2e = {"value": g2n / wall, "unit": "points/s", "ms_per_step": wall * 1e3, "h2d_bytes_per_step": g2n * 32, "d2h_bytes_per_step": 128,
                    "api": "b200zk_g2_msm_resident (pinned host scalars -> 128 result bytes; bases resident)"}
@@ -549,11 +584,12 @@ def run_gpu(args):
             ctx.bases_precompute(hs_, 0)
             sc = torch.empty(4 * m, dtype=torch.int64, device="cuda")
             ctx.fr_random_device(sc, m, SEED_SCALARS, lo)
-            sms, _, _ = timed_loop(lambda: result.__setitem__("s" + tag, msm_sharded(ctx, None, sc, m, g2=is_g2, handle=hs_)), max(3, args.steps // 2), 2)
+            sms, _, _ = timed_loop(lambda: result.__setitem__("s" + tag, msm_sharded(ctx, None, sc, m, g2=is_g2, handle=hs_)), args.steps, 2)
             ctx.bases_free(hs_)
             del sc
             torch.cuda.empty_cache()
             strong[tag + "_ms"] = sms
+            dumps[tag + "_msm_strong"] = words(result["s" + tag])
             strong[tag + "_points_per_s"] = n / (sms / 1e3)
             # the same MSM on ONE GPU, in the same run (rank 0 alone; the other ranks wait at the barrier)
             if not args.no_strong_n1:
@@ -571,7 +607,7 @@ def run_gpu(args):
                         result["one" + tag] = fn1(h1, sc1, n)
                     torch.cuda.synchronize()
                     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    reps = 3
+                    reps = args.steps
                     e0.record()
                     for _ in range(reps):
                         fn1(h1, sc1, n)
@@ -598,9 +634,12 @@ def run_gpu(args):
         ctx.fr_random_device(d_ntt, n, SEED_NTT, start, eb.SCALARS_MONT)
         ref = d_ntt.clone()
         fwd_ms, fl, _ = timed_loop(lambda: ctx.fr_ntt_device(d_ntt, log_n, 0), args.steps, args.warmup)
+        dumps["ntt_forward_sample"] = ntt_sample(d_ntt)
         d_ntt.copy_(ref)
         ctx.fr_ntt_device(d_ntt, log_n, 0)
         inv_ms, _, _ = timed_loop(lambda: ctx.fr_ntt_device(d_ntt, log_n, eb.NTT_INVERSE), args.steps, args.warmup)
+        dumps["ntt_inverse_sample"] = ntt_sample(d_ntt)
+        dumps["ntt_sample_rows"] = ntt_rows.astype(np.float64)
         # round trip check on fresh data
         d_ntt.copy_(ref)
         ctx.fr_ntt_device(d_ntt, log_n, 0)
@@ -623,7 +662,7 @@ def run_gpu(args):
         if not args.no_e2e and world == 1:
             h_ntt = torch.empty(4 * n, dtype=torch.int64).pin_memory()
             h_ntt.copy_(ref)
-            wall = wall_loop(lambda: ctx.fr_ntt(h_ntt, log_n, 0), max(2, args.steps // 2), 1)
+            wall = wall_loop(lambda: ctx.fr_ntt(h_ntt, log_n, 0), args.steps, 1)
             ntt["e2e"] = {"value": n / wall, "unit": "elements/s", "ms_per_step": wall * 1e3, "h2d_bytes_per_step": 32 * n, "d2h_bytes_per_step": 32 * n,
                           "api": "b200zk_fr_ntt (pinned host buffer, in place): PCIe-bound, 2 x 512 MiB per transform"}
             del h_ntt
@@ -643,12 +682,13 @@ def run_gpu(args):
         backend = B200Backend(ctx, circuit)
         backend.prove({"batch": 0})  # warm-up (workspaces, twiddles)
         times, digests, pl0 = [], [], ctx.launch_count
-        reps = max(2, min(args.steps, 5))
+        reps = args.steps
         for i in range(reps):
             barrier()
             pr, dt = backend.prove_timed({"batch": i + 1}, ProofFormat.GROTH16)
             times.append(max_over_ranks(dt))
             digests.append(pr.proof.hex()[:16])
+        dumps["proof"] = words(pr.proof)
         proof_launches = (ctx.launch_count - pl0) // reps
         # same bytes on every rank (the fold is replicated)
         if world > 1:
@@ -671,7 +711,7 @@ def run_gpu(args):
                  "domain_log2": args.proof_log_n, "proving_key_setup_s": setup_s, "n_gpus": world, "proof_prefix": digests[-1], "gpu_launches_per_proof": proof_launches,
                  "api": "B200Backend.prove -> ONE b200zk_groth16_commit call (device inputs), one synchronisation" if world == 1 else
                         "B200Backend.prove -> dealt NTTs (3 broadcasts), b200zk_groth16_commit_partial, ONE all_gather of 768-byte blocks, b200zk_groth16_fold",
-                 "separate_calls_ms": sep_ms, "timed_log_line": log_proved(reps, med),
+                 "separate_calls_ms": sep_ms, "timed_log_line": log_proved(reps, med), "plain_columns": circuit.plain_columns,
                  "work": "3 iNTT + 3 coset NTT + quotient + 1 coset iNTT, 4 G1 MSM + 1 G2 MSM (synthetic R1CS, chain proving key, no blinding; STARK stage excluded)",
                  "real_input_leg": "absent: decoding fixtures/cache/rpc_prover/cache_hoodi_1265656.json into a witness needs the Rust ProgramInput types and the zkVM's "
                                    "wrap circuit, neither available here; the witness is derived deterministically from the serialized input instead"}
@@ -705,6 +745,7 @@ def run_gpu(args):
     if rank == 0:
         line = {
             "metric": "bn254_g1_msm_points_per_sec", "value": value, "unit": "points/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
+            "gpu": gpu_identity(local),
             "ms_per_step": ms_step, "step_ms": msm_step_stats, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u32x8 Montgomery (254-bit modular integer)", "data": "synthetic",
             "config": {"workload": f"2^{log_n}-point BN254 G1 MSM per GPU (chain bases P_i=(k+i*d)G, uniform Fr scalars), bases+scalars resident in HBM",
@@ -716,6 +757,8 @@ def run_gpu(args):
             "g2": g2, "strong": strong, "ntt": ntt, "proof": proof, "cpu_baseline": cpu,
         }
         emit_result(line)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumps)
     ctx.close()
     if world > 1:
         dist.destroy_process_group()
@@ -744,6 +787,7 @@ def main():
     ap.add_argument("--no-proof-separate", action="store_true")
     ap.add_argument("--no-precompute", action="store_true", help="plain resident bases (no 2^(cw) P_i table)")
     ap.add_argument("--window", type=int, default=0, help="force the MSM window bits (0 = automatic)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the timed paths returned in their last step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,6 +1,6 @@
-"""ethrex_b200 -- host side of the B200-native BN254 MSM + Fr NTT backend for ethrex's L2 prover.
+"""ethrex_b200 -- host side of the H100-native BN254 MSM + Fr NTT backend for ethrex's L2 prover.
 
-Everything numerical happens in libb200zk.so (hand-written sm_100a CUDA behind the C ABI of
+Everything numerical happens in libb200zk.so (hand-written sm_90a CUDA behind the C ABI of
 include/b200zk.h); this package is the Python twin of the Rust shim in rust/ (the reference's
 toolchain is absent from the build image).  There is no CPU fallback.
 """

@@ -1,4 +1,4 @@
-"""Host-side handle on one B200: the Python mirror of the `B200zk` wrapper in rust/ethrex-backend.
+"""Host-side handle on one H100: the Python mirror of the `B200zk` wrapper in rust/ethrex-backend.
 
 One `Context` per process per GPU (SURVEY.md section 8b: the reference's prover actor runs on one
 blocking thread, `/root/reference/crates/prover/src/prover.rs:240-251`, and scales out as one process

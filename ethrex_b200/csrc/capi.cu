@@ -186,7 +186,7 @@ int b200zk_init(int device, b200zk_ctx** out) {
   for (auto& e : ctx->ev) cudaEventCreate(&e);
   {
     // The accumulation gathers 64-byte affine points at random: with the default L2 fetch granularity every gather pulls
-    // 128 bytes out of HBM (ncu r1c: 29.3 GB read per 2^24 MSM against 14.8 GB of gathers).  A 64-byte granularity is
+    // 128 bytes out of HBM, twice the bytes the gather uses.  A 64-byte granularity is
     // all this library's access patterns need (every stream it reads is either contiguous or 64/128-byte records).
     // The limit is a per-device hint; B200ZK_L2_FETCH=0 leaves the device default, 32 / 64 / 128 set it explicitly.
     const char* e = getenv("B200ZK_L2_FETCH");

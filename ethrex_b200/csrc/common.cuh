@@ -48,7 +48,7 @@ struct BasesEntry {
 
 struct b200zk_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   std::string last_error;
   uint64_t launches = 0;

@@ -1,4 +1,4 @@
-// curve.cuh -- BN254 G1 (over Fq) and G2 (over Fq2) group law for sm_100a, y^2 = x^3 + b, a = 0.
+// curve.cuh -- BN254 G1 (over Fq) and G2 (over Fq2) group law for sm_90a, y^2 = x^3 + b, a = 0.
 //
 // Affine points are the HBM-resident base format: (x, y) in Montgomery form, (0,0) = identity (the
 // EIP-196/197 convention of /root/reference/crates/common/crypto/provider.rs:201-330).  Accumulators use

@@ -1,4 +1,4 @@
-// field.cuh -- 254-bit prime-field arithmetic for sm_100a: BN254 base field Fq and scalar field Fr,
+// field.cuh -- 254-bit prime-field arithmetic for sm_90a: BN254 base field Fq and scalar field Fr,
 // Montgomery form with R = 2^256, eight 32-bit limbs per element (little-endian; the same bytes as
 // ark-ff's Fp256<MontBackend> 4x64 in-memory form on a little-endian host).
 //
@@ -504,8 +504,7 @@ struct Fq2 {
   static B2_D Fq2 neg(const Fq2& a) { return {Fq::neg(a.c0), Fq::neg(a.c1)}; }
   // Schoolbook with ONE reduction per component: c0 = a0 b0 + (p - a1) b1, c1 = a0 b1 + a1 b0 -- 2 x 200 multiply
   // instructions and one negation.  Karatsuba (3 x 136 and five additions/subtractions with their temporaries) was
-  // the first version: measured on B200, the G2 MSM accumulation went 35.1 -> 30.4 ms at 2^22 with this form
-  // (profiles/r1h_g2.md); the register pressure of the temporaries cost more than the 8 multiply instructions saved.
+  // the first version and slower: the register pressure of the temporaries cost more than the 8 multiply instructions saved.
   static B2_D Fq2 mul(const Fq2& a, const Fq2& b) {
     return {Fq::mul2_add(a.c0, b.c0, Fq::neg(a.c1), b.c1), Fq::mul2_add(a.c0, b.c1, a.c1, b.c0)};
   }

@@ -1,4 +1,4 @@
-// msm.cu -- windowed Pippenger multi-scalar multiplication over BN254 G1 / G2 for sm_100a.
+// msm.cu -- windowed Pippenger multi-scalar multiplication over BN254 G1 / G2 for sm_90a.
 //
 // Replaces ark_ec::VariableBaseMSM::msm (ark-ec 0.5.0, /root/reference/Cargo.lock:978) as reached by the
 // Groth16 wrap behind /root/reference/crates/prover/src/backend/sp1.rs:97-134 and risc0.rs:24-29,71-82
@@ -28,7 +28,7 @@ namespace b200zk {
 
 static constexpr int kMaxWindows = 64;
 static constexpr uint32_t kMaxPipelineChunks = 64;  // = events in b200zk_ctx::ev_up
-static constexpr int kChunk = 16;  // buckets per running-sum chunk (measured 8/16/32/64: profiles/r1h_g2.md)
+static constexpr int kChunk = 16;  // buckets per running-sum chunk (B200ZK_CHUNK=8|32|64 selects others)
 static constexpr int kG2MinBlocks = 1;  // register cap of msm_accumulate<Fq2> (see the launch site)
 
 struct MsmPlan {
@@ -44,8 +44,8 @@ struct MsmPlan {
 uint32_t precompute_window(size_t n) {
   uint32_t lg = 0;
   while (((size_t)1 << lg) < n) ++lg;
-  // measured on B200 (profiles/): c = 20 wins at 2^20 and 2^24 (beyond it the scatter's atomics over 2^(c-1)
-  // counters and the bucket reduction cost more than the saved window)
+  // c = 20: a G1 MSM at 2^24 on an H100 SXM (700 W) takes 48.1 / 45.2 / 41.6 / 44.0 ms at c = 18 / 19 / 20 / 21 (beyond
+  // 20 the sort over 2^(c-1) buckets and the bucket reduction cost more than the saved window)
   if (lg >= 20) return 20;
   if (lg <= 6) return 6;
   return lg;
@@ -56,7 +56,8 @@ uint32_t precompute_window(size_t n) {
 static MsmPlan make_plan(size_t n, uint32_t forced_c, uint32_t scalar_bits = 255) {
   uint32_t lg = 0;
   while (((size_t)1 << lg) < n) ++lg;
-  // measured on B200 (profiles/): c = 16 is best for 2^18..2^22 points, 17 from 2^23 up; below that lg-4
+  // c = 16 for 2^18..2^22 points, 17 from 2^23 up; below that lg-4.  At 2^24 on an H100 SXM at a 400 W power limit a G1
+  // MSM over plain bases takes 54.8-54.9 / 52.4-52.8 / 54.9 ms at c = 16 / 17 / 18 (median step, two alternating runs)
   uint32_t c = forced_c ? forced_c : (lg > 8 ? lg - 4 : 4);
   if (!forced_c && c > 16) c = lg >= 23 ? 17 : 16;
   if (c < 2) c = 2;
@@ -129,8 +130,7 @@ static constexpr uint32_t kNoDigit = 0xffffffffu;
 
 // One atomic per distinct key per warp: hot buckets (top window, scalars 0/1/small) would otherwise serialise
 // 32 atomics on one L2 address.  Returns the warp-wide count of `key` and this lane's rank within its group.
-// MATCH costs about as many address-divergence-unit cycles as the divergent atomic it saves (ncu r1f: pipe_adu 89 %
-// busy in msm_hist, 73-92 % in msm_scatter), so it only runs when the warp shows skew: `adaptive` first counts the
+// MATCH costs about as many address-divergence-unit cycles as the divergent atomic it saves, so it only runs when the warp shows skew: `adaptive` first counts the
 // lanes that carry the first active lane's key (one SHFL + one VOTE); fewer than kSkewLanes of them and every lane
 // simply is its own group.  Uniform digits (the prover's case) take the cheap path, a hot bucket the exact one.
 static constexpr uint32_t kSkewLanes = 3;
@@ -195,8 +195,8 @@ __global__ void __launch_bounds__(kHistTile) msm_hist(const void* scalars, size_
 }
 
 // kScatterIlp independent entries per thread per iteration: the slot allocation is an L2 atomic WITH return, i.e. a
-// full round trip per entry; with one entry in flight per thread the kernel was latency bound (ncu: long_scoreboard
-// 22.8 stall cycles per issue, LTS 41 % busy), so each thread keeps several allocations in flight.
+// full round trip per entry; with one entry in flight per thread the kernel is latency bound, so each thread keeps
+// several allocations in flight.
 static constexpr int kScatterIlp = 4;
 __global__ void __launch_bounds__(256) msm_scatter(const uint32_t* __restrict__ digits, size_t n, MsmPlan pl, uint32_t* cursor, uint32_t* idx) {
   const size_t total = (size_t)pl.W * n;
@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(256) msm_scatter(const uint32_t* __restrict__ 
 
 // ---- two-level sort (r2): tile-local counting sort in shared memory, no per-entry global atomic ------------------------
 // The r1 sort paid, per entry, one divergent L2 reduction (msm_hist), one divergent L2 atomic WITH return and one
-// divergent 4-byte store (msm_scatter): the SM's address-divergence unit was the limit (profiles/r1f_prof_sort_summary.md).
+// divergent 4-byte store (msm_scatter): the SM's address-divergence unit is the limit.
 // Here the (window,bucket) key g of an entry is split into a coarse bin (g >> fb) and a fine key (g & (2^fb - 1)):
 //   msm_sort_count   every CTA owns a CONTIGUOUS range of scalars; it recodes them (scalar tiles staged by the copy engine,
 //                    as in msm_hist) and counts its entries per coarse bin in shared memory -> cnt[bin][cta]
@@ -416,9 +416,9 @@ __global__ void __launch_bounds__(kSortTile, 1) msm_sort_coarse(const void* __re
 }
 
 // ---- fine pass, balanced: work items are SEGMENTS of kFineSeg entries of a coarse bin ------------------------------------
-// One CTA per coarse bin (the first r2 version) is as unbalanced as the bins are -- and they are: the top window of a
-// 254-bit scalar only has 254 - 240 = 14 bits at c = 20, so all of its 2^24 entries land in the 16 lowest bins (3.5x the
-// average; at c = 19 / 21 / 22 in one or two bins: 12-13 ms), and skewed witnesses do the same to any bin.  Now:
+// One CTA per coarse bin would be as unbalanced as the bins are -- and they are: the top window of a 254-bit scalar
+// only has 254 - 240 = 14 bits at c = 20, so all of its 2^24 entries land in the 16 lowest bins (3.5x the average; at
+// c = 19 / 21 / 22 in one or two bins), and skewed witnesses do the same to any bin.  Now:
 //   msm_sort_items     item_start[b] = sum_{b' < b} ceil(size(b') / kFineSeg)                          (one small CTA)
 //   msm_sort_fine_count  item i = (bin, segment): histogram of its entries' fine keys -> cnt2[i][key]
 //   msm_sort_fine_prefix thread (bin, key): exclusive prefix of cnt2[.][key] over the bin's segments, total -> hist[g]
@@ -641,8 +641,7 @@ static constexpr uint32_t kSegLenMax = 256;  // the slice length itself is a lau
 static constexpr uint32_t kTreeRadix = 64;
 // Buckets with at most kDirectRuns runs are NOT folded by partial_tree: their consumers (bucket_chunk, bucket_merge) add
 // the runs themselves.  With slices of ~240 entries and buckets of ~416 (c = 20 at 2^24) nearly every bucket has 2-3 runs:
-// folding them in the tree kernel kept one lane in 2.6 busy (0.73 ms per G1 MSM, ncu r2); the consumers walk buckets
-// anyway.  The tree only remains for heavy buckets (skewed scalars).
+// folding them in the tree kernel keeps only one lane in 2-3 busy; the consumers walk buckets anyway.  The tree only remains for heavy buckets (skewed scalars).
 static constexpr uint32_t kDirectRuns = 4;
 
 // Slice length for M entries: every thread does the same work, so the launch runs in lock-step "waves" of
@@ -718,8 +717,8 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate(const void* __restri
 
 // ---- G2 accumulation on lane pairs -----------------------------------------------------------------------------
 // msm_accumulate<Fq2> keeps an XYZZ accumulator over Fq2 (64 registers), the point and its prefetch (2 x 32) and the
-// temporaries of an Fq2 product in ONE thread: 255 registers, 2 CTAs (8 warps) per SM, ~74 % of the multiplier ceiling
-// (r2c bench).  Here two adjacent lanes share one slice: lane 2k holds the real component (c0) of every Fq2 value,
+// temporaries of an Fq2 product in ONE thread: 255 registers, 2 CTAs (8 warps) per SM, too few warps to cover the
+// carry chains' latency.  Here two adjacent lanes share one slice: lane 2k holds the real component (c0) of every Fq2 value,
 // lane 2k+1 the imaginary one (c1) -- half the registers per thread, the occupancy of the G1 kernel -- and the
 // components an Fq2 product needs from the partner lane travel by SHFL.XOR 1 (8 shuffles per value, ~90 per mixed
 // addition against ~1800 wide multiplies per lane).  Every product stays a shared-reduction form of field.cuh:
@@ -731,11 +730,11 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate(const void* __restri
 // slice scheme and run numbering are those of msm_accumulate: the other kernels do not know the difference.
 // The three products of the lane-pair kernel as REAL functions (arguments and result travel in registers: checked in SASS,
 // no local-memory traffic).  Inlined, one G2 mixed addition is ~3500 SASS instructions = 56 KB and the loop body does not
-// fit the instruction cache (ncu r2g: stall_no_instruction 1.2 per issue, the top stall); as calls the body is ~13 KB plus
+// fit the instruction cache (instruction-cache misses were the top stall); as calls the body is ~13 KB plus
 // ~13 KB of callees, the size of the G1 kernel's body.
 // One product per call: callees that compute the two independent products the formulas offer at every step (U2 | S2,
-// PP | R^2, PPP | Q, ZZ3 | ZZZ3) were measured too and lose (111-115 ms against 106 ms at 2^24: marshalling 64 argument
-// registers per call costs more than the second carry chain per warp gains; profiles/r2_g2_pair*.jsonl).
+// PP | R^2, PPP | Q, ZZ3 | ZZZ3) lose: marshalling 64 argument registers per call costs more than the second carry
+// chain per warp gains.
 __device__ __noinline__ Fq fq_mul_call(Fq a, Fq b) { return Fq::mul(a, b); }
 __device__ __noinline__ Fq fq_mul2_add_call(Fq a, Fq b, Fq c, Fq d) { return Fq::mul2_add(a, b, c, d); }
 __device__ __noinline__ Fq fq_mul4_add_call(Fq a, Fq b, Fq c, Fq d, Fq e, Fq f, Fq g, Fq h) { return Fq::mul4_add(a, b, c, d, e, f, g, h); }
@@ -852,7 +851,7 @@ __global__ void __launch_bounds__(128, MINB) msm_accumulate_g2_pair(const void* 
   XYZZHalf acc = {Fq::zero(), Fq::zero(), Fq::zero(), Fq::zero()};
   // The next point is prefetched into L2 (prefetch.global.L2), not into registers: with the 16 registers of a register
   // prefetch the kernel needs 168+ registers; an addition (~1800 wide multiplies per lane) is long enough for the other
-  // warps to cover an L2 hit (measured: accumulation 110.3 -> 106.2 ms at 2^24).
+  // warps to cover an L2 hit.
   auto prefetch_half = [&](uint32_t v) {
     const uint8_t* q = reinterpret_cast<const uint8_t*>(points) + (4 * (size_t)(v & 0x7fffffffu) + comp) * 32;
     asm volatile("prefetch.global.L2 [%0];" ::"l"(q));
@@ -1256,7 +1255,8 @@ static inline void phase_mark(b200zk_ctx* ctx, int k, cudaStream_t st) {
 // ---- accumulation launch: G1 one thread per slice; G2 one lane PAIR per slice (msm_accumulate_g2_pair) unless the knob says otherwise
 static int g2_pair_knob() {
   // experiment knob B200ZK_G2_PAIR=0: the one-thread-per-slice G2 kernel; 3 | 4: CTAs per SM the lane-pair kernel is
-  // compiled for (154 registers, no spills | 128 registers, spills).  Default 3 (measured: 106.2 | 107.0 ms at 2^24)
+  // compiled for (154 registers, no spills | 128 registers, spills).  Default 3: a G2 MSM at 2^24 on an H100 SXM at a
+  // 400 W power limit takes 134.8 | 138.6-143.8 ms (median step, two alternating runs each)
   static int k = -1;
   if (k < 0) { const char* e = getenv("B200ZK_G2_PAIR"); k = (e && (*e == '0' || *e == '3' || *e == '4')) ? (*e - '0') : 3; }
   return k;
@@ -1330,7 +1330,7 @@ static int run_two_level_sort(b200zk_ctx* ctx, const void* d_scalars, size_t n, 
 }
 
 // ---- chunk-pipelined schedule --------------------------------------------------------------------------------
-// Host scalars arrive over PCIe (512 MiB at 2^24: ~10 ms, a quarter of the MSM).  The points are cut into K chunks;
+// Host scalars arrive over PCIe (512 MiB at 2^24, a sizeable fraction of the MSM's time).  The points are cut into K chunks;
 // chunk k's scalars are uploaded on a second stream while earlier chunks are being sorted and accumulated, so that only
 // the FIRST chunk's upload is exposed.  r1 also ran the sort of chunk k+1 concurrently with the accumulation of chunk k
 // (second stream, a shared-memory reservation to keep room on the SMs); with the r2 two-level sort -- whose CTAs want a
@@ -1349,8 +1349,7 @@ static int msm_run_pipelined(b200zk_ctx* ctx, const void* d_points, const void* 
   size_t bnd[kMaxPipelineChunks + 1];
   uint32_t chunks = 0;
   {
-    // measured at 2^24 (tools/e2e_sweep.py, profiles/r2_e2e_sweep.jsonl): G1 3 chunks x4 (37.8 ms against 40.2 ms for 4 equal
-    // chunks, 35.9 ms resident), G2 2 chunks x12 (115.7 against 118.7, 112.4 resident): the ratio tracks compute time / copy time
+    // G1 3 chunks x4, G2 2 chunks x12 (tools/e2e_sweep.py sweeps them): the ratio tracks compute time / copy time
     const double r = h_scalars ? chunk_ratio_knob(IsFq2<F>::value ? 12.0 : 4.0) : 1.0;
     double tot = 0, w = 1;
     for (uint32_t k = 0; k < K; ++k) { tot += w; w *= r; }
@@ -1434,8 +1433,8 @@ static int msm_run_pipelined(b200zk_ctx* ctx, const void* d_points, const void* 
     const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
     const uint32_t L = Lk[k];
     const size_t slices = (nk * pl.W + L - 1) / L;
-    // sort(k) waits for upload k only: with the kernels serialised there is nothing to gain from sorting ahead (measured:
-    // sort(k+1) before accumulate(k) stalls the stream on upload k+1 -- 42.0 ms at 2^24 against the order below)
+    // sort(k) waits for upload k only: with the kernels serialised there is nothing to gain from sorting ahead, and
+    // sort(k+1) before accumulate(k) would stall the stream on upload k+1
     B2_TRY(sort_chunk(k));
     SortSlot& s = ctx->slot[k & 1];
     const void* pts = (const uint8_t*)d_points + lo * pt;
@@ -1491,11 +1490,9 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
   if ((unsigned long long)n * pl.W >= (1ull << 32)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: n * windows must be < 2^32 (shard the MSM)");
   {
     // large inputs: chunk-pipelined schedule (unless phases are being profiled or pair rounds are forced)
-    // measured on B200 (profiles/r1_probe.md): with scalars already in HBM one shot is as fast as any chunking
-    // (40.9 ms vs 40.0-42 ms at 2^24: the accumulation fills the SMs, so the next chunk's sort barely overlaps);
-    // with HOST scalars 4 chunks hide most of the 512 MiB upload (50.5 -> 41.9 ms)
-    // chunks of the host-scalar pipeline: few and geometrically growing (msm_run_pipelined); with EQUAL chunks 4 was best
-    // (45.5 / 41.3 / 40.2 / 41.4 ms for 1 / 2 / 4 / 8 chunks against 35.8 ms with resident scalars)
+    // with scalars already in HBM one shot: the accumulation fills the SMs, so a next chunk's sort would barely overlap;
+    // with HOST scalars the chunks hide most of the 512 MiB upload at 2^24
+    // chunks of the host-scalar pipeline: few and geometrically growing (msm_run_pipelined)
     static int k_knob = -1;  // experiment knob B200ZK_E2E_CHUNKS: default chunk count of the host-scalar pipeline
     if (k_knob < 0) { const char* e = getenv("B200ZK_E2E_CHUNKS"); k_knob = (e && *e) ? atoi(e) : 0; if (k_knob < 0 || k_knob > 64) k_knob = 0; }
     uint32_t K = ctx->msm_chunks ? ctx->msm_chunks : ((h_scalars && n >= ((size_t)1 << 22)) ? (k_knob ? (uint32_t)k_knob : (IsFq2<F>::value ? 2u : 3u)) : 1u);
@@ -1522,9 +1519,8 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
   B2_TRY(ensure(ctx, ctx->ws_idx, n * (size_t)pl.W * 4));
   B2_TRY(ensure(ctx, ctx->ws_digits, n * (size_t)pl.W * 4));
   const size_t M_max = n * (size_t)pl.W;
-  // pair-summing rounds.  Measured on B200 (profiles/r1_pair_sum.md): a round costs ~180 ps per pair (it is
-  // bound by its ~330 B of scattered memory traffic per pair, not by its 6.7 products) against the ~158 ps XYZZ
-  // addition it removes, so the automatic setting is OFF; the path stays available (b200zk_set_msm_pair_rounds)
+  // pair-summing rounds.  A round is bound by its ~330 B of scattered memory traffic per pair, not by its 6.7
+  // products, and costs more than the XYZZ addition it removes, so the automatic setting is OFF; the path stays available (b200zk_set_msm_pair_rounds)
   // for parts with a different compute:bandwidth balance and is covered by the parity tests.
   uint32_t rounds = 0;
   if (ctx->msm_pair_rounds >= 0) rounds = (uint32_t)ctx->msm_pair_rounds;

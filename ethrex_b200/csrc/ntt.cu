@@ -1,4 +1,4 @@
-// ntt.cu -- number-theoretic transform over the BN254 scalar field Fr for sm_100a.
+// ntt.cu -- number-theoretic transform over the BN254 scalar field Fr for sm_90a.
 //
 // Replaces ark_poly::Radix2EvaluationDomain::{fft,ifft,coset_fft,coset_ifft}_in_place (ark-poly 0.5.0,
 // /root/reference/Cargo.lock:1140; equal to gnark-crypto bn254 fr/fft) as used by the Groth16 wrap behind
@@ -408,7 +408,7 @@ static Plan make_ntt_plan(uint32_t k) {
   }
   if (!p.P) {
     if (k <= (uint32_t)kMaxStage) { p.P = 1; p.s[0] = k; }
-    // measured on B200: 64 KiB tiles (several CTAs per SM) beat 128 KiB ones, so stages are capped at 10-11
+    // 64 KiB tiles keep several CTAs per SM to cover barrier and copy latency, so stages are capped at 10-11
     else if (k <= 20) { p.P = 2; p.s[0] = (k + 1) / 2; p.s[1] = k - p.s[0]; }
     else { p.P = 3; p.s[0] = (k + 2) / 3; p.s[1] = (k - p.s[0] + 1) / 2; p.s[2] = k - p.s[0] - p.s[1]; }
   }

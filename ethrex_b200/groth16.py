@@ -1,4 +1,4 @@
-"""Groth16-shaped commitment pipeline on the B200 kernels (SURVEY.md section 8f row 1, BASELINE config #5).
+"""Groth16-shaped commitment pipeline on the library's CUDA kernels (SURVEY.md section 8f row 1, BASELINE config #5).
 
 This is the arithmetic the SNARK wrap behind `ProofFormat::Groth16` performs
 (/root/reference/crates/prover/src/backend/sp1.rs:97-134 -> gnark; risc0.rs:24-29,71-82 -> risc0-groth16):
@@ -161,6 +161,11 @@ class ProvingKey:
 class SyntheticWrapCircuit:
     """Domain size 2^log_n; `n` witness entries; H has n-1 coefficients."""
     QUERIES = (("a_g1", False), ("b_g1", False), ("b_g2", True), ("l_g1", False), ("h_g1", False))
+    # device bytes per domain point a context may hold beside the proving key: the witness and the three evaluation
+    # vectors (128 B), the NTT scratch (32 B), the one-shot digit sort of a plain-bases MSM (16 B per entry x 15 windows
+    # = 240 B), the two sort slots of a host-scalar MSM (2 x 16 B x 12 entries = 384 B), G2 bucket runs (~200 B) and
+    # the workspaces' 1/8 growth slack
+    PROVE_WORKSPACE_PER_POINT = 1152
 
     def __init__(self, ctx, log_n: int, precompute: bool = True, g2: bool = True, rank: int = 0, world: int = 1):
         """rank/world: every rank keeps only its contiguous shard [lo, hi) of each proving-key column (point-split
@@ -172,6 +177,17 @@ class SyntheticWrapCircuit:
         self.lo, self.hi = shard_range(self.n, rank, world)
         self.pk = ProvingKey(log_n)
         m = self.hi - self.lo
+        # A window table holds ceil(255/c) multiples of every base (13x the bases at 2^24), and at domain 2^24 the five
+        # tables alone take 78 GiB: more than an 80 GB GPU holds beside the prove's workspaces.  Columns get their tables
+        # in QUERIES order while the key fits in the device's TOTAL memory less PROVE_WORKSPACE_PER_POINT * n bytes (a
+        # rule that depends on the device model only, not on what else runs on it); the others keep plain bases (same
+        # proof, slower MSMs).  H comes last in QUERIES and has scalars of its own, so it is the first to go and no
+        # shared digit sort is lost.  The table's size per plain byte is read off the first table built (an integer).
+        self.plain_columns = []
+        widths = [16 if is_g2 else 8 for _, is_g2 in self.QUERIES if g2 or not is_g2]
+        key_bytes = sum(8 * w for w in widths) * max(m, 1)  # every column as plain bases
+        budget = torch.cuda.mem_get_info()[1] - self.PROVE_WORKSPACE_PER_POINT * self.n
+        expand = None
         for name, is_g2 in self.QUERIES:
             if is_g2 and not g2:
                 continue
@@ -181,7 +197,18 @@ class SyntheticWrapCircuit:
             h = (ctx.g2_bases_from_device if is_g2 else ctx.g1_bases_from_device)(pts, m)
             del pts
             if precompute:
-                ctx.bases_precompute(h, 0)
+                plain = (128 if is_g2 else 64) * max(m, 1)
+                if expand is None:
+                    torch.cuda.empty_cache()
+                    free = torch.cuda.mem_get_info()[0]
+                    ctx.bases_precompute(h, 0)
+                    expand = round((free - torch.cuda.mem_get_info()[0]) / plain) + 1
+                    key_bytes += (expand - 1) * plain
+                elif key_bytes + (expand - 1) * plain <= budget:
+                    ctx.bases_precompute(h, 0)
+                    key_bytes += (expand - 1) * plain
+                else:
+                    self.plain_columns.append(name)
             self.pk.handles[name] = h
             self.pk.chains[name] = (k, d, is_g2)
         self.zinv = coset_vanishing_inverse(log_n)
@@ -261,9 +288,11 @@ class SyntheticWrapCircuit:
         run = msm or local
         names = [q for q in ("a_g1", "b_g1", "b_g2", "l_g1") if q in self.pk.handles]
         if msm is None and self.world == 1:
-            # the four witness MSMs share one scalar sort (b200zk_msm_multi_resident_device)
-            res = ctx.msm_multi_resident_device([self.pk.handles[q] for q in names], [self.pk.chains[q][2] for q in names], w, n, 0)
-            out = dict(zip(names, res))
+            # the witness MSMs over window tables share one scalar sort (b200zk_msm_multi_resident_device)
+            shared = [q for q in names if q not in self.plain_columns]
+            res = ctx.msm_multi_resident_device([self.pk.handles[q] for q in shared], [self.pk.chains[q][2] for q in shared], w, n, 0)
+            out = dict(zip(shared, res))
+            out.update({q: run(q, w, n, 0) for q in names if q in self.plain_columns})
         else:
             out = {q: run(q, w, n, 0) for q in names}
         out["h_g1"] = run("h_g1", h_coeffs, n - 1, F.SCALARS_MONT)

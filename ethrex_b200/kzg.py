@@ -1,4 +1,4 @@
-"""EIP-4844 blob commitments on the B200 kernels: the host-side mirror of the reference's `crypto::kzg` surface
+"""EIP-4844 blob commitments on the library's CUDA kernels: the host-side mirror of the reference's `crypto::kzg` surface
 (/root/reference/crates/common/crypto/kzg.rs:259-293, used by /root/reference/crates/common/types/blobs_bundle.rs:90-118
 and the L2 committer, crates/l2/sequencer/l1_committer.rs:1488-1521).
 

@@ -1,4 +1,4 @@
-/* b200zk.h -- frozen C ABI of libb200zk.so, the B200 (sm_100a) BN254 MSM + Fr NTT backend.
+/* b200zk.h -- frozen C ABI of libb200zk.so, the H100 (sm_90a) BN254 MSM + Fr NTT backend.
  *
  * This is the drop-in boundary for ethrex's L2 prover hot path (SURVEY.md section 8b): the entry points a
  * `crates/prover/src/backend/b200.rs` ProverBackend implementation binds through `unsafe extern "C"`

@@ -2,7 +2,7 @@
 //! G1/G2 multi-scalar multiplications and Fr NTTs of the Groth16 wrap that the reference reaches only inside
 //! third-party SDKs when the coordinator asks for `ProofFormat::Groth16`
 //! (`crates/l2/sequencer/proof_coordinator.rs:252-256`, `crates/prover/src/backend/sp1.rs:97-134`) -- runs on
-//! a B200 through `libb200zk.so`.
+//! an H100 through `libb200zk.so`.
 //!
 //! Scope (SURVEY.md section 8b): this backend does not introduce a new proof system.  It reports the
 //! `ProverType` of the zkVM whose on-chain Groth16 verifier it targets and replaces the *commitment

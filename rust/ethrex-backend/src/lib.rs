@@ -1,4 +1,4 @@
-//! B200 prover backend for ethrex: safe wrapper over `b200zk-sys` plus the `ProverBackend` implementation.
+//! H100 prover backend for ethrex: safe wrapper over `b200zk-sys` plus the `ProverBackend` implementation.
 pub mod b200;
 pub mod crypto;
 pub mod ffi;

@@ -289,6 +289,28 @@ def test_groth16_one_call_equals_separate_calls(ctx, log_n, precompute):
         circuit.close()
 
 
+def test_groth16_with_columns_left_on_plain_bases(ctx, monkeypatch):
+    """A key too large for window tables on every column (domain 2^24 on an 80 GB GPU) keeps some columns on plain
+    bases: the one-call prove over mixed plans and the separate calls still give the proof of an all-plain key."""
+    import torch
+    from ethrex_b200.groth16 import SyntheticWrapCircuit
+    log_n = 10
+    plain = SyntheticWrapCircuit(ctx, log_n, precompute=False)
+    try:
+        ref = plain.prove_device(b"batch-1")
+    finally:
+        plain.close()
+    # a workspace reserve no device can meet: only the first column gets its table
+    monkeypatch.setattr(SyntheticWrapCircuit, "PROVE_WORKSPACE_PER_POINT", torch.cuda.mem_get_info()[1] // (1 << log_n) + 1)
+    circuit = SyntheticWrapCircuit(ctx, log_n, precompute=True)
+    try:
+        assert circuit.plain_columns == ["b_g1", "b_g2", "l_g1", "h_g1"]
+        assert circuit.prove_device(b"batch-1") == ref
+        assert circuit.prove_separate(b"batch-1")[0] == ref[0]
+    finally:
+        circuit.close()
+
+
 def test_groth16_commit_rejects_inconsistent_keys(ctx):
     from ethrex_b200.groth16 import SyntheticWrapCircuit
     circuit = SyntheticWrapCircuit(ctx, 6, precompute=False)

@@ -1,7 +1,7 @@
 // Exploration probe (not the product): a 254-bit Montgomery product built on the FP64 pipe (DFMA) against the
 // shipped 8 x 32-bit IMAD.WIDE carry-chain product of csrc/field.cuh.  VERDICT r1 "next" item 3.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I ethrex_b200/csrc -Xcompiler -frounding-math \
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I ethrex_b200/csrc -Xcompiler -frounding-math \
 //        -o tools/build/dfma_mul_probe tools/dfma_mul_probe.cu
 //   tools/build/dfma_mul_probe cpu [count]   host run of the SAME code (fma() under FE_TOWARDZERO): prints
 //                                             "a b r" hex triples for the big-integer check in tools/dfma_check.py

@@ -1,6 +1,6 @@
 // Exploration probe (not the product): a carry-flag-free Montgomery product on 9 x 29-bit limbs against the
 // shipped 8 x 32-bit carry-chain product (csrc/field.cuh), and the raw issue rates behind the difference.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -I ethrex_b200/csrc -o tools/build/mul29_probe tools/mul29_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -I ethrex_b200/csrc -o tools/build/mul29_probe tools/mul29_probe.cu
 //   tools/build/mul29_probe cpu   -> prints test vectors (hex) for a big-integer check, no GPU needed
 //   tools/build/mul29_probe       -> throughput on the GPU
 #include <cstdint>

@@ -1,8 +1,8 @@
 """Digest of an `ncu --page source --csv` export (gzip) of one kernel: opcode mix by executed instructions and by warp-stall
 samples, the stall reasons summed over the kernel, and the SASS lines where warps wait longest.
     ncu --set full --import-source on --clock-control none -k regex:"^msm_accumulate$" -s 1 -c 1 -o acc python tools/profile_workload.py 22 g1
-    ncu -i acc.ncu-rep --page source --csv | gzip -9 > profiles/r2_ncu_source_accumulate.csv.gz
-    python tools/ncu_source_digest.py profiles/r2_ncu_source_accumulate.csv.gz "<workload>" "<reading>" > profiles/r2_ncu_source_accumulate.md"""
+    ncu -i acc.ncu-rep --page source --csv | gzip -9 > ncu_source_accumulate.csv.gz
+    python tools/ncu_source_digest.py ncu_source_accumulate.csv.gz "<workload>" "<reading>" > ncu_source_accumulate.md"""
 import collections
 import csv
 import gzip

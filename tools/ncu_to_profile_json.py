@@ -92,6 +92,7 @@ def main():
            "how": "ncu --set full --clock-control none python tools/profile_workload.py (2^24 G1 MSM, G2 MSM over window tables, forward NTT); durations in ms, "
                   "cold-cache and serialised: use shares and percentages, not absolutes",
            "kernels": kernels}
+    os.makedirs(os.path.dirname(os.path.abspath(dst)), exist_ok=True)
     with open(dst, "w") as f:
         json.dump(doc, f, indent=1)
     for k, v in kernels.items():

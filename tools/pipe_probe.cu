@@ -1,6 +1,6 @@
 // Pipe probe (exploration, not the product): do IMAD.WIDE (fmaheavy pipe) and DFMA (fp64 pipe) issue concurrently
-// on sm_100a, and at what rates?  Decides whether a double-precision limb product can run beside the integer one.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/build/pipe_probe tools/pipe_probe.cu && tools/build/pipe_probe
+// on sm_90a, and at what rates?  Decides whether a double-precision limb product can run beside the integer one.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/build/pipe_probe tools/pipe_probe.cu && tools/build/pipe_probe
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
-"""profiles/r2_sass_excerpt.md from the built libb200zk.so: per-kernel SASS mnemonic counts (cuobjdump -sass) and resource
-usage (cuobjdump -res-usage) -- the evidence that the shipped kernels are sm_100a code built from IMAD.WIDE carry chains and
-bulk-copy (TMA) staging, with no tensor-core or legacy paths.   python tools/sass_excerpt.py > profiles/r2_sass_excerpt.md"""
+"""A markdown excerpt (on stdout) of the built libb200zk.so: per-kernel SASS mnemonic counts (cuobjdump -sass) and resource
+usage (cuobjdump -res-usage) -- the evidence that the shipped kernels are sm_90a code built from IMAD.WIDE carry chains and
+bulk-copy (TMA) staging, with no tensor-core or legacy paths.   python tools/sass_excerpt.py > sass_excerpt.md"""
 import collections
 import os
 import re
