@@ -66,15 +66,15 @@ __global__ void __launch_bounds__(64) bls_g1_decode(const uint8_t* __restrict__ 
   store_affine<Fp381>(native, i, pt);
 }
 
-// first index of a big-endian 32-byte scalar that is not below the BLS12-381 group order
-__global__ void __launch_bounds__(256) bls_scalar_check(const uint8_t* __restrict__ scalars, size_t n, unsigned long long* bad) {
+// first index of a 32-byte scalar (big-endian, or little-endian limbs) that is not below the BLS12-381 group order
+__global__ void __launch_bounds__(256) bls_scalar_check(const uint8_t* __restrict__ scalars, size_t n, int big_endian, unsigned long long* bad) {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t* w = reinterpret_cast<const uint32_t*>(scalars + 32 * i);
   uint64_t br = 0;
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
-    const uint32_t limb = __byte_perm(__ldg(w + 7 - k), 0, 0x0123);
+    const uint32_t limb = big_endian ? __byte_perm(__ldg(w + 7 - k), 0, 0x0123) : __ldg(w + k);
     const uint64_t d = (uint64_t)limb - bls_r_limb(k) - br;
     br = (d >> 32) & 1u;
   }
@@ -96,7 +96,7 @@ int bls_points_to_native(b200zk_ctx* ctx, const void* d_in, void* d_native, size
   return B200ZK_OK;
 }
 
-int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars_be, size_t n, cudaStream_t st, size_t* bad_index) {
+int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big_endian, cudaStream_t st, size_t* bad_index) {
   *bad_index = n;
   if (!n) return B200ZK_OK;
   B2_TRY(ensure(ctx, ctx->ws_misc, 512));
@@ -104,7 +104,7 @@ int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars_be, size_t n, cudaS
   unsigned long long* h = (unsigned long long*)(ctx->h_pinned + 1024);
   h[0] = (unsigned long long)n;
   B2_CUDA(ctx, cudaMemcpyAsync(status, h, 8, cudaMemcpyHostToDevice, st));
-  B2_LAUNCH(ctx, bls_scalar_check, (unsigned)((n + 255) / 256), 256, 0, st, (const uint8_t*)d_scalars_be, n, status);
+  B2_LAUNCH(ctx, bls_scalar_check, (unsigned)((n + 255) / 256), 256, 0, st, (const uint8_t*)d_scalars, n, big_endian ? 1 : 0, status);
   B2_CUDA(ctx, cudaMemcpyAsync(h, status, 8, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   *bad_index = (size_t)h[0];
@@ -117,14 +117,13 @@ using namespace b200zk;
 
 namespace {
 int bls_msm_host_scalars(b200zk_ctx* ctx, const BasesEntry& e, const void* scalars, size_t n, uint32_t flags, cudaStream_t st, uint8_t out[48]) {
-  // scalars must be canonical field elements of the BLS12-381 scalar field (c-kzg bytes_to_bls_field rejects the rest)
+  // scalars must be canonical field elements of the BLS12-381 scalar field (c-kzg bytes_to_bls_field rejects the rest), in
+  // either byte order: the MSM does not reduce them, and a value >= 2^255 would overflow the signed-digit recoding's top window
   B2_TRY(ensure(ctx, ctx->ws_scalars, n * 32 + 32));
   if (n) B2_CUDA(ctx, cudaMemcpyAsync(ctx->ws_scalars.p, scalars, n * 32, cudaMemcpyHostToDevice, st));
-  if (flags & B200ZK_SCALARS_BE) {
-    size_t bad = n;
-    B2_TRY(bls_scalars_check(ctx, ctx->ws_scalars.p, n, st, &bad));
-    if (bad < n) return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, "bls12-381 scalar >= the group order");
-  }
+  size_t bad = n;
+  B2_TRY(bls_scalars_check(ctx, ctx->ws_scalars.p, n, (flags & B200ZK_SCALARS_BE) != 0, st, &bad));
+  if (bad < n) return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, "bls12-381 scalar >= the group order");
   B2_TRY(ensure(ctx, ctx->ws_result, 512));
   B2_TRY(ensure(ctx, ctx->ws_out, 512));
   B2_TRY(msm_run_bls(ctx, e.d, ctx->ws_scalars.p, n, flags & (B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW), st, ctx->ws_result.p, e.table_c, e.n));

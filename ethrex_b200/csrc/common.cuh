@@ -236,8 +236,8 @@ int msm_encode_bls(b200zk_ctx* ctx, const void* d_partials, size_t count, uint32
 // compressed (48 B, ZCash format) or uncompressed (96 B big-endian x | y) G1 points -> native affine; status[0] = first index with a coordinate >= p,
 // status[1] = first index not on the curve / with malformed flag bits (each n when none)
 int bls_points_to_native(b200zk_ctx* ctx, const void* d_in, void* d_native, size_t n, bool compressed, cudaStream_t st);
-// first index of a 32-byte big-endian scalar >= the BLS12-381 group order among n, or n
-int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars_be, size_t n, cudaStream_t st, size_t* bad_index);
+// first index of a 32-byte scalar (big-endian, or little-endian limbs) >= the BLS12-381 group order among n, or n
+int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big_endian, cudaStream_t st, size_t* bad_index);
 int msm_precompute_g1(b200zk_ctx* ctx, const void* d_bases, size_t n, uint32_t c, void* d_table, cudaStream_t st);
 int msm_precompute_g2(b200zk_ctx* ctx, const void* d_bases, size_t n, uint32_t c, void* d_table, cudaStream_t st);
 uint32_t precompute_window(size_t n);

@@ -56,7 +56,7 @@ uint32_t precompute_window(size_t n) {
 static MsmPlan make_plan(size_t n, uint32_t forced_c, uint32_t scalar_bits = 255) {
   uint32_t lg = 0;
   while (((size_t)1 << lg) < n) ++lg;
-  // c = 16 for 2^18..2^22 points, 17 from 2^23 up; below that lg-4.  At 2^24 on an H100 SXM at a 400 W power limit a G1
+  // c = 16 for 2^20..2^22 points, 17 from 2^23 up; below that lg-4.  At 2^24 on an H100 SXM at a 400 W power limit a G1
   // MSM over plain bases takes 54.8-54.9 / 52.4-52.8 / 54.9 ms at c = 16 / 17 / 18 (median step, two alternating runs)
   uint32_t c = forced_c ? forced_c : (lg > 8 ? lg - 4 : 4);
   if (!forced_c && c > 16) c = lg >= 23 ? 17 : 16;
@@ -91,7 +91,8 @@ B2_D void decode_scalar(uint4 lo, uint4 hi, uint32_t flags, uint32_t s[8]) {
 #pragma unroll
   for (int k = 0; k < 8; ++k) f.v[k] = s[k];
   if (flags & B200ZK_SCALARS_RAW) {
-    // another group's scalars (BLS12-381): no reduction; the caller guarantees < 2^255 (validated by bls_scalars_check)
+    // another group's scalars (BLS12-381): no reduction; the caller guarantees < r < 2^255 (bls_scalars_check, either byte
+    // order).  msm_run_g1 / msm_run_g2 refuse the flag: BN254 scalars are always reduced.
   } else if (flags & B200ZK_SCALARS_MONT) {
     // a Montgomery residue may be any value < 2^256 only if malformed; reduce first so mul's bound holds
 #pragma unroll 1
@@ -1675,8 +1676,16 @@ static int precompute_host(b200zk_ctx* ctx, const void* d_bases, size_t n, uint3
 int msm_precompute_g1(b200zk_ctx* ctx, const void* b, size_t n, uint32_t c, void* t, cudaStream_t st) { return precompute_host<Fq>(ctx, b, n, c, t, st); }
 int msm_precompute_g2(b200zk_ctx* ctx, const void* b, size_t n, uint32_t c, void* t, cudaStream_t st) { return precompute_host<Fq2>(ctx, b, n, c, t, st); }
 
-int msm_run_g1(b200zk_ctx* ctx, const void* p, const void* s, size_t n, uint32_t f, cudaStream_t st, void* out, uint32_t tc, size_t ts, const void* hs, int sort_mode) { return msm_run<Fq>(ctx, p, s, n, f, st, out, tc, ts, hs, sort_mode); }
-int msm_run_g2(b200zk_ctx* ctx, const void* p, const void* s, size_t n, uint32_t f, cudaStream_t st, void* out, uint32_t tc, size_t ts, const void* hs, int sort_mode) { return msm_run<Fq2>(ctx, p, s, n, f, st, out, tc, ts, hs, sort_mode); }
+// BN254 scalars are always reduced mod r: an unreduced 256-bit scalar (bit 254 or 255 set) would carry a top-window
+// coefficient above 2^(c-1), which the signed-digit recoding cannot represent (its bucket index falls outside the tables)
+int msm_run_g1(b200zk_ctx* ctx, const void* p, const void* s, size_t n, uint32_t f, cudaStream_t st, void* out, uint32_t tc, size_t ts, const void* hs, int sort_mode) {
+  if (f & B200ZK_SCALARS_RAW) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm: B200ZK_SCALARS_RAW is for BLS12-381 calls only");
+  return msm_run<Fq>(ctx, p, s, n, f, st, out, tc, ts, hs, sort_mode);
+}
+int msm_run_g2(b200zk_ctx* ctx, const void* p, const void* s, size_t n, uint32_t f, cudaStream_t st, void* out, uint32_t tc, size_t ts, const void* hs, int sort_mode) {
+  if (f & B200ZK_SCALARS_RAW) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm: B200ZK_SCALARS_RAW is for BLS12-381 calls only");
+  return msm_run<Fq2>(ctx, p, s, n, f, st, out, tc, ts, hs, sort_mode);
+}
 int msm_run_bls(b200zk_ctx* ctx, const void* p, const void* s, size_t n, uint32_t f, cudaStream_t st, void* out, uint32_t tc, size_t ts, const void* hs, int sort_mode) { return msm_run<Fp381>(ctx, p, s, n, f | B200ZK_SCALARS_RAW, st, out, tc, ts, hs, sort_mode); }
 int msm_precompute_bls(b200zk_ctx* ctx, const void* b, size_t n, uint32_t c, void* t, cudaStream_t st) { return precompute_host<Fp381>(ctx, b, n, c, t, st); }
 int msm_encode_bls(b200zk_ctx* ctx, const void* p, size_t c, uint32_t f, cudaStream_t st, void* out) { return msm_encode_host<Fp381>(ctx, p, c, f, st, out); }

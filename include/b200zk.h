@@ -81,7 +81,8 @@ enum {
   B200ZK_NTT_BE = 1u << 7,          /* NTT data are 32-byte big-endian canonical values */
   B200ZK_G16_INPUTS_DEVICE = 1u << 8, /* b200zk_groth16_commit*: witness and evaluation buffers are DEVICE pointers (used in place) */
   B200ZK_G16_H_COEFFS = 1u << 9,    /* b200zk_groth16_commit*: a_evals already holds the quotient's coefficients (Montgomery); skip the NTTs */
-  B200ZK_SCALARS_RAW = 1u << 10,    /* scalars are plain 256-bit integers < 2^255, NOT reduced mod the BN254 group order (BLS12-381 calls) */
+  B200ZK_SCALARS_RAW = 1u << 10,    /* internal to the BLS12-381 calls (scalars range-checked, not reduced); every BN254 MSM entry point
+                                       refuses it with B200ZK_ERR_INVALID_ARG */
   B200ZK_POINTS_COMPRESSED = 1u << 11 /* BLS12-381 G1 points in the 48-byte compressed ZCash / IETF format (the trusted setup's form) */
 };
 
@@ -273,7 +274,7 @@ int b200zk_groth16_fold(b200zk_ctx* ctx, const void* d_partials, size_t count, v
  * scalar out of its field, 3 = not a curve point / malformed flag bits.  The subgroup check is the trusted setup's
  * business (c-kzg validates it when loading), not repeated here.  The handle works with b200zk_bases_precompute /
  * b200zk_bases_free like any other.  Scalars: 32-byte integers < the BLS12-381 group order r, little-endian limbs or
- * big-endian with B200ZK_SCALARS_BE (then checked against r); result: 48 bytes compressed. */
+ * big-endian with B200ZK_SCALARS_BE; either order is checked against r (status 2 otherwise); result: 48 bytes compressed. */
 int b200zk_bls12_381_g1_bases_upload(b200zk_ctx* ctx, const void* points, size_t n, uint32_t flags, uint64_t* handle);
 int b200zk_bls12_381_g1_msm_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags,
                                      uint8_t out[48]);

@@ -132,6 +132,39 @@ def _jac_add_mixed(X1, Y1, Z1, x2, y2):
     return X3, (r * (V - X3) - Y1 * HHH) % P, Z1 * H % P
 
 
+def chain(n: int, k: int, d: int, block: int = 4096):
+    """Synthetic bases P_i = (k + i*d) * G, i < n, as n x 96 bytes uncompressed big-endian (identity: the 0x40 form) --
+    what bls12_381_g1_bases_upload(..., flags=0) takes.  Every base is a known multiple of G, so an MSM over them has the
+    closed form ((sum_i s_i (k + i d)) mod r) * G: one scalar multiplication, whatever n.  Built by Jacobian mixed
+    additions of D = d * G, normalised a block at a time with one inversion per block (Montgomery's trick)."""
+    k0, dd = generator_multiples([k, d])
+    out = bytearray()
+    X, Y, Z = (k0[0], k0[1], 1) if k0 is not None else (0, 1, 0)
+    for lo in range(0, n, block):
+        jac = []
+        for _ in range(min(block, n - lo)):
+            jac.append((X, Y, Z))
+            if dd is not None:
+                X, Y, Z = _jac_add_mixed(X, Y, Z, *dd)
+        prefix, acc = [], 1
+        for _, _, z in jac:
+            prefix.append(acc)
+            if z:
+                acc = acc * z % P
+        inv = pow(acc, -1, P)
+        aff = [None] * len(jac)
+        for j in range(len(jac) - 1, -1, -1):
+            x, y, z = jac[j]
+            if z:
+                zi = inv * prefix[j] % P
+                inv = inv * z % P
+                zi2 = zi * zi % P
+                aff[j] = (x * zi2 % P, y * zi2 * zi % P)
+        for p in aff:
+            out += uncompressed(p)
+    return bytes(out)
+
+
 def generator_multiples(scalars):
     """[s * G for s in scalars] (affine, None for the identity)"""
     tab = _pow2_table()

@@ -41,7 +41,7 @@ def test_bls12_381_g1_msm_matches_oracle(ctx, n, table):
         if table:
             ctx.bases_precompute(h, 0)
         assert ctx.bls12_381_g1_msm_resident(h, b"".join(v.to_bytes(32, "big") for v in s), n) == exp
-        # little-endian limbs (no range check on that path): same bytes
+        # little-endian limbs (range-checked like big-endian ones): same bytes
         le = b"".join(v.to_bytes(32, "little") for v in s)
         assert ctx.bls12_381_g1_msm_resident(h, le, n, 0) == exp
         # all-zero scalars: the identity, in its compressed form
@@ -125,14 +125,21 @@ def test_kzg_blob_commitment_and_proof_closed_form(ctx, synthetic_setup):
     try:
         rng = np.random.default_rng(4844)
         blobs = []
-        for b in range(3):
+        for b in range(6):
             vals = [int.from_bytes(rng.bytes(32), "big") % bls.R for _ in range(4096)]
             if b == 1:
                 vals = [0] * 4096  # the all-zero blob: the identity commitment
             if b == 2:
                 vals[5], vals[6], vals[7] = bls.R - 1, 0, 1
+            if b == 3:
+                vals = [bls.R - 1] * 4096  # every element at the top of the field: -(sum_i L_i(tau)) = -1
+            if b in (4, 5):
+                vals = [0] * 4096  # one non-zero element, at the first and at the last Lagrange point
+                vals[0 if b == 4 else 4095] = 0x1234567890ABCDEF1234567890ABCDEF1234567890ABCDEF1234567890ABCDEF % bls.R
             blobs.append(b"".join(v.to_bytes(32, "big") for v in vals))
-        commitments = settings.blobs_to_kzg_commitments(blobs)
+        commitments = settings.blobs_to_kzg_commitments(blobs)  # all six in one call
+        assert len(commitments) == 6
+        assert commitments[3] == bls.compress((bls.G1[0], bls.P - bls.G1[1]))  # sum_i L_i = 1, times r - 1
         for blob, c in zip(blobs, commitments):
             vals = [int.from_bytes(blob[32 * i:32 * i + 32], "big") for i in range(4096)]
             p_tau = sum(v * l for v, l in zip(vals, lag)) % bls.R

@@ -73,6 +73,42 @@ def test_mont_roundtrip_and_random(ctx):
     assert (to_host(d).reshape(n, 4) == host).all()
     ctx.fr_random_device(d, n, pyref.SEED_NTT, 77, eb.SCALARS_MONT)
     assert (to_host(d).reshape(n, 4) == orc.fr_to_mont(orc.rand_fr(pyref.SEED_NTT, 77, n))).all()
+    # Fq (which = 0): random values and the edges 0, 1, p - 1, p, 2^256 - 1 (to_mont reduces its input first)
+    rng = np.random.default_rng(0xF9)
+    vals = [int.from_bytes(rng.bytes(32), "little") % pyref.P for _ in range(n)]
+    edges = [0, 1, pyref.P - 1, pyref.P, pyref.P + 1, (1 << 256) - 1, (1 << 255), (1 << 254) - 1]
+    vals[:len(edges)] = edges
+    canon = orc.ints_to_array([v % pyref.P for v in vals])
+    d = to_dev(orc.ints_to_array(vals))
+    ctx.field_to_mont_device(d, n, 0)
+    mont = orc.fq_to_mont(canon)
+    assert (to_host(d).reshape(n, 4) == mont).all()
+    assert orc.array_to_ints(mont[:3]) == [0, (1 << 256) % pyref.P, (pyref.P - 1) * (1 << 256) % pyref.P]
+    ctx.field_from_mont_device(d, n, 0)
+    assert (to_host(d).reshape(n, 4) == canon).all()
+
+
+@pytest.mark.parametrize("n", [1, 255, 256, 257, 33 * 4096 + 1, 1 << 20])
+def test_fr_quotient_matches_oracle(ctx, n):
+    """fr_quotient_device, the pointwise step (a*b - c) * zinv of the Groth16 quotient, against the oracle: rows holding
+    0, 1 and r - 1 in every operand, zinv in {1, r - 1, random}, into a separate buffer and in place over a (how
+    ethrex_b200/groth16.py calls it)"""
+    a, b, c = (orc.rand_fr(0xF0 + j, 0, n) for j in range(3))
+    edges = [0, 1, pyref.R - 1]
+    for row in range(min(n, 9)):
+        a[row] = orc.int_to_limbs(edges[row % 3])
+        b[row] = orc.int_to_limbs(edges[(row // 3) % 3])
+        c[row] = orc.int_to_limbs(edges[(row + 1) % 3])
+    a, b, c = orc.fr_to_mont(a), orc.fr_to_mont(b), orc.fr_to_mont(c)
+    da, db, dc = to_dev(a), to_dev(b), to_dev(c)
+    for zinv in (1, pyref.R - 1, pyref.rand_fr(0xF3, n)):
+        exp = orc.fr_quotient(a, b, c, zinv)
+        out = dev_empty(4 * n)
+        ctx.fr_quotient_device(da, db, dc, out, n, zinv)
+        assert (to_host(out).reshape(n, 4) == exp).all(), zinv
+        inplace = da.clone()
+        ctx.fr_quotient_device(inplace, db, dc, inplace, n, zinv)
+        assert (to_host(inplace).reshape(n, 4) == exp).all(), zinv
 
 
 # ------------------------------------------------------------------------------------------ synthetic bases
@@ -219,10 +255,27 @@ def test_g1_msm_kats_from_reference(ctx):
     assert ctx.g1_msm_device(to_dev(g), to_dev(orc.ints_to_array([pyref.R])), 1) == bytes(64)
 
 
-def test_g1_msm_edge_distributions(ctx):
+def _group(g2):
+    """(chain, device MSM, oracle MSM, native -> BE) of G1 or G2"""
+    return ((orc.g2_chain, "g2_msm_device", orc.g2_msm, orc.g2_native_to_be) if g2 else
+            (orc.g1_chain, "g1_msm_device", orc.g1_msm, orc.g1_native_to_be))
+
+
+def _negate_native(pts_row, g2):
+    """-P of one native point: y -> p - y coordinate-wise (BE: G1 x|y, G2 x_im|x_re|y_im|y_re)"""
+    size = 128 if g2 else 64
+    raw = bytearray((orc.g2_native_to_be if g2 else orc.g1_native_to_be)(np.ascontiguousarray(pts_row)))
+    for off in ((64, 96) if g2 else (32,)):
+        raw[off:off + 32] = ((pyref.P - int.from_bytes(raw[off:off + 32], "big")) % pyref.P).to_bytes(32, "big")
+    return (orc.g2_be_to_native if g2 else orc.g1_be_to_native)(bytes(raw[:size]))[0]
+
+
+def _msm_edge_distributions(ctx, g2):
+    chain, dev_msm, oracle_msm, _ = _group(g2)
+    msm = getattr(ctx, dev_msm)
     k, d = chain_kd()
     n = 2048
-    pts = orc.g1_chain(n, k, d)
+    pts = chain(n, k, d)
     dp = to_dev(pts)
     cases = {
         "all_zero": [0] * n,
@@ -235,46 +288,72 @@ def test_g1_msm_edge_distributions(ctx):
     }
     for name, vals in cases.items():
         s = orc.ints_to_array(vals)
-        assert ctx.g1_msm_device(dp, to_dev(s), n) == orc.g1_msm(pts, s), name
+        assert msm(dp, to_dev(s), n) == oracle_msm(pts, s), name
     # repeated points, P and -P pairs, identity points among the bases
     pts2 = pts.copy()
     pts2[1] = pts2[0]
     pts2[3] = pts2[2]
-    neg = orc.g1_be_to_native(pyref.g1_to_be(pyref.pt_neg(pyref._Fq, pyref.g1_from_be(orc.g1_native_to_be(pts[4:5])))))
-    pts2[5] = neg[0]
+    pts2[5] = _negate_native(pts[4:5], g2)
     pts2[7] = 0
     s = orc.rand_fr(11, 0, n)
     s[1] = s[0]
     s[5] = s[4]
     s[3] = orc.int_to_limbs((pyref.R - orc.limbs_to_int(s[2])) % pyref.R)
-    assert ctx.g1_msm_device(to_dev(pts2), to_dev(s), n) == orc.g1_msm(pts2, s)
+    assert msm(to_dev(pts2), to_dev(s), n) == oracle_msm(pts2, s)
 
 
-def test_g1_msm_window_sweep(ctx):
+def test_g1_msm_edge_distributions(ctx):
+    _msm_edge_distributions(ctx, g2=False)
+
+
+def test_g2_msm_edge_distributions(ctx):
+    _msm_edge_distributions(ctx, g2=True)
+
+
+def _msm_window_sweep(ctx, g2):
+    chain, dev_msm, oracle_msm, _ = _group(g2)
     k, d = chain_kd()
     n = 3000
-    pts, s = orc.g1_chain(n, k, d), scalars_special(n)
-    exp = orc.g1_msm(pts, s)
+    pts, s = chain(n, k, d), scalars_special(n)
+    exp = oracle_msm(pts, s)
     dp, ds = to_dev(pts), to_dev(s)
     try:
         for c in (2, 3, 5, 8, 11, 13, 16):
             ctx.set_msm_window(c)
-            assert ctx.g1_msm_device(dp, ds, n) == exp, f"c={c}"
+            assert getattr(ctx, dev_msm)(dp, ds, n) == exp, f"c={c}"
     finally:
         ctx.set_msm_window(0)
 
 
-def test_g1_msm_scalar_formats(ctx):
+def test_g1_msm_window_sweep(ctx):
+    _msm_window_sweep(ctx, g2=False)
+
+
+def test_g2_msm_window_sweep(ctx):
+    _msm_window_sweep(ctx, g2=True)
+
+
+def _msm_scalar_formats(ctx, g2):
+    chain, dev_msm, oracle_msm, native_to_be = _group(g2)
+    msm = getattr(ctx, dev_msm)
     k, d = chain_kd()
     n = 777
-    pts, s = orc.g1_chain(n, k, d), scalars_special(n)
-    exp = orc.g1_msm(pts, s)
+    pts, s = chain(n, k, d), scalars_special(n)
+    exp = oracle_msm(pts, s)
     dp = to_dev(pts)
-    assert ctx.g1_msm_device(dp, to_dev(orc.fr_to_mont(s)), n, eb.SCALARS_MONT) == exp
+    assert msm(dp, to_dev(orc.fr_to_mont(s)), n, eb.SCALARS_MONT) == exp
     be = b"".join(pyref.fr_to_be(v) for v in orc.array_to_ints(s))
-    assert ctx.g1_msm_device(dp, to_dev(np.frombuffer(be, dtype=np.uint64)), n, eb.SCALARS_BE) == exp
-    native = ctx.g1_msm_device(dp, to_dev(s), n, eb.OUT_NATIVE)
-    assert orc.g1_native_to_be(np.frombuffer(native, dtype=np.uint64)) == exp
+    assert msm(dp, to_dev(np.frombuffer(be, dtype=np.uint64)), n, eb.SCALARS_BE) == exp
+    native = msm(dp, to_dev(s), n, eb.OUT_NATIVE)
+    assert native_to_be(np.frombuffer(native, dtype=np.uint64)) == exp
+
+
+def test_g1_msm_scalar_formats(ctx):
+    _msm_scalar_formats(ctx, g2=False)
+
+
+def test_g2_msm_scalar_formats(ctx):
+    _msm_scalar_formats(ctx, g2=True)
 
 
 @pytest.mark.parametrize("log_n", [16, 20])

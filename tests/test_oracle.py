@@ -285,3 +285,32 @@ def test_bls12_381_oracle_constants():
     import hashlib
     want = int.from_bytes(hashlib.sha256(b"FSBLOBVERIFY_V1_" + (4096).to_bytes(16, "big") + blob + c).digest(), "big") % b.R
     assert kzg.KzgSettings.compute_challenge(blob, c) == want
+
+
+def _bls_chain_points(raw: bytes):
+    import bls_ref as b
+    pts = []
+    for i in range(len(raw) // 96):
+        x, y = int.from_bytes(raw[96 * i:96 * i + 48], "big"), int.from_bytes(raw[96 * i + 48:96 * i + 96], "big")
+        pts.append(None if raw[96 * i] == 0x40 else (x, y))
+    return pts
+
+
+def test_bls12_381_chain_is_the_generator_multiples():
+    """bls_ref.chain -- the synthetic BLS12-381 bases whose MSM has a closed form -- against generator_multiples: sampled
+    indices across block boundaries, every point on the curve, and chains that pass through the identity and through a
+    doubling (k = 0: P_1 = D, then P_1 + D = 2D)."""
+    import bls_ref as b
+    k, d = 0x1234567890ABCDEF1234567890ABCDEF % b.R, 0xFEDCBA0987654321FEDCBA0987654321 % b.R
+    n = 5000
+    raw = b.chain(n, k, d)
+    assert len(raw) == 96 * n
+    pts = _bls_chain_points(raw)
+    assert all(b.on_curve(p) and p is not None for p in pts)
+    idx = [0, 1, 2, 4095, 4096, 4097, n - 1]
+    assert [pts[i] for i in idx] == b.generator_multiples([k + i * d for i in idx])
+    # small blocks: every block boundary; k + 3d = 0 puts the identity at index 3; k = 0 starts at the identity
+    for kk, dd in (((b.R - 3 * d) % b.R, d), (0, d), (k, 0)):
+        pts = _bls_chain_points(b.chain(9, kk, dd, block=4))
+        assert pts == b.generator_multiples([kk + i * dd for i in range(9)]), (kk, dd)
+    assert _bls_chain_points(b.chain(9, (b.R - 3 * d) % b.R, d))[3] is None
