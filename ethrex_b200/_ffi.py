@@ -37,6 +37,12 @@ class Groth16Pk(C.Structure):
     _fields_ = [("log_n", C.c_uint32), ("reserved", C.c_uint32), ("handle", C.c_uint64 * 5), ("count", C.c_uint64 * 5), ("offset", C.c_uint64 * 5)]
 
 
+class Groth16Zk(C.Structure):
+    """struct b200zk_groth16_zk (include/b200zk.h): key-term handles (G1 alpha, beta, delta; G2 beta, delta) and the
+    blinding scalars r, s as canonical little-endian bytes below the group order"""
+    _fields_ = [("g1_terms", C.c_uint64), ("g2_terms", C.c_uint64), ("r", C.c_uint8 * 32), ("s", C.c_uint8 * 32)]
+
+
 # name -> (restype, argtypes); every symbol include/b200zk.h declares
 SIGNATURES = {
     "b200zk_abi_version": (_int, []),
@@ -70,6 +76,8 @@ SIGNATURES = {
     "b200zk_groth16_commit": (_int, [_ctx, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp]),
     "b200zk_groth16_commit_partial": (_int, [_ctx, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp]),
     "b200zk_groth16_fold": (_int, [_ctx, _vp, _sz, _vp, _vp, _vp]),
+    "b200zk_groth16_prove": (_int, [_ctx, _vp, _vp, _vp, _vp, _vp, _vp, _u32, _vp, _vp]),
+    "b200zk_groth16_fold_zk": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_g1_msm_partial_device": (_int, [_ctx, _vp, _vp, _sz, _u32, _vp, _vp]),
     "b200zk_g2_msm_partial_device": (_int, [_ctx, _vp, _vp, _sz, _u32, _vp, _vp]),
     "b200zk_g1_msm_partial_resident_device": (_int, [_ctx, _u64, _vp, _sz, _u32, _vp, _vp]),

@@ -386,6 +386,36 @@ class Context:
         self._check(F.lib.b200zk_groth16_fold(self._h, _dev_ptr(d_partials), count, _current_stream_ptr(self.device), proof, b1), "b200zk_groth16_fold")
         return proof.raw, b1.raw
 
+    @staticmethod
+    def groth16_zk(g1_terms: int, g2_terms: int, r: int, s: int) -> "F.Groth16Zk":
+        """g1_terms: handle of alpha1, beta1, delta1; g2_terms: handle of beta2, delta2 (plain resident bases);
+        r, s: blinding scalars, integers in [0, group order) -- the library refuses larger values, it does not reduce them"""
+        if not (0 <= r < 1 << 256 and 0 <= s < 1 << 256):
+            raise B200Error.serialization("groth16_zk: r and s must be 256-bit non-negative integers")
+        zk = F.Groth16Zk()
+        zk.g1_terms, zk.g2_terms = g1_terms, g2_terms
+        zk.r[:] = list(int(r).to_bytes(32, "little"))
+        zk.s[:] = list(int(s).to_bytes(32, "little"))
+        return zk
+
+    def groth16_prove(self, pk, zk, witness, a_evals, b_evals, c_evals, flags: int = 0) -> bytes:
+        """-> the blinded proof A | B2 | C (256 bytes) over a key with separate alpha / beta / delta terms (`zk`, from
+        groth16_zk).  Host buffers, or device tensors with G16_INPUTS_DEVICE, as groth16_commit."""
+        wp, ap, bp, cp, keep = self._g16_ptrs(pk, witness, a_evals, b_evals, c_evals, flags)
+        proof = C.create_string_buffer(256)
+        self._check(F.lib.b200zk_groth16_prove(self._h, C.byref(pk), C.byref(zk) if zk is not None else None, wp, ap, bp, cp, flags,
+                                               _current_stream_ptr(self.device), proof), "b200zk_groth16_prove")
+        return proof.raw
+
+    def groth16_fold_zk(self, zk, d_partials, count: int) -> bytes:
+        """folds `count` 768-byte blocks of groth16_commit_partial, then adds the key terms and the blinding once"""
+        if d_partials.numel() * d_partials.element_size() < 768 * count:
+            raise B200Error.serialization("groth16_fold_zk: d_partials must hold 768 bytes per block")
+        proof = C.create_string_buffer(256)
+        self._check(F.lib.b200zk_groth16_fold_zk(self._h, C.byref(zk) if zk is not None else None, _dev_ptr(d_partials), count,
+                                                 _current_stream_ptr(self.device), proof), "b200zk_groth16_fold_zk")
+        return proof.raw
+
     def g1_msm_partial_device(self, d_points, d_scalars, n: int, d_partial, flags: int = 0):
         self._check(F.lib.b200zk_g1_msm_partial_device(self._h, _dev_ptr(d_points), _dev_ptr(d_scalars), n, flags, _current_stream_ptr(self.device), _dev_ptr(d_partial)), "b200zk_g1_msm_partial_device")
 

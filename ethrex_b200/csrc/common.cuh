@@ -254,6 +254,10 @@ int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const 
                             uint32_t flags, cudaStream_t st, void* d_partials);
 // d_partials: count blocks of 768 B (A | B1 | B2 | L | H as XYZZ); d_out: proof A|B2|C (256 B) | B1 (64 B) | 4 x u32 is_infinity (A, B2, C, B1)
 int groth16_assemble_dev(b200zk_ctx* ctx, const void* d_partials, size_t count, cudaStream_t st, void* d_out);
+// same blocks with the key terms (g1: alpha, beta, delta; g2: beta, delta; native affine) and the blinding scalars r, s
+// (canonical LE, < the group order); d_out: proof A|B2|C (256 B) | 3 x u32 is_infinity (A, B2, C)
+int groth16_assemble_zk_dev(b200zk_ctx* ctx, const void* d_partials, size_t count, const void* d_g1_terms, const void* d_g2_terms,
+                            const uint8_t r_le[32], const uint8_t s_le[32], cudaStream_t st, void* d_out);
 int bn254_g1_add_batch(b200zk_ctx* ctx, const uint8_t* a, const uint8_t* b, size_t count, uint8_t* out, uint8_t* status);
 int bn254_g1_mul_batch(b200zk_ctx* ctx, const uint8_t* points, const uint8_t* scalars, size_t count, uint8_t* out, uint8_t* status);
 int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint32_t* pair_offsets, size_t count, uint8_t* result, uint8_t* status);

@@ -6,6 +6,8 @@
 //   quotient   3 iNTT (A.z, B.z, C.z on the domain -> coefficients), 3 coset NTT, (a*b - c)/Z_H pointwise, 1 coset iNTT
 //   commit     [A]1 = <pk.A_g1, z>   [B]1 = <pk.B_g1, z>   [B]2 = <pk.B_g2, z>   [L]1 = <pk.L_g1, z_private>   [H]1 = <pk.H_g1, h>
 //   assemble   proof = A | B2 | C,  C = [L]1 + [H]1         (EIP-196/197 bytes, 256 B; no blinding: r = s = 0)
+//   or, b200zk_groth16_prove / _fold_zk: the ark-groth16 / gnark proof with the key's alpha / beta / delta terms and the
+//              caller's blinding scalars r, s (groth16_assemble_zk in msm.cu)
 //
 // Everything is enqueued on one stream with no host round trip in between; columns that multiply the same scalar
 // slice share ONE digit sort (msm_run sort_mode 1/2), and the five results stay on the device as XYZZ partial sums
@@ -94,6 +96,40 @@ int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const 
   return B200ZK_OK;
 }
 
+// x (32 bytes little-endian) < the group order r: blinding scalars are refused, not reduced, so that raw random bytes
+// cannot skew their distribution
+static bool fr_canonical(const uint8_t* x) {
+  for (int i = 7; i >= 0; --i) {
+    const uint32_t w = (uint32_t)x[4 * i] | (uint32_t)x[4 * i + 1] << 8 | (uint32_t)x[4 * i + 2] << 16 | (uint32_t)x[4 * i + 3] << 24;
+    if (w != FrCfg::mod(i)) return w < FrCfg::mod(i);
+  }
+  return false;
+}
+
+// the key terms of a b200zk_groth16_zk: plain (not precomputed) BN254 bases of the right group and point count
+static int zk_terms(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void** g1, const void** g2) {
+  if (!zk) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: null argument");
+  auto it1 = ctx->bases.find(zk->g1_terms), it2 = ctx->bases.find(zk->g2_terms);
+  if (it1 == ctx->bases.end() || it1->second.bls || it1->second.g2 || it1->second.table_c || it1->second.n != 3)
+    return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: g1_terms must be a plain G1 handle of 3 points (alpha, beta, delta)");
+  if (it2 == ctx->bases.end() || it2->second.bls || !it2->second.g2 || it2->second.table_c || it2->second.n != 2)
+    return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: g2_terms must be a plain G2 handle of 2 points (beta, delta)");
+  if (!fr_canonical(zk->r) || !fr_canonical(zk->s)) return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, "groth16 zk: r or s is not below the group order");
+  *g1 = it1->second.d;
+  *g2 = it2->second.d;
+  return B200ZK_OK;
+}
+
+static int fold_zk(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void* g1, const void* g2, const void* d_partials, size_t count,
+                   cudaStream_t st, uint8_t proof[256]) {
+  B2_TRY(ensure(ctx, ctx->ws_out, 512));
+  B2_TRY(groth16_assemble_zk_dev(ctx, d_partials, count, g1, g2, zk->r, zk->s, st, ctx->ws_out.p));
+  B2_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, ctx->ws_out.p, 256, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  memcpy(proof, ctx->h_pinned, 256);
+  return B200ZK_OK;
+}
+
 }  // namespace b200zk
 
 using namespace b200zk;
@@ -128,6 +164,30 @@ int b200zk_groth16_commit(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const vo
   B2_TRY(ensure(ctx, ctx->ws_g16[3], 1024));
   B2_TRY(groth16_commit_partials(ctx, pk, witness, a_evals, b_evals, c_evals, flags, st, ctx->ws_g16[3].p));
   return b200zk_groth16_fold(ctx, ctx->ws_g16[3].p, 1, (void*)st, proof, b_g1);
+}
+
+int b200zk_groth16_fold_zk(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void* d_partials, size_t count, void* stream, uint8_t proof[256]) {
+  if (!ctx || !proof || (!d_partials && count)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_fold_zk: null argument");
+  DeviceGuard guard(ctx);
+  const void *g1 = nullptr, *g2 = nullptr;
+  B2_TRY(zk_terms(ctx, zk, &g1, &g2));
+  return fold_zk(ctx, zk, g1, g2, d_partials, count, pick_stream(ctx, stream), proof);
+}
+
+int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const b200zk_groth16_zk* zk, const void* witness, void* a_evals, void* b_evals,
+                         void* c_evals, uint32_t flags, void* stream, uint8_t proof[256]) {
+  if (!ctx || !proof || !pk) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_prove: null argument");
+  DeviceGuard guard(ctx);
+  const void *g1 = nullptr, *g2 = nullptr;
+  B2_TRY(zk_terms(ctx, zk, &g1, &g2));
+  bool r_zero = true;
+  for (int i = 0; i < 32; ++i) r_zero = r_zero && !zk->r[i];
+  // C = ... + r [B]1: only r = 0 may skip the B_g1 column (what ark-groth16 does)
+  if (!pk->handle[1] && !r_zero) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_prove: r != 0 needs the B_g1 column");
+  cudaStream_t st = pick_stream(ctx, stream);
+  B2_TRY(ensure(ctx, ctx->ws_g16[3], 1024));
+  B2_TRY(groth16_commit_partials(ctx, pk, witness, a_evals, b_evals, c_evals, flags, st, ctx->ws_g16[3].p));
+  return fold_zk(ctx, zk, g1, g2, ctx->ws_g16[3].p, 1, st, proof);
 }
 
 }  // extern "C"

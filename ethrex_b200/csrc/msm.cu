@@ -1248,6 +1248,139 @@ int groth16_assemble_dev(b200zk_ctx* ctx, const void* d_partials, size_t count, 
   return B200ZK_OK;
 }
 
+// ---- zero-knowledge Groth16 assembly (b200zk_groth16_fold_zk): the proof of ark-groth16 0.5 / gnark groth16.Prove for the
+// blinding scalars r, s, with the key terms alpha1, beta1, delta1 (g1_terms) and beta2, delta2 (g2_terms) as native affine:
+//   A  = alpha1 + [A] + r delta1        B2 = beta2 + [B2] + s delta2        B1 = beta1 + [B1] + s delta1
+//   C  = [L] + [H] + s A + r B1 - (rs) delta1
+// C is evaluated as [L] + [H] + s (alpha1 + [A]) + r (beta1 + [B1]) + (rs) delta1: the same group element (the r s delta1
+// inside s A and inside r B1 cancel against one - rs delta1), but it needs neither A nor B1 first, so the three CTAs
+// are independent: 0 -> A (r delta1), 1 -> B2 (s delta2), 2 -> C (one Straus pass over three scalars, 256 shared
+// doublings instead of three double-and-add chains).  rs mod r comes from the Fr Montgomery product.  Each CTA ends
+// with one Fermat inversion.  out: A (64) | B2 (128) | C (64) | 3 x u32 is_infinity (A, B2, C).
+struct G16Blinding {
+  uint32_t r[8], s[8];  // canonical little-endian limbs, < the group order
+};
+B2_D uint32_t scalar_bit(const uint32_t* k, int i) { return (k[i >> 5] >> (i & 31)) & 1u; }
+// k * pts[idx] (double-and-add, MSB first) that re-reads the point from memory at every addition instead of keeping
+// it live across the loop: those 32 registers are what the Fq2 formulas need to stay clear of local memory
+template <class F> B2_D XYZZ<F> scalar_mul_reload(const uint32_t* k, const void* pts, size_t idx) {
+  XYZZ<F> acc = XYZZ<F>::identity();
+  for (int i = 255; i >= 0; --i) {
+    acc = xyzz_dbl(acc);
+    if (scalar_bit(k, i)) {
+      asm volatile("" ::: "memory");
+      const Affine<F> p = load_affine_nc<F>(pts, idx);
+      xyzz_add_mixed(acc, p.x, p.y);
+    }
+  }
+  return acc;
+}
+// acc += *q (add-2008-s, exceptional cases as xyzz_add) for a q parked in shared memory: its coordinates are re-read
+// where they are needed instead of being held across the formula, which keeps a G2 addition inside 255 registers
+template <class F> B2_D void xyzz_add_parked(XYZZ<F>& acc, const XYZZ<F>* q) {
+  if (q->is_inf()) return;
+  if (acc.is_inf()) { acc = *q; return; }
+  const F U1 = F::mul(acc.x, q->zz), S1 = F::mul(acc.y, q->zzz);
+  asm volatile("" ::: "memory");
+  const F P = F::sub(F::mul(q->x, acc.zz), U1), R = F::sub(F::mul(q->y, acc.zzz), S1);
+  if (P.is_zero()) {
+    if (R.is_zero()) acc = xyzz_dbl(acc);
+    else acc = XYZZ<F>::identity();
+    return;
+  }
+  const F PP = F::sqr(P), PPP = F::mul(P, PP), Q = F::mul(U1, PP);
+  const F x3 = F::sub(F::sub(F::sqr(R), PPP), F::dbl(Q));
+  acc.y = F::mul2_sub(R, F::sub(Q, x3), S1, PPP);
+  acc.x = x3;
+  asm volatile("" ::: "memory");
+  acc.zz = F::mul(F::mul(acc.zz, q->zz), PP);
+  acc.zzz = F::mul(F::mul(acc.zzz, q->zzz), PPP);
+}
+
+// The scalars sit in shared memory (bit lookups with a run-time index stay out of local memory), and every CTA runs its
+// scalar multiplication BEFORE folding the partial sums into it, so that no second accumulator is live across the
+// 256-step loop.  With scalar_mul_reload and xyzz_add_parked this keeps the G2 branch within 255 registers, no spills.
+__global__ void groth16_assemble_zk(const uint8_t* __restrict__ partials, size_t count, const void* __restrict__ g1_terms,
+                                    const void* __restrict__ g2_terms, G16Blinding zk, uint8_t* __restrict__ out) {
+  __shared__ XYZZ<Fq> table[7];  // Straus table: table[b - 1] = bit0(b) A' + bit1(b) B1' + bit2(b) delta1
+  __shared__ uint32_t sc[3][8];  // s, r, rs
+  if (threadIdx.x) return;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { sc[0][i] = zk.s[i]; sc[1][i] = zk.r[i]; }
+  uint32_t* inf = reinterpret_cast<uint32_t*>(out + 256);
+  if (blockIdx.x == 1) {  // B2 = s delta2 + beta2 + [B2]
+    XYZZ<Fq2> acc = scalar_mul_reload<Fq2>(sc[0], g2_terms, 1);
+    const Affine<Fq2> beta = load_affine_nc<Fq2>(g2_terms, 0);
+    xyzz_add_mixed(acc, beta.x, beta.y);
+    XYZZ<Fq2>* parked = reinterpret_cast<XYZZ<Fq2>*>(table);  // this CTA does not use the Straus table
+    for (size_t k = 0; k < count; ++k) {
+      *parked = load_xyzz<Fq2>(partials + k * 768 + 256, 0);
+      asm volatile("" ::: "memory");
+      xyzz_add_parked(acc, parked);
+    }
+    Affine<Fq2> a = xyzz_to_affine(acc);
+    encode_point(out + 64, a, false);
+    inf[1] = a.is_inf() ? 1u : 0u;
+    return;
+  }
+  const Affine<Fq> alpha = load_affine_nc<Fq>(g1_terms, 0), delta = load_affine_nc<Fq>(g1_terms, 2);
+  if (blockIdx.x == 0) {  // A = r delta1 + alpha1 + [A]
+    XYZZ<Fq> a = xyzz_scalar_mul<Fq>(sc[1], delta);
+    xyzz_add_mixed(a, alpha.x, alpha.y);
+    for (size_t k = 0; k < count; ++k) { XYZZ<Fq> p = load_xyzz<Fq>(partials + k * 768, 0); xyzz_add(a, p); }
+    Affine<Fq> aa = xyzz_to_affine(a);
+    encode_point(out, aa, false);
+    inf[0] = aa.is_inf() ? 1u : 0u;
+    return;
+  }
+  // C = s A' + r B1' + (rs) delta1 + [L] + [H],  A' = alpha1 + [A],  B1' = beta1 + [B1]
+  {
+    const Affine<Fq> beta = load_affine_nc<Fq>(g1_terms, 1);
+    XYZZ<Fq> a = XYZZ<Fq>::identity(), b = XYZZ<Fq>::identity();
+    for (size_t k = 0; k < count; ++k) {
+      XYZZ<Fq> p = load_xyzz<Fq>(partials + k * 768, 0); xyzz_add(a, p);
+      XYZZ<Fq> q = load_xyzz<Fq>(partials + k * 768 + 128, 0); xyzz_add(b, q);
+    }
+    xyzz_add_mixed(a, alpha.x, alpha.y);
+    xyzz_add_mixed(b, beta.x, beta.y);
+    table[0] = a; table[1] = b;
+    xyzz_add(a, b); table[2] = a;
+  }
+  table[3] = xyzz_from_affine(delta);
+  for (int t = 4; t < 7; ++t) { XYZZ<Fq> e = table[t - 4]; xyzz_add_mixed(e, delta.x, delta.y); table[t] = e; }
+  {
+    Fr r, s;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { r.v[i] = zk.r[i]; s.v[i] = zk.s[i]; }
+    const Fr rs = Fr::mul(Fr::to_mont(r), s);  // (r R) s / R = r s mod the group order, canonical
+#pragma unroll
+    for (int i = 0; i < 8; ++i) sc[2][i] = rs.v[i];
+  }
+  XYZZ<Fq> c = XYZZ<Fq>::identity();
+  for (int i = 255; i >= 0; --i) {
+    c = xyzz_dbl(c);
+    const uint32_t sel = scalar_bit(sc[0], i) | (scalar_bit(sc[1], i) << 1) | (scalar_bit(sc[2], i) << 2);
+    if (sel) { XYZZ<Fq> t = table[sel - 1]; xyzz_add(c, t); }
+  }
+  for (size_t k = 0; k < count; ++k) {
+    XYZZ<Fq> l = load_xyzz<Fq>(partials + k * 768 + 512, 0); xyzz_add(c, l);
+    XYZZ<Fq> h = load_xyzz<Fq>(partials + k * 768 + 640, 0); xyzz_add(c, h);
+  }
+  Affine<Fq> cc = xyzz_to_affine(c);
+  encode_point(out + 192, cc, false);
+  inf[2] = cc.is_inf() ? 1u : 0u;
+}
+int groth16_assemble_zk_dev(b200zk_ctx* ctx, const void* d_partials, size_t count, const void* d_g1_terms, const void* d_g2_terms,
+                            const uint8_t r_le[32], const uint8_t s_le[32], cudaStream_t st, void* d_out) {
+  G16Blinding zk;
+  for (int i = 0; i < 8; ++i) {
+    zk.r[i] = (uint32_t)r_le[4 * i] | (uint32_t)r_le[4 * i + 1] << 8 | (uint32_t)r_le[4 * i + 2] << 16 | (uint32_t)r_le[4 * i + 3] << 24;
+    zk.s[i] = (uint32_t)s_le[4 * i] | (uint32_t)s_le[4 * i + 1] << 8 | (uint32_t)s_le[4 * i + 2] << 16 | (uint32_t)s_le[4 * i + 3] << 24;
+  }
+  B2_LAUNCH(ctx, groth16_assemble_zk, 3, 32, 0, st, (const uint8_t*)d_partials, count, d_g1_terms, d_g2_terms, zk, (uint8_t*)d_out);
+  return B200ZK_OK;
+}
+
 // ---- host orchestration ---------------------------------------------------------------------------------------
 static inline void phase_mark(b200zk_ctx* ctx, int k, cudaStream_t st) {
   if (ctx->profiling) cudaEventRecord(ctx->ev[k], st);

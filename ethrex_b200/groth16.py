@@ -7,17 +7,22 @@ This is the arithmetic the SNARK wrap behind `ProofFormat::Groth16` performs
     commit     [A]1 = MSM(pk.A_g1, w)   [B]1 = MSM(pk.B_g1, w)   [B]2 = MSM(pk.B_g2, w)
                [L]1 = MSM(pk.L_g1, w_private)   [H]1 = MSM(pk.H_g1, h)
     assemble   proof = A | B | C with C = [L]1 + [H]1      (EIP-197 byte order, 256 bytes)
+    blinded    A += alpha1 + r delta1, B += beta2 + s delta2, C += s A + r B1 - rs delta1   (b200zk_groth16_prove)
 
 The reference's real wrap circuit and proving key live inside the zkVM SDKs and are not in the tree, so the
 circuit here is SYNTHETIC (SURVEY.md section 8d, config 5): witness and constraint evaluations are derived
 deterministically from the serialized program input, with C = A o B on the domain so that the quotient is an
-exact polynomial, and the proving key is a set of chain bases.  The STARK stage is excluded and no blinding
-is applied; what is measured and parity-checked is exactly the MSM + NTT work of a Groth16 prove.
+exact polynomial, and the proving key is a set of chain bases.  The STARK stage is excluded.  `prove` applies no
+blinding; `prove_zk_device` (a circuit built with zk=True) adds synthetic alpha / beta / delta key terms and the r, s
+blinding on the device.  What is measured and parity-checked is exactly the MSM + NTT work of a Groth16 prove.
+`Groth16Prover` proves a caller-supplied key whose alpha / beta ride on variable 0 (no blinding); `Groth16ZkProver`
+proves a key in the ark-groth16 / gnark layout, blinded, as those provers do.
 All arithmetic runs in libb200zk.so; Python only sequences the calls.
 """
 from __future__ import annotations
 
 import hashlib
+import secrets
 from dataclasses import dataclass, field
 
 from . import _ffi as F
@@ -33,6 +38,16 @@ def _seed64(data: bytes, tag: bytes) -> int:
 def _chain_kd(tag: bytes) -> tuple[int, int]:
     h = hashlib.sha256(b"b200zk-pk-" + tag).digest()
     return (int.from_bytes(h[:16], "little") | 1), (int.from_bytes(h[16:], "little") | 1)
+
+
+def random_scalar(randbits=secrets.randbits) -> int:
+    """A uniform blinding scalar in [0, r): 254 random bits, drawn again while the value is >= r.  Rejection instead of
+    a reduction mod r, which would make the values below 2^254 - r twice as likely; r > 2^253, so fewer than two draws
+    are needed on average.  `randbits(k)` -> k random bits (a CSPRNG by default)."""
+    while True:
+        x = randbits(254)
+        if x < R_MOD:
+            return x
 
 
 def quotient_on_device(ctx, log_n: int, a, b, c, zinv: int):
@@ -55,7 +70,7 @@ class Groth16Prover:
     """The same pipeline over a CALLER-SUPPLIED proving key (what a zkVM SDK would hand to `B200Backend`): query
     columns as EIP-196/197 byte strings, one point per R1CS variable (`a_g1`, `b_g1`, `b_g2`), per private variable
     (`l_g1`) and per quotient coefficient (`h_g1`, n-1 points).  No blinding (r = s = 0): the proof verifies, it is
-    not zero-knowledge.  tests/test_gpu_parity.py proves a small real R1CS with it and checks the Groth16
+    not zero-knowledge (Groth16ZkProver is).  tests/test_gpu_parity.py proves a small real R1CS with it and checks the Groth16
     verification equation with the GPU pairing check."""
 
     def __init__(self, ctx, log_n: int, a_g1: bytes, b_g1: bytes, b_g2: bytes, l_g1: bytes, h_g1: bytes, n_public: int):
@@ -77,10 +92,8 @@ class Groth16Prover:
             self.ctx.bases_free(h)
         self.h.clear()
 
-    def prove(self, z, a_evals, b_evals, c_evals) -> bytes:
-        """z: the full assignment (integers mod r, z[0] = 1, then the public inputs, then the private variables);
-        a/b/c_evals: (A z), (B z), (C z) on the domain.  Returns A (64) | B (128) | C (64).
-        ONE call of the C ABI (b200zk_groth16_commit) with host buffers -- what rust/ethrex-backend/src/b200.rs does."""
+    def _host_inputs(self, z, a_evals, b_evals, c_evals):
+        """(witness, a, b, c) host buffers of the C ABI: canonical LE witness, Montgomery LE evaluations"""
         if len(z) != self.m or any(len(e) != self.n for e in (a_evals, b_evals, c_evals)):
             raise ValueError("assignment / evaluation vector sizes do not match the proving key")
         r_mont = (1 << 256) % R_MOD
@@ -89,8 +102,40 @@ class Groth16Prover:
             return b"".join(int(v % R_MOD * r_mont % R_MOD).to_bytes(32, "little") for v in vals)
 
         zb = b"".join(int(v % R_MOD).to_bytes(32, "little") for v in z)
-        proof, self.b_g1 = self.ctx.groth16_commit(self.pk, zb, bytearray(mont(a_evals)), bytearray(mont(b_evals)), bytearray(mont(c_evals)))
+        return zb, bytearray(mont(a_evals)), bytearray(mont(b_evals)), bytearray(mont(c_evals))
+
+    def prove(self, z, a_evals, b_evals, c_evals) -> bytes:
+        """z: the full assignment (integers mod r, z[0] = 1, then the public inputs, then the private variables);
+        a/b/c_evals: (A z), (B z), (C z) on the domain.  Returns A (64) | B (128) | C (64).
+        ONE call of the C ABI (b200zk_groth16_commit) with host buffers -- what rust/ethrex-backend/src/b200.rs does."""
+        proof, self.b_g1 = self.ctx.groth16_commit(self.pk, *self._host_inputs(z, a_evals, b_evals, c_evals))
         return proof
+
+
+class Groth16ZkProver(Groth16Prover):
+    """The zero-knowledge prove over a key in the ark-groth16 / gnark layout: the query columns WITHOUT alpha and beta
+    folded into variable 0, and beside them the key terms alpha1, beta1, delta1 (G1, 64 bytes each) and beta2, delta2
+    (G2, 128 bytes each), all EIP-196/197 bytes.  `prove` returns the proof ark-groth16 0.5 (create_proof_with_reduction)
+    and gnark (groth16.Prove) return for the same blinding scalars r, s:
+        A = alpha1 + sum z_i A_i + r delta1      B = beta2 + sum z_i B2_i + s delta2
+        C = [L] + [H] + s A + r (beta1 + sum z_i B1_i + s delta1) - r s delta1
+    r and s default to fresh draws of `random_scalar`; pass them to get a reproducible proof."""
+
+    def __init__(self, ctx, log_n: int, a_g1: bytes, b_g1: bytes, b_g2: bytes, l_g1: bytes, h_g1: bytes, n_public: int,
+                 alpha_g1: bytes, beta_g1: bytes, beta_g2: bytes, delta_g1: bytes, delta_g2: bytes):
+        if any(len(x) != 64 for x in (alpha_g1, beta_g1, delta_g1)) or any(len(x) != 128 for x in (beta_g2, delta_g2)):
+            raise ValueError("key terms: alpha1, beta1, delta1 are 64-byte G1 points, beta2 and delta2 128-byte G2 points")
+        super().__init__(ctx, log_n, a_g1, b_g1, b_g2, l_g1, h_g1, n_public)
+        self.h["terms_g1"] = ctx.g1_bases_upload(alpha_g1 + beta_g1 + delta_g1, 3, F.POINTS_BE)
+        self.h["terms_g2"] = ctx.g2_bases_upload(beta_g2 + delta_g2, 2, F.POINTS_BE)
+
+    def prove(self, z, a_evals, b_evals, c_evals, r: int | None = None, s: int | None = None) -> bytes:
+        """As Groth16Prover.prove, blinded with r and s (each in [0, group order); None = a fresh random draw).
+        ONE call of the C ABI (b200zk_groth16_prove)."""
+        r = random_scalar() if r is None else r
+        s = random_scalar() if s is None else s
+        zk = self.ctx.groth16_zk(self.h["terms_g1"], self.h["terms_g2"], r, s)
+        return self.ctx.groth16_prove(self.pk, zk, *self._host_inputs(z, a_evals, b_evals, c_evals))
 
 
 class Groth16Verifier:
@@ -167,9 +212,13 @@ class SyntheticWrapCircuit:
     # the workspaces' 1/8 growth slack
     PROVE_WORKSPACE_PER_POINT = 1152
 
-    def __init__(self, ctx, log_n: int, precompute: bool = True, g2: bool = True, rank: int = 0, world: int = 1):
+    # synthetic ark-layout key terms (zk=True): alpha1, beta1, delta1 and beta2, delta2 as short chains
+    ZK_TERMS = (("terms_g1", False, 3), ("terms_g2", True, 2))
+
+    def __init__(self, ctx, log_n: int, precompute: bool = True, g2: bool = True, rank: int = 0, world: int = 1, zk: bool = False):
         """rank/world: every rank keeps only its contiguous shard [lo, hi) of each proving-key column (point-split
-        MSMs, ethrex_b200.dist.msm_sharded); the NTTs of the quotient are cheap and computed on every rank."""
+        MSMs, ethrex_b200.dist.msm_sharded); the NTTs of the quotient are cheap and computed on every rank.
+        zk: also hold the alpha / beta / delta key terms (whole, on every rank) that prove_zk_device blinds with."""
         import torch
         from .dist import shard_range
         self.ctx, self.log_n, self.n = ctx, log_n, 1 << log_n
@@ -211,6 +260,13 @@ class SyntheticWrapCircuit:
                     self.plain_columns.append(name)
             self.pk.handles[name] = h
             self.pk.chains[name] = (k, d, is_g2)
+        if zk:
+            for name, is_g2, cnt in self.ZK_TERMS:
+                k, d = _chain_kd(name.encode())
+                pts = torch.empty((16 if is_g2 else 8) * cnt, dtype=torch.int64, device="cuda")
+                (ctx.g2_chain_device if is_g2 else ctx.g1_chain_device)(pts, 0, cnt, k, d)
+                self.pk.handles[name] = (ctx.g2_bases_from_device if is_g2 else ctx.g1_bases_from_device)(pts, cnt)
+                self.pk.chains[name] = (k, d, is_g2)
         self.zinv = coset_vanishing_inverse(log_n)
 
     def close(self):
@@ -251,7 +307,6 @@ class SyntheticWrapCircuit:
         """-> (proof bytes A | B2 | C, [B]1 bytes).  One GPU: ONE C-ABI call (b200zk_groth16_commit) on device inputs.
         Several GPUs: the quotient's NTTs are dealt across ranks (dist.quotient_dealt), every rank commits its shard of
         the proving key (b200zk_groth16_commit_partial), ONE all_gather moves the 768-byte blocks and every rank folds."""
-        import torch
         ctx = self.ctx
         w, a, b, c = self.assign(serialized_input)
         pk = self.pk_struct()
@@ -259,14 +314,45 @@ class SyntheticWrapCircuit:
             raise ValueError("the one-call path needs the G2 column")
         if self.world == 1:
             return ctx.groth16_commit(pk, w, a, b, c, F.G16_INPUTS_DEVICE)
+        return ctx.groth16_fold(self._gathered_blocks(pk, w, a, b, c, group), self.world)
+
+    def _gathered_blocks(self, pk, w, a, b, c, group):
+        """several GPUs: the dealt quotient, this rank's commit_partial and ONE all_gather of the 768-byte blocks"""
+        import torch
         import torch.distributed as dist
         from .dist import quotient_dealt
-        h = quotient_dealt(ctx, self.log_n, a, b, c, self.zinv, self.rank, self.world, group)
+        h = quotient_dealt(self.ctx, self.log_n, a, b, c, self.zinv, self.rank, self.world, group)
         block = torch.zeros(96, dtype=torch.int64, device=w.device)  # 768 bytes: A | B1 | B2 | L | H partial sums
-        ctx.groth16_commit_partial(pk, w, h, None, None, block, F.G16_INPUTS_DEVICE | F.G16_H_COEFFS)
+        self.ctx.groth16_commit_partial(pk, w, h, None, None, block, F.G16_INPUTS_DEVICE | F.G16_H_COEFFS)
         gathered = torch.empty(96 * self.world, dtype=torch.int64, device=w.device)
         dist.all_gather_into_tensor(gathered, block, group=group)
-        return ctx.groth16_fold(gathered, self.world)
+        return gathered
+
+    def prove_zk_device(self, serialized_input: bytes, r: int | None = None, s: int | None = None, group=None) -> bytes:
+        """-> the blinded proof A | B2 | C over the synthetic key with its alpha / beta / delta terms (built with zk=True).
+        r, s: blinding scalars in [0, group order); None = a fresh random draw.  One GPU: ONE C-ABI call
+        (b200zk_groth16_prove).  Several GPUs: rank 0's r and s are broadcast, every rank commits its shard, the blocks
+        are all-gathered once and every rank folds them with the same r and s (b200zk_groth16_fold_zk)."""
+        import torch
+        ctx, hd = self.ctx, self.pk.handles
+        if "terms_g1" not in hd:
+            raise ValueError("prove_zk_device needs the key terms: build the circuit with zk=True")
+        if "b_g2" not in hd:
+            raise ValueError("the one-call path needs the G2 column")
+        r = random_scalar() if r is None else r
+        s = random_scalar() if s is None else s
+        w, a, b, c = self.assign(serialized_input)
+        pk = self.pk_struct()
+        if self.world > 1:
+            import torch.distributed as dist
+            rs = torch.tensor(list(int(r).to_bytes(32, "little") + int(s).to_bytes(32, "little")), dtype=torch.uint8, device=w.device)
+            dist.broadcast(rs, src=0 if group is None else dist.get_global_rank(group, 0), group=group)
+            rsb = bytes(rs.cpu().tolist())
+            r, s = int.from_bytes(rsb[:32], "little"), int.from_bytes(rsb[32:], "little")
+        zk = ctx.groth16_zk(hd["terms_g1"], hd["terms_g2"], r, s)
+        if self.world == 1:
+            return ctx.groth16_prove(pk, zk, w, a, b, c, F.G16_INPUTS_DEVICE)
+        return ctx.groth16_fold_zk(zk, self._gathered_blocks(pk, w, a, b, c, group), self.world)
 
     def commit(self, w, h_coeffs, msm=None):
         """The five MSMs as separate calls (the pre-ABI-v2 path, kept as a cross-check of the one-call path and for the

@@ -238,6 +238,8 @@ int b200zk_msm_multi_resident_device(b200zk_ctx* ctx, const uint64_t* handles, s
  *     quotient  3 iNTT + 3 coset NTT + (a*b - c)/Z_H + 1 coset iNTT    (coset generator 5, the context's NTT root)
  *     commit    [A]1, [B]1, [B]2 over the witness, [L]1 over its private part, [H]1 over the quotient's coefficients
  *     assemble  proof = A (64) | B2 (128, x_im|x_re|y_im|y_re) | C (64), C = [L]1 + [H]1; no blinding (r = s = 0)
+ *               and no alpha / beta terms (a key that folds them into variable 0); b200zk_groth16_prove below is the
+ *               blinded proof over the ark / gnark key layout
  * Columns: 0 = A_g1, 1 = B_g1 (handle 0 = absent), 2 = B_g2, 3 = L_g1, 4 = H_g1.  count[k] = points of column k this
  * context multiplies; offset[k] = index of the scalar its first point multiplies -- into the witness for columns 0..3
  * (L_g1 of a whole key: offset = number of public inputs incl. the leading 1), into the quotient's coefficients for
@@ -264,6 +266,33 @@ int b200zk_groth16_commit_partial(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, 
                                   void* b_evals, void* c_evals, uint32_t flags, void* stream, void* d_partials768);
 int b200zk_groth16_fold(b200zk_ctx* ctx, const void* d_partials, size_t count, void* stream, uint8_t proof[256],
                         uint8_t b_g1[64]);
+
+/* ---- zero-knowledge Groth16: the key's alpha / beta / delta terms and the blinding scalars r, s ----------------------
+ * The proof ark-groth16 0.5 (create_proof_with_reduction, behind risc0-groth16) and gnark groth16.Prove (behind SP1's
+ * wrap) return for the same r and s, over a key in their layout, where alpha and beta are NOT folded into the columns:
+ *     A  = alpha1 + sum z_i A_i + r delta1           B2 = beta2 + sum z_i B2_i + s delta2
+ *     C  = [L]1 + [H]1 + s A + r B1 - (r s) delta1,   B1 = beta1 + sum z_i B1_i + s delta1
+ *     proof = A (64) | B2 (128, x_im|x_re|y_im|y_re) | C (64), EIP-196/197 bytes
+ * The key terms are uploaded once with b200zk_g1_bases_upload / b200zk_g2_bases_upload (validated like any column) and
+ * must stay plain bases (not precomputed).  r and s are inputs -- the library never draws randomness, so a proof is
+ * reproducible -- and must be canonical little-endian values below the group order: a larger value is refused with
+ * B200ZK_ERR_NOT_IN_FIELD, not reduced (reducing would bias raw random bytes).  r = s = 0 gives the unblinded proof.
+ * B200ZK_ERR_INVALID_ARG: a NULL zk; a term handle that is unknown, of the wrong group or point count, BLS12-381 or
+ * precomputed; and in b200zk_groth16_prove, r != 0 with the B_g1 column absent (C needs [B]1). */
+typedef struct b200zk_groth16_zk {
+  uint64_t g1_terms;  /* resident G1 handle of exactly 3 points: alpha, beta, delta (plain bases, not precomputed) */
+  uint64_t g2_terms;  /* resident G2 handle of exactly 2 points: beta, delta */
+  uint8_t r[32];      /* canonical little-endian, < group order */
+  uint8_t s[32];
+} b200zk_groth16_zk;
+/* b200zk_groth16_commit_partial followed by b200zk_groth16_fold_zk on one stream, one synchronisation at the end;
+ * arguments as b200zk_groth16_commit */
+int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const b200zk_groth16_zk* zk, const void* witness,
+                         void* a_evals, void* b_evals, void* c_evals, uint32_t flags, void* stream, uint8_t proof[256]);
+/* folds `count` 768-byte blocks of b200zk_groth16_commit_partial (one per rank), then adds the key terms and the
+ * blinding once: every rank of a point-split prove folds the all-gathered blocks with the same r and s */
+int b200zk_groth16_fold_zk(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void* d_partials, size_t count,
+                           void* stream, uint8_t proof[256]);
 
 /* ---- BLS12-381 G1 / EIP-4844 blob commitments (SURVEY.md section 8(f) rank 3) -------------------------------------
  * The L2 committer's "commit" step: /root/reference/crates/common/crypto/kzg.rs:259-272 (blob_to_kzg_commitment_and_proof ->

@@ -53,6 +53,17 @@ pub struct b200zk_groth16_pk {
     pub offset: [u64; 5],
 }
 
+/// `struct b200zk_groth16_zk` (include/b200zk.h): resident handles of the key terms (G1: alpha, beta, delta; G2: beta,
+/// delta; plain bases) and the blinding scalars r, s (canonical little-endian, below the group order).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct b200zk_groth16_zk {
+    pub g1_terms: u64,
+    pub g2_terms: u64,
+    pub r: [u8; 32],
+    pub s: [u8; 32],
+}
+
 unsafe extern "C" {
     pub fn b200zk_abi_version() -> c_int;
     pub fn b200zk_device_count() -> c_int;
@@ -88,6 +99,8 @@ unsafe extern "C" {
     pub fn b200zk_groth16_commit(ctx: *mut b200zk_ctx, pk: *const b200zk_groth16_pk, witness: *const c_void, a_evals: *mut c_void, b_evals: *mut c_void, c_evals: *mut c_void, flags: u32, stream: *mut c_void, proof: *mut u8, b_g1: *mut u8) -> c_int;
     pub fn b200zk_groth16_commit_partial(ctx: *mut b200zk_ctx, pk: *const b200zk_groth16_pk, witness: *const c_void, a_evals: *mut c_void, b_evals: *mut c_void, c_evals: *mut c_void, flags: u32, stream: *mut c_void, d_partials768: *mut c_void) -> c_int;
     pub fn b200zk_groth16_fold(ctx: *mut b200zk_ctx, d_partials: *const c_void, count: usize, stream: *mut c_void, proof: *mut u8, b_g1: *mut u8) -> c_int;
+    pub fn b200zk_groth16_prove(ctx: *mut b200zk_ctx, pk: *const b200zk_groth16_pk, zk: *const b200zk_groth16_zk, witness: *const c_void, a_evals: *mut c_void, b_evals: *mut c_void, c_evals: *mut c_void, flags: u32, stream: *mut c_void, proof: *mut u8) -> c_int;
+    pub fn b200zk_groth16_fold_zk(ctx: *mut b200zk_ctx, zk: *const b200zk_groth16_zk, d_partials: *const c_void, count: usize, stream: *mut c_void, proof: *mut u8) -> c_int;
 
     pub fn b200zk_g1_msm_partial_device(ctx: *mut b200zk_ctx, d_points: *const c_void, d_scalars: *const c_void, n: usize, flags: u32, stream: *mut c_void, d_partial128: *mut c_void) -> c_int;
     pub fn b200zk_g2_msm_partial_device(ctx: *mut b200zk_ctx, d_points: *const c_void, d_scalars: *const c_void, n: usize, flags: u32, stream: *mut c_void, d_partial256: *mut c_void) -> c_int;

@@ -10,6 +10,7 @@
 //! zkVM SDK and is injected through [`WrapCircuit`]; without one, `prove` returns
 //! `BackendError::NotImplemented` for `ProofFormat::Groth16`, exactly like a backend built without its SDK.
 //! Drop this file in as `crates/prover/src/backend/b200.rs` (wiring in INTEGRATION.md).
+use std::io::Read;
 use std::sync::OnceLock;
 use std::time::{Duration, Instant};
 
@@ -22,7 +23,8 @@ use ethrex_prover::backend::{BackendError, ExecBackend, ProverBackend};
 
 use crate::ffi;
 
-/// What the zkVM SDK has to provide for the Groth16 wrap: the witness vector and the proving-key columns.
+/// What the zkVM SDK has to provide for the Groth16 wrap: the witness vector and the proving key in the layout of
+/// ark-groth16 / gnark (query columns plus the separate alpha, beta, delta terms).
 /// All buffers use the library's native formats (ark-ff Montgomery limbs for points, canonical limbs for
 /// scalars), i.e. the in-memory form the arkworks-based wrap provers already hold them in.
 pub trait WrapCircuit: Send + Sync {
@@ -36,17 +38,25 @@ pub trait WrapCircuit: Send + Sync {
     /// one scalar per point of `pk_a_g1`.
     fn witness(&self, serialized_input: &[u8]) -> Result<Vec<u8>, BackendError>;
     /// Proving-key columns as native affine points: A (G1), B (G1), B (G2) with one point per variable; L (G1) with
-    /// one point per PRIVATE variable; H (G1) with one point per quotient coefficient (2^k - 1 points).
+    /// one point per PRIVATE variable; H (G1) with one point per quotient coefficient (2^k - 1 points).  alpha and
+    /// beta are NOT folded into the columns (ark-groth16 `a_query` / `b_g1_query` / `b_g2_query`, gnark `G1.A` ...).
     fn pk_a_g1(&self) -> &[u8];
     fn pk_b_g1(&self) -> &[u8];
     fn pk_b_g2(&self) -> &[u8];
     fn pk_l_g1(&self) -> &[u8];
     fn pk_h_g1(&self) -> &[u8];
+    /// The key terms as native affine points: alpha, beta, delta in G1 (64 bytes each), beta, delta in G2 (128 bytes
+    /// each).  The device adds them and the blinding r delta1, s delta2, s A + r B1 - r s delta1 to the proof.
+    fn pk_alpha_g1(&self) -> &[u8];
+    fn pk_beta_g1(&self) -> &[u8];
+    fn pk_beta_g2(&self) -> &[u8];
+    fn pk_delta_g1(&self) -> &[u8];
+    fn pk_delta_g2(&self) -> &[u8];
     /// Evaluations of A*w, B*w, C*w over the domain (Montgomery limbs), from which the library builds the quotient H.
     fn abc_evaluations(&self, witness: &[u8]) -> Result<[Vec<u8>; 3], BackendError>;
-    /// Final assembly with the SDK's blinding terms and selector bytes (`sp1.rs:176-194`, `risc0.rs:43-59`); `proof`
-    /// is the unblinded A | B2 | C the device produced, `b_g1` the [B]1 commitment blinding needs.
-    fn assemble(&self, proof: &[u8; 256], b_g1: &[u8; 64]) -> Result<Vec<u8>, BackendError>;
+    /// Final encoding with the SDK's selector bytes (`sp1.rs:176-194`, `risc0.rs:43-59`); `proof` is the blinded
+    /// A | B2 | C the device produced.
+    fn assemble(&self, proof: &[u8; 256]) -> Result<Vec<u8>, BackendError>;
     /// The ecpairing calldata of the Groth16 verification equation for `proof`
     /// (`-A | B | alpha | beta | IC(public inputs) | gamma | C | delta`, 4 x 192 bytes), when the SDK exposes its
     /// verifying key; `None` makes `verify` answer "not implemented", like the reference's default.
@@ -64,6 +74,39 @@ pub struct B200ProveOutput {
 /// `static PROVER_SETUP: OnceLock<ProverSetup>` in the reference (`sp1.rs:30,93-95`).
 struct ResidentKey {
     pk: b200zk_sys::b200zk_groth16_pk,
+    g1_terms: u64,
+    g2_terms: u64,
+}
+
+/// The BN254 group order r, little-endian bytes.
+const FR_ORDER_LE: [u8; 32] = [
+    0x01, 0x00, 0x00, 0xf0, 0x93, 0xf5, 0xe1, 0x43, 0x91, 0x70, 0xb9, 0x79, 0x48, 0xe8, 0x33, 0x28, 0x5d, 0x58, 0x81, 0x81, 0xb6, 0x45,
+    0x50, 0xb8, 0x29, 0xa0, 0x31, 0xe1, 0x72, 0x4e, 0x64, 0x30,
+];
+
+fn below_order(x: &[u8; 32]) -> bool {
+    for (a, b) in x.iter().rev().zip(FR_ORDER_LE.iter().rev()) {
+        if a != b {
+            return a < b;
+        }
+    }
+    false
+}
+
+/// A uniform blinding scalar in [0, r), canonical little-endian: 254 random bits, drawn again while the value is >= r.
+/// Rejection rather than a reduction mod r, which would make the values below 2^254 - r twice as likely; fewer than two
+/// draws are needed on average.
+fn blinding_scalar(rng: &mut impl Read) -> Result<[u8; 32], BackendError> {
+    loop {
+        let mut x = [0u8; 32];
+        rng.read_exact(&mut x).map_err(BackendError::proving)?;
+        if let Some(top) = x.last_mut() {
+            *top &= 0x3f;
+        }
+        if below_order(&x) {
+            return Ok(x);
+        }
+    }
 }
 
 #[derive(Default)]
@@ -88,7 +131,8 @@ impl B200Backend {
         Self { circuit: Some(circuit), resident: OnceLock::new() }
     }
 
-    /// Upload + precompute the five columns once; checks the column sizes against each other instead of truncating.
+    /// Upload + precompute the five columns and upload the key terms once; checks the sizes against each other instead
+    /// of truncating.
     fn load_key(circuit: &dyn WrapCircuit, gpu: &mut ffi::B200zk) -> Result<ResidentKey, BackendError> {
         let k = circuit.domain_log2();
         let n = 1u64.checked_shl(k).ok_or_else(|| BackendError::serialization("domain too large"))?;
@@ -101,6 +145,14 @@ impl B200Backend {
                 "proving-key columns disagree: A {m}, B1 {mb1}, B2 {mb2} (must be equal), L {ml} (must be A - {n_pub} public), H {mh} (must be 2^{k} - 1)"
             )));
         }
+        let g1_sizes = [circuit.pk_alpha_g1().len(), circuit.pk_beta_g1().len(), circuit.pk_delta_g1().len()];
+        let g2_sizes = [circuit.pk_beta_g2().len(), circuit.pk_delta_g2().len()];
+        if g1_sizes != [64; 3] || g2_sizes != [128; 2] {
+            return Err(BackendError::serialization("key terms: alpha, beta, delta in G1 are 64 bytes each, beta and delta in G2 128 bytes each"));
+        }
+        // plain bases: the key terms are three scalar multiplications' worth of work, not an MSM
+        let g1_terms = gpu.g1_bases_upload(&[circuit.pk_alpha_g1(), circuit.pk_beta_g1(), circuit.pk_delta_g1()].concat(), 0)?;
+        let g2_terms = gpu.g2_bases_upload(&[circuit.pk_beta_g2(), circuit.pk_delta_g2()].concat(), 0)?;
         let handles = [
             gpu.g1_bases_upload(circuit.pk_a_g1(), 0)?,
             gpu.g1_bases_upload(circuit.pk_b_g1(), 0)?,
@@ -113,12 +165,15 @@ impl B200Backend {
         }
         Ok(ResidentKey {
             pk: b200zk_sys::b200zk_groth16_pk { log_n: k, reserved: 0, handle: handles, count: [m, m, m, ml, mh], offset: [0, 0, 0, n_pub, 0] },
+            g1_terms,
+            g2_terms,
         })
     }
 
     /// The hot path: one call -- 3 iNTT + 3 coset NTT + quotient + 1 coset iNTT, 4 G1 MSMs + 1 G2 MSM over the
-    /// resident key (A, B1, B2 share one digit sort), C = L + H -- and one synchronisation.
-    fn commit(&self, circuit: &dyn WrapCircuit, serialized: &[u8]) -> Result<([u8; 256], [u8; 64]), BackendError> {
+    /// resident key (A, B1, B2 share one digit sort), then the key terms and the blinding with fresh r, s from the
+    /// OS's random source -- and one synchronisation.
+    fn prove_blinded(&self, circuit: &dyn WrapCircuit, serialized: &[u8]) -> Result<[u8; 256], BackendError> {
         let gpu = ffi::global()?;
         let mut gpu = gpu.lock().map_err(|_| BackendError::proving("b200zk context poisoned"))?;
         let key = self
@@ -128,7 +183,14 @@ impl B200Backend {
             .map_err(BackendError::proving)?;
         let witness = circuit.witness(serialized)?;
         let [mut a, mut b, mut c] = circuit.abc_evaluations(&witness)?;
-        gpu.groth16_commit(&key.pk, &witness, &mut a, &mut b, &mut c)
+        let mut urandom = std::fs::File::open("/dev/urandom").map_err(BackendError::proving)?;
+        let zk = b200zk_sys::b200zk_groth16_zk {
+            g1_terms: key.g1_terms,
+            g2_terms: key.g2_terms,
+            r: blinding_scalar(&mut urandom)?,
+            s: blinding_scalar(&mut urandom)?,
+        };
+        gpu.groth16_prove(&key.pk, &zk, &witness, &mut a, &mut b, &mut c)
     }
 }
 
@@ -156,8 +218,8 @@ impl ProverBackend for B200Backend {
         ExecBackend::new().execute(input)?;
         match (format, self.circuit.as_deref()) {
             (ProofFormat::Groth16, Some(circuit)) => {
-                let (proof, b_g1) = self.commit(circuit, &serialized)?;
-                Ok(B200ProveOutput { prover_type: circuit.prover_type(), proof: circuit.assemble(&proof, &b_g1)? })
+                let proof = self.prove_blinded(circuit, &serialized)?;
+                Ok(B200ProveOutput { prover_type: circuit.prover_type(), proof: circuit.assemble(&proof)? })
             }
             (ProofFormat::Groth16, None) => Err(BackendError::not_implemented(
                 "b200 backend built without a wrap circuit: ProofFormat::Groth16 needs a zkVM SDK's proving key",

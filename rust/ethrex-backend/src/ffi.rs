@@ -28,6 +28,26 @@ pub fn global() -> Result<&'static Mutex<B200zk>, BackendError> {
         .map_err(BackendError::proving)
 }
 
+/// The host buffers of a Groth16 call must hold what the library copies out of them: 2^log_n evaluations each, and a
+/// witness that reaches the end of every column multiplying it (columns 0..3).
+fn check_groth16_inputs(what: &str, pk: &sys::b200zk_groth16_pk, witness: &[u8], a: &[u8], b: &[u8], c: &[u8]) -> Result<(), BackendError> {
+    let n_bytes = 32usize.checked_shl(pk.log_n).ok_or_else(|| BackendError::serialization(format!("{what}: log_n too large")))?;
+    if a.len() != n_bytes || b.len() != n_bytes || c.len() != n_bytes {
+        return Err(BackendError::serialization(format!("{what}: evaluation vectors must hold 2^log_n elements")));
+    }
+    let mut wit_end = 0u64;
+    for ((h, cnt), off) in pk.handle.iter().zip(pk.count.iter()).zip(pk.offset.iter()).take(4) {
+        if *h != 0 {
+            wit_end = wit_end.max(off.checked_add(*cnt).ok_or_else(|| BackendError::serialization(format!("{what}: column range overflows")))?);
+        }
+    }
+    let have = u64::try_from(witness.len() / 32).map_err(BackendError::serialization)?;
+    if have < wit_end {
+        return Err(BackendError::serialization(format!("{what}: witness holds {have} scalars, the proving key multiplies {wit_end}")));
+    }
+    Ok(())
+}
+
 fn status_message(ctx: Option<&B200zk>, status: i32) -> String {
     // SAFETY: both functions return NUL-terminated strings owned by the library / the context.
     let base = unsafe { CStr::from_ptr(sys::b200zk_strerror(status)) }.to_string_lossy().into_owned();
@@ -150,21 +170,7 @@ impl B200zk {
     /// call with one synchronisation.  `witness`: canonical LE scalars; `a`, `b`, `c`: (A z), (B z), (C z) on the
     /// domain, Montgomery LE, 2^log_n elements each.  Returns (A | B2 | C, [B]1).
     pub fn groth16_commit(&mut self, pk: &sys::b200zk_groth16_pk, witness: &[u8], a: &mut [u8], b: &mut [u8], c: &mut [u8]) -> Result<([u8; 256], [u8; 64]), BackendError> {
-        let n_bytes = 32usize.checked_shl(pk.log_n).ok_or_else(|| BackendError::serialization("groth16_commit: log_n too large"))?;
-        if a.len() != n_bytes || b.len() != n_bytes || c.len() != n_bytes {
-            return Err(BackendError::serialization("groth16_commit: evaluation vectors must hold 2^log_n elements"));
-        }
-        // the witness must reach the end of every column that multiplies it (columns 0..3)
-        let mut wit_end = 0u64;
-        for ((h, cnt), off) in pk.handle.iter().zip(pk.count.iter()).zip(pk.offset.iter()).take(4) {
-            if *h != 0 {
-                wit_end = wit_end.max(off.checked_add(*cnt).ok_or_else(|| BackendError::serialization("groth16_commit: column range overflows"))?);
-            }
-        }
-        let have = u64::try_from(witness.len() / 32).map_err(BackendError::serialization)?;
-        if have < wit_end {
-            return Err(BackendError::serialization(format!("groth16_commit: witness holds {have} scalars, the proving key multiplies {wit_end}")));
-        }
+        check_groth16_inputs("groth16_commit", pk, witness, a, b, c)?;
         let mut proof = [0u8; 256];
         let mut b1 = [0u8; 64];
         // SAFETY: lengths checked above; host buffers outlive the synchronous call; NULL stream = the context's own.
@@ -174,6 +180,21 @@ impl B200zk {
         };
         check(self, status)?;
         Ok((proof, b1))
+    }
+
+    /// The blinded Groth16 proof (ark-groth16 / gnark) in one call: `groth16_commit`'s pipeline, then the key's alpha /
+    /// beta / delta terms (`zk.g1_terms`, `zk.g2_terms`) and the blinding scalars `zk.r`, `zk.s` added on the device.
+    /// Returns A | B2 | C.
+    pub fn groth16_prove(&mut self, pk: &sys::b200zk_groth16_pk, zk: &sys::b200zk_groth16_zk, witness: &[u8], a: &mut [u8], b: &mut [u8], c: &mut [u8]) -> Result<[u8; 256], BackendError> {
+        check_groth16_inputs("groth16_prove", pk, witness, a, b, c)?;
+        let mut proof = [0u8; 256];
+        // SAFETY: lengths checked above; host buffers outlive the synchronous call; NULL stream = the context's own.
+        let status = unsafe {
+            sys::b200zk_groth16_prove(self.ctx.as_ptr(), pk, zk, witness.as_ptr().cast(), a.as_mut_ptr().cast(), b.as_mut_ptr().cast(), c.as_mut_ptr().cast(), 0,
+                                      std::ptr::null_mut(), proof.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(proof)
     }
 
     pub fn g1_msm_resident(&mut self, handle: u64, scalars: &[u8], flags: u32) -> Result<[u8; 64], BackendError> {
