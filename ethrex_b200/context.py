@@ -320,6 +320,31 @@ class Context:
         self._check(F.lib.b200zk_kzg_blob_to_commitment(self._h, setup_handle, bp, k, out), "b200zk_kzg_blob_to_commitment")
         return [out.raw[48 * i:48 * i + 48] for i in range(k)]
 
+    @staticmethod
+    def _blob_count(blobs) -> int:
+        total = _host_len(blobs)
+        if total % (4096 * 32):
+            raise B200Error.serialization("a blob is 4096 x 32 bytes")
+        return total // (4096 * 32)
+
+    def kzg_blob_to_commitment_and_proof(self, setup_handle: int, blobs) -> tuple:
+        """blobs: k x 131072 bytes -> ([48-byte commitments], [48-byte proofs at the EIP-4844 Fiat-Shamir challenge])"""
+        k = self._blob_count(blobs)
+        bp, keep = _host_ptr(blobs)
+        cm, pr = C.create_string_buffer(max(1, 48 * k)), C.create_string_buffer(max(1, 48 * k))
+        self._check(F.lib.b200zk_kzg_blob_to_commitment_and_proof(self._h, setup_handle, bp, k, cm, pr), "b200zk_kzg_blob_to_commitment_and_proof")
+        return [cm.raw[48 * i:48 * i + 48] for i in range(k)], [pr.raw[48 * i:48 * i + 48] for i in range(k)]
+
+    def kzg_compute_proof(self, setup_handle: int, blobs, z) -> tuple:
+        """blobs: k x 131072 bytes, z: k x 32-byte big-endian -> ([48-byte proofs], [y = p(z), 32-byte big-endian])"""
+        k = self._blob_count(blobs)
+        _need(z, 32 * k, "b200zk_kzg_compute_proof z")
+        bp, keep = _host_ptr(blobs)
+        zp, keep_z = _host_ptr(z)
+        pr, y = C.create_string_buffer(max(1, 48 * k)), C.create_string_buffer(max(1, 32 * k))
+        self._check(F.lib.b200zk_kzg_compute_proof(self._h, setup_handle, bp, k, zp, pr, y), "b200zk_kzg_compute_proof")
+        return [pr.raw[48 * i:48 * i + 48] for i in range(k)], [y.raw[32 * i:32 * i + 32] for i in range(k)]
+
     # ------------------------------------------------------------------ NTT root of unity (SURVEY.md section 8c)
     NTT_ROOT_ARK, NTT_ROOT_HALO2 = 0, 1
 

@@ -89,7 +89,7 @@ struct FeBig {
     for (int i = 0; i < N; ++i) r.v[i] = borrow ? a.v[i] : t.v[i];
     return r;
   }
-  static B2_D FeBig add(const FeBig& a, const FeBig& b) {  // 2p < 2^384: no carry out
+  static B2_D FeBig add(const FeBig& a, const FeBig& b) {  // 2p < 2^384 and 2r < 2^256: no carry out
     FeBig s;
     uint64_t c = 0;
 #pragma unroll
@@ -133,7 +133,7 @@ struct FeBig {
     FeBig r;
 #pragma unroll
     for (int i = 0; i < N; ++i) r.v[i] = t[i];
-    return reduce_once(r);  // inputs < p => value < 2p, and t[N] == 0 (p < 2^381)
+    return reduce_once(r);  // inputs < p => value < 2p, and t[N] == 0 (2p < 2^(32 N) for both moduli)
   }
   static B2_D FeBig sqr(const FeBig& a) { return mul(a, a); }
   static B2_D FeBig mul2_sub(const FeBig& a, const FeBig& b, const FeBig& c, const FeBig& d) { return sub(mul(a, b), mul(c, d)); }
@@ -151,9 +151,9 @@ struct FeBig {
   }
   static B2_D FeBig inv(const FeBig& a) {  // Fermat; inv(0) = 0
     uint32_t e[N];
+    uint32_t br = 2;  // e = modulus - 2, borrow propagated: r ends in ...00000001
 #pragma unroll
-    for (int i = 0; i < N; ++i) e[i] = Cfg::mod(i);
-    e[0] -= 2;  // p ends in ...aaab: no borrow
+    for (int i = 0; i < N; ++i) { e[i] = Cfg::mod(i) - br; br = Cfg::mod(i) < br ? 1u : 0u; }
     return pow(a, e);
   }
   static B2_D FeBig sqrt_candidate(const FeBig& a) {  // a^((p+1)/4)
@@ -165,5 +165,23 @@ struct FeBig {
 };
 
 typedef FeBig<Fp381Cfg> Fp381;
+
+// BLS12-381 scalar field Fr (255 bits, 8 x 32-bit limbs, Montgomery R = 2^256): the field blobs are polynomials over, for
+// the EIP-4844 proof (evaluation at z and the quotient (p(X) - y) / (X - z)).  2r < 2^256, so FeBig's add and mul bounds hold.
+struct Fr381Cfg {
+  static constexpr int N = 8;
+  static B2_HD constexpr uint32_t mod(int i) { return bls_r_limb(i); }
+  static B2_HD constexpr uint32_t r1(int i) {  // 2^256 mod r
+    constexpr uint32_t m[8] = {0xfffffffeu, 0x00000001u, 0x00034802u, 0x5884b7fau, 0xecbc4ff5u, 0x998c4fefu, 0xacc5056fu, 0x1824b159u};
+    return m[i];
+  }
+  static B2_HD constexpr uint32_t r2(int i) {  // 2^512 mod r
+    constexpr uint32_t m[8] = {0xf3f29c6du, 0xc999e990u, 0x87925c23u, 0x2b6cedcbu, 0x7254398fu, 0x05d31496u, 0x9f59ff11u, 0x0748d9d9u};
+    return m[i];
+  }
+  static constexpr uint32_t INV = 0xffffffffu;  // -r^-1 mod 2^32 (r = 1 mod 2^32)
+};
+
+typedef FeBig<Fr381Cfg> Fr381;
 
 }  // namespace b200zk

@@ -64,7 +64,12 @@ struct b200zk_ctx {
   b200zk::DevBuf ws_zinv;     // 1/(5^n - 1) of the last quotient domain, canonical limbs (cached per log_n)
   uint32_t zinv_log_n = 0xffffffffu;
   // cudaFuncSetAttribute (opt-in to > 48 KiB dynamic shared memory) is per DEVICE: remembered per context, not per process
-  bool attr_sort = false, attr_acc = false, attr_ntt512 = false, attr_ntt256 = false;
+  bool attr_sort = false, attr_acc = false, attr_ntt512 = false, attr_ntt256 = false, attr_kzg = false;
+  // EIP-4844 proofs (bls381.cu): the blob domain's 4096 roots of unity in bit-reversed order, then 1/4096 (Fr381
+  // Montgomery), built once per context; consumers on other streams wait on kzg_roots_ready.  ws_kzg: blobs, z, quotients,
+  // partial sums and encoded results of one call
+  b200zk::DevBuf kzg_roots, ws_kzg;
+  cudaEvent_t kzg_roots_ready = nullptr;
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};

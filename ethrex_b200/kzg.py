@@ -7,14 +7,19 @@ and the L2 committer, crates/l2/sequencer/l1_committer.rs:1488-1521).
     compute_blob_kzg_proof(blob, commitment)   the same at the Fiat-Shamir challenge of EIP-4844
     blob_to_kzg_commitment_and_proof(blob)     what `BlobsBundle::create_from_blobs` calls per blob (wrapper version 0)
 
-The two MSMs run on the GPU (libb200zk.so, `b200zk_kzg_blob_to_commitment` / `b200zk_bls12_381_g1_msm_resident`); the scalar-
-field bookkeeping around them (4096 modular inverses, one SHA-256) is host work, exactly as it is CPU work in c-kzg.  The
+With a `Context` everything runs in libb200zk.so: the MSMs, and the scalar-field work of a proof (p(z), the quotient, its
+4096 inverses as one batch) in a CUDA kernel (`b200zk_kzg_compute_proof`, `b200zk_kzg_blob_to_commitment_and_proof`); the
+library hashes the challenge itself.  `compute_challenge` below is the same hash in Python, for callers that pass a
+commitment in.  KzgSettings also accepts a context object that serves only the two MSM calls (`kzg_blob_to_commitment`,
+`bls12_381_g1_msm_resident`); for such an object the proof's scalar-field work is done here in Python integers.  The
 trusted setup is an INPUT (4096 compressed G1 points in c-kzg's g1_lagrange_brp order): the reference gets it from inside the
 c-kzg / kzg-rs crates, which are not in the tree, so no setup is bundled here.  Cell proofs (wrapper version 1) are out of scope.
 """
 from __future__ import annotations
 
 import hashlib
+
+from .errors import B200Error
 
 BLS_MODULUS = 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001
 FIELD_ELEMENTS_PER_BLOB = 4096
@@ -67,10 +72,31 @@ class KzgSettings:
     def blobs_to_kzg_commitments(self, blobs) -> list:
         return self.ctx.kzg_blob_to_commitment(self.handle, b"".join(blobs)) if blobs else []
 
+    def _one_call(self) -> bool:
+        """a `Context` proves in one device call; an object that serves only the two MSM calls does not"""
+        return hasattr(self.ctx, "kzg_compute_proof")
+
     def compute_kzg_proof(self, blob: bytes, z: int):
-        """-> (proof 48 bytes, y = p(z)): the quotient (p(x) - y) / (x - z) in evaluation form, committed with one MSM"""
+        """-> (proof 48 bytes, y = p(z)): p(z) by the barycentric formula and the commitment of the quotient
+        (p(x) - y) / (x - z).  With a `Context` both are computed on the device (`b200zk_kzg_compute_proof`)."""
+        if not 0 <= z < BLS_MODULUS:
+            raise ValueError("field element out of range")
+        if not self._one_call():
+            return self._compose_proof(blob, z)
+        try:
+            proofs, ys = self.ctx.kzg_compute_proof(self.handle, blob, z.to_bytes(32, "big"))
+        except B200Error as e:
+            if e.status == 2:  # a blob element >= r (c-kzg: C_KZG_BADARGS)
+                raise ValueError("field element out of range") from e
+            raise
+        return proofs[0], int.from_bytes(ys[0], "big")
+
+    def _compose_proof(self, blob: bytes, z: int):
+        """For a context object that offers only `bls12_381_g1_msm_resident` and `kzg_blob_to_commitment` (the MSM calls):
+        the scalar-field work in Python integers, as c-kzg does it on the CPU, then one MSM over the quotient.  A `Context`
+        never takes this path."""
         poly = [int.from_bytes(blob[32 * i:32 * i + 32], "big") for i in range(FIELD_ELEMENTS_PER_BLOB)]
-        if any(v >= BLS_MODULUS for v in poly) or not 0 <= z < BLS_MODULUS:
+        if any(v >= BLS_MODULUS for v in poly):
             raise ValueError("field element out of range")
         roots = roots_of_unity_brp()
         r = BLS_MODULUS
@@ -83,8 +109,7 @@ class KzgSettings:
             for i, w in enumerate(roots):
                 if i == m:
                     continue
-                d = pow((w - z) % r, -1, r)
-                q[i] = (poly[i] - y) * d % r
+                q[i] = (poly[i] - y) * pow((w - z) % r, -1, r) % r
                 q[m] = (q[m] + (poly[i] - y) * w % r * zinv % r * pow((z - w) % r, -1, r)) % r
         else:
             # barycentric evaluation: p(z) = (z^n - 1)/n * sum_i p_i w_i / (z - w_i)
@@ -105,5 +130,18 @@ class KzgSettings:
         return self.compute_kzg_proof(blob, self.compute_challenge(blob, commitment))[0]
 
     def blob_to_kzg_commitment_and_proof(self, blob: bytes):
-        c = self.blob_to_kzg_commitment(blob)
-        return c, self.compute_blob_kzg_proof(blob, c)
+        """the commitment and the proof at the Fiat-Shamir challenge, in one device call"""
+        if not self._one_call():
+            c = self.blob_to_kzg_commitment(blob)
+            return c, self.compute_blob_kzg_proof(blob, c)
+        if len(blob) != BYTES_PER_BLOB:
+            raise ValueError("a blob is 131072 bytes")
+        commitments, proofs = self.ctx.kzg_blob_to_commitment_and_proof(self.handle, blob)
+        return commitments[0], proofs[0]
+
+    def blobs_to_kzg_commitments_and_proofs(self, blobs) -> tuple:
+        """([commitments], [proofs]) for a batch of blobs in one device call"""
+        if not self._one_call():
+            pairs = [self.blob_to_kzg_commitment_and_proof(b) for b in blobs]
+            return [c for c, _ in pairs], [p for _, p in pairs]
+        return self.ctx.kzg_blob_to_commitment_and_proof(self.handle, b"".join(blobs)) if blobs else ([], [])

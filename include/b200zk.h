@@ -312,6 +312,22 @@ int b200zk_bls12_381_g1_msm_resident(b200zk_ctx* ctx, uint64_t handle, const voi
  * commitments: n_blobs x 48 bytes */
 int b200zk_kzg_blob_to_commitment(b200zk_ctx* ctx, uint64_t setup_handle, const uint8_t* blobs, size_t n_blobs,
                                   uint8_t* commitments);
+/* EIP-4844 proofs, computed on the device: y = p(z) by the barycentric formula, the quotient (p(X) - y) / (X - z) in
+ * evaluation form (the spec's special case when z is one of the 4096 roots of unity), and its commitment.  Rules of both:
+ *   - setup_handle must be a BLS12-381 handle of exactly 4096 points, else status 4; null pointers with n_blobs > 0: 4;
+ *   - every blob element and every z must be < r.  All are checked before any MSM; a failure returns 2, writes no output,
+ *     and b200zk_last_error names the blob;
+ *   - n_blobs = 0 returns 0;
+ *   - an identity commitment or proof is encoded as 0xc0 | 0..0 and the status is still 0.
+ * blob_to_kzg_commitment_and_proof (/root/reference/crates/common/crypto/kzg.rs:259-272) for n_blobs blobs: the commitment,
+ * then the proof at the Fiat-Shamir challenge z = hash_to_bls_field(SHA-256("FSBLOBVERIFY_V1_" | 4096 as 16-byte big-endian
+ * | blob | commitment)).  The commitments are read back once for the hash (on the host), then the proofs are computed.
+ * commitments and proofs: n_blobs x 48 bytes compressed each. */
+int b200zk_kzg_blob_to_commitment_and_proof(b200zk_ctx* ctx, uint64_t setup_handle, const uint8_t* blobs, size_t n_blobs,
+                                            uint8_t* commitments, uint8_t* proofs);
+/* c-kzg compute_kzg_proof for n_blobs (blob, z) pairs: z and y are n_blobs x 32-byte big-endian; proofs n_blobs x 48 bytes */
+int b200zk_kzg_compute_proof(b200zk_ctx* ctx, uint64_t setup_handle, const uint8_t* blobs, size_t n_blobs,
+                             const uint8_t* z, uint8_t* proofs, uint8_t* y);
 
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:

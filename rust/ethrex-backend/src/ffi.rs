@@ -206,6 +206,26 @@ impl B200zk {
         check(self, status)?;
         Ok(out)
     }
+
+    /// `blob_to_kzg_commitment_and_proof` (kzg.rs:259-272) for a batch of blobs in one call: each blob is 4096 x 32-byte
+    /// big-endian field elements; `setup_handle` holds the 4096-point Lagrange-form setup.  Returns (commitments, proofs),
+    /// 48 bytes compressed each.
+    pub fn kzg_blob_to_commitment_and_proof(&mut self, setup_handle: u64, blobs: &[u8]) -> Result<(Vec<[u8; 48]>, Vec<[u8; 48]>), BackendError> {
+        const BLOB: usize = 4096 * 32;
+        if blobs.len() % BLOB != 0 {
+            return Err(BackendError::serialization("kzg_blob_to_commitment_and_proof: a blob is 4096 x 32 bytes"));
+        }
+        let n = blobs.len() / BLOB;
+        let mut commitments = vec![[0u8; 48]; n];
+        let mut proofs = vec![[0u8; 48]; n];
+        // SAFETY: `blobs` holds n blobs; both outputs hold n x 48 contiguous bytes; the call is synchronous.
+        let status = unsafe {
+            sys::b200zk_kzg_blob_to_commitment_and_proof(self.ctx.as_ptr(), setup_handle, blobs.as_ptr(), n, commitments.as_mut_ptr().cast(),
+                                                         proofs.as_mut_ptr().cast())
+        };
+        check(self, status)?;
+        Ok((commitments, proofs))
+    }
 }
 
 /// Per-item outcome of the batched precompile calls (include/b200zk.h: 0 ok, 1 ok-identity, 2 coordinate >= p,
