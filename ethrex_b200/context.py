@@ -345,6 +345,53 @@ class Context:
         self._check(F.lib.b200zk_kzg_compute_proof(self._h, setup_handle, bp, k, zp, pr, y), "b200zk_kzg_compute_proof")
         return [pr.raw[48 * i:48 * i + 48] for i in range(k)], [y.raw[32 * i:32 * i + 32] for i in range(k)]
 
+    # ------------------------------------------------------------------ BLS12-381 pairing / EIP-4844 KZG verification
+    def bls12_381_g2_bases_upload(self, points, n: int, flags: int = F.POINTS_COMPRESSED) -> int:
+        """points: n x 96 bytes compressed G2 (the trusted setup's g2_monomial form); subgroup-checked"""
+        _need(points, 96 * n, "b200zk_bls12_381_g2_bases_upload points")
+        pp, keep = _host_ptr(points)
+        h = C.c_uint64()
+        self._check(F.lib.b200zk_bls12_381_g2_bases_upload(self._h, pp, n, flags, C.byref(h)), "b200zk_bls12_381_g2_bases_upload")
+        return h.value
+
+    def bls12_381_pairing_check_batch(self, checks):
+        """checks: list of EIP-2537 pairing calldata byte strings (k*384 bytes each) -> ([result 0/1], [status])"""
+        offs, blob = [0], bytearray()
+        for cd in checks:
+            if len(cd) % 384:
+                raise B200Error.serialization("bls12 pairing input must be a multiple of 384 bytes")
+            blob += cd
+            offs.append(len(blob) // 384)
+        count = len(checks)
+        offsets = np.asarray(offs, dtype=np.uint32)
+        res, st = C.create_string_buffer(max(1, count)), C.create_string_buffer(max(1, count))
+        pairs = np.frombuffer(bytes(blob) or b"\0", dtype=np.uint8)
+        self._check(F.lib.b200zk_bls12_381_pairing_check_batch(self._h, pairs.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p),
+                                                              count, res, st), "b200zk_bls12_381_pairing_check_batch")
+        return list(res.raw[:count]), list(st.raw[:count])
+
+    def kzg_verify_proof_batch(self, g2_setup: int, commitments, z, y, proofs) -> tuple:
+        """n items: commitments and proofs n x 48 bytes, z and y n x 32-byte big-endian -> ([result 0/1], [status])"""
+        n = _host_len(commitments) // 48
+        _need(z, 32 * n, "b200zk_kzg_verify_proof_batch z")
+        _need(y, 32 * n, "b200zk_kzg_verify_proof_batch y")
+        _need(proofs, 48 * n, "b200zk_kzg_verify_proof_batch proofs")
+        bufs = [_host_ptr(b) for b in (commitments, z, y, proofs)]
+        res, st = C.create_string_buffer(max(1, n)), C.create_string_buffer(max(1, n))
+        self._check(F.lib.b200zk_kzg_verify_proof_batch(self._h, g2_setup, *[p for p, _ in bufs], n, res, st), "b200zk_kzg_verify_proof_batch")
+        return list(res.raw[:n]), list(st.raw[:n])
+
+    def kzg_verify_blob_proof_batch(self, g2_setup: int, blobs, commitments, proofs) -> bool:
+        """blobs: k x 131072 bytes, commitments and proofs k x 48 bytes -> one bool for the batch"""
+        k = self._blob_count(blobs)
+        _need(commitments, 48 * k, "b200zk_kzg_verify_blob_proof_batch commitments")
+        _need(proofs, 48 * k, "b200zk_kzg_verify_blob_proof_batch proofs")
+        bufs = [_host_ptr(b) if _host_len(b) else (None, None) for b in (blobs, commitments, proofs)]
+        valid = C.c_int(-1)
+        self._check(F.lib.b200zk_kzg_verify_blob_proof_batch(self._h, g2_setup, *[p for p, _ in bufs], k, C.byref(valid)),
+                    "b200zk_kzg_verify_blob_proof_batch")
+        return valid.value == 1
+
     # ------------------------------------------------------------------ NTT root of unity (SURVEY.md section 8c)
     NTT_ROOT_ARK, NTT_ROOT_HALO2 = 0, 1
 

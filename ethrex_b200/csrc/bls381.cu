@@ -7,21 +7,12 @@
 // returned in the 48-byte compressed format.  The MSM itself is msm.cu instantiated over Fp381 (window tables included).
 // The proof (c-kzg compute_kzg_proof / compute_blob_kzg_proof) evaluates p at z and builds the quotient on the device
 // (kzg_eval_quotient, over the scalar field Fr381), then commits to it with the same MSM.
-#include "common.cuh"
+#include "bls12.cuh"
 #include "sha256.h"
 #include <cstring>
 #include <vector>
 
 namespace b200zk {
-
-B2_D Fp381 load_be48(const uint8_t* in, uint32_t clear_top_mask) {
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(in);
-  Fp381 v;
-#pragma unroll
-  for (int k = 0; k < 12; ++k) v.v[k] = __byte_perm(__ldg(w + 11 - k), 0, 0x0123);
-  v.v[11] &= clear_top_mask;
-  return v;
-}
 
 // status[0] = first index whose coordinate is >= p, status[1] = first index that is not a curve point or whose flag bits
 // are inconsistent (atomicMin; initialised to n by the host)
@@ -33,28 +24,12 @@ __global__ void __launch_bounds__(64) bls_g1_decode(const uint8_t* __restrict__ 
   const bool c_flag = flags & 0x80, inf_flag = flags & 0x40, sign_flag = flags & 0x20;
   Affine<Fp381> pt = {Fp381::zero(), Fp381::zero()};
   bool bad_field = false, bad_point = false;
-  Fp381 x = load_be48(src, 0x1fffffffu);
   if (compressed) {
-    if (!c_flag) bad_point = true;
-    else if (inf_flag) { if (sign_flag || !x.is_zero()) bad_point = true; }
-    else {
-      if (!Fp381::less(x, Fp381::modulus())) bad_field = true;
-      else {
-        const Fp381 xm = Fp381::to_mont(x);
-        const Fp381 rhs = Fp381::add(Fp381::mul(Fp381::sqr(xm), xm), CurveB<Fp381>::b());
-        Fp381 y = Fp381::sqrt_candidate(rhs);
-        if (Fp381::sqr(y) != rhs) bad_point = true;  // x^3 + 4 is not a square: no such point
-        else {
-          Fp381 half;
-#pragma unroll
-          for (int k = 0; k < 12; ++k) half.v[k] = Fp381Cfg::half(k);
-          const bool largest = Fp381::less(half, Fp381::from_mont(y));
-          if (largest != sign_flag) y = Fp381::neg(y);
-          pt = {xm, y};
-        }
-      }
-    }
+    const uint32_t st = bls_g1_decompress(src, &pt);
+    bad_field = st == B200ZK_ERR_NOT_IN_FIELD;
+    bad_point = st == B200ZK_ERR_NOT_ON_CURVE;
   } else {  // uncompressed: x | y big-endian, flag bits must be clear except infinity
+    const Fp381 x = load_be48(src, 0x1fffffffu);
     Fp381 y = load_be48(src + 48, 0xffffffffu);
     if (c_flag || sign_flag) bad_point = true;
     else if (inf_flag) { if (!x.is_zero() || !y.is_zero()) bad_point = true; }
@@ -90,13 +65,6 @@ constexpr uint32_t kBlobN = 4096;      // FIELD_ELEMENTS_PER_BLOB
 constexpr uint32_t kEvalThreads = 256;  // one CTA per blob, 16 elements per thread: element k * 256 + t belongs to thread t
 constexpr size_t kEvalSmem = (kBlobN + 2 * kEvalThreads) * 32;  // per-element products / inverses + a 512-node product tree
 
-B2_D Fr381 load_be32(const uint8_t* in) {  // 32-byte big-endian integer -> canonical limbs
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(in);
-  Fr381 v;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) v.v[k] = __byte_perm(__ldg(w + 7 - k), 0, 0x0123);
-  return v;
-}
 B2_D void store_be32(uint8_t* out, const Fr381& canonical) {
   uint32_t* o = reinterpret_cast<uint32_t*>(out);
 #pragma unroll
@@ -330,13 +298,7 @@ int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_
 
 // z of every blob in L.z, checked: y into L.y, the proofs' encodings into enc
 int kzg_proofs(b200zk_ctx* ctx, const BasesEntry& e, const KzgLayout& L, size_t n, uint8_t* enc, cudaStream_t st) {
-  const void* roots = nullptr;
-  B2_TRY(kzg_roots(ctx, st, &roots));
-  if (!ctx->attr_kzg) {
-    B2_CUDA(ctx, cudaFuncSetAttribute(kzg_eval_quotient, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEvalSmem));
-    ctx->attr_kzg = true;
-  }
-  B2_LAUNCH(ctx, kzg_eval_quotient, (unsigned)n, kEvalThreads, kEvalSmem, st, (const uint8_t*)L.blobs, (const uint8_t*)L.z, roots, (void*)L.q, L.y);
+  B2_TRY(kzg_eval_run(ctx, L.blobs, L.z, n, L.q, L.y, st));
   return kzg_msms(ctx, e, L.q, n, 0 /* little-endian limbs */, L.partials + n * KzgLayout::kPartial, enc, st);
 }
 
@@ -344,15 +306,16 @@ int kzg_proofs(b200zk_ctx* ctx, const BasesEntry& e, const KzgLayout& L, size_t 
 int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e) {
   auto it = ctx->bases.find(handle);
   std::string msg = what;
-  if (it == ctx->bases.end() || !it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": unknown setup handle").c_str());
+  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": unknown setup handle").c_str());
   if (it->second.n != kBlobN) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points").c_str());
   *e = &it->second;
   return B200ZK_OK;
 }
 
-// EIP-4844 compute_challenge: hash_to_bls_field(SHA-256("FSBLOBVERIFY_V1_" | 4096 as 16-byte big-endian | blob | commitment)),
-// the digest read as a big-endian integer and reduced mod r (< 2^256 < 3r: at most two subtractions)
-void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]) {
+}  // namespace
+
+// EIP-4844 compute_challenge: hash_to_bls_field(SHA-256("FSBLOBVERIFY_V1_" | 4096 as 16-byte big-endian | blob | commitment))
+void b200zk::kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]) {
   static const uint8_t kDomain[16] = {'F', 'S', 'B', 'L', 'O', 'B', 'V', 'E', 'R', 'I', 'F', 'Y', '_', 'V', '1', '_'};
   uint8_t degree[16] = {};
   degree[14] = kBlobN >> 8;
@@ -363,6 +326,11 @@ void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_
   h.update(commitment, 48);
   uint8_t d[32];
   h.final(d);
+  hash_to_bls_field(d, z_be);
+}
+
+// the digest read as a big-endian integer and reduced mod r (< 2^256 < 3r: at most two subtractions)
+void b200zk::hash_to_bls_field(const uint8_t d[32], uint8_t z_be[32]) {
   uint32_t v[8];
   for (int k = 0; k < 8; ++k) v[k] = (uint32_t)d[31 - 4 * k] | (uint32_t)d[30 - 4 * k] << 8 | (uint32_t)d[29 - 4 * k] << 16 | (uint32_t)d[28 - 4 * k] << 24;
   for (int pass = 0; pass < 2; ++pass) {
@@ -374,7 +342,18 @@ void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_
   for (int k = 0; k < 8; ++k)
     for (int j = 0; j < 4; ++j) z_be[31 - 4 * k - j] = (uint8_t)(v[k] >> (8 * j));
 }
-}  // namespace
+
+// y = p(z) of n blobs (kzg_eval_quotient, one CTA per blob); the quotient goes to q (n x 4096 x 32 bytes)
+int b200zk::kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st) {
+  const void* roots = nullptr;
+  B2_TRY(kzg_roots(ctx, st, &roots));
+  if (!ctx->attr_kzg) {
+    B2_CUDA(ctx, cudaFuncSetAttribute(kzg_eval_quotient, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEvalSmem));
+    ctx->attr_kzg = true;
+  }
+  B2_LAUNCH(ctx, kzg_eval_quotient, (unsigned)n, kEvalThreads, kEvalSmem, st, d_blobs, d_z, roots, d_q, d_y);
+  return B200ZK_OK;
+}
 
 extern "C" {
 
@@ -401,7 +380,7 @@ int b200zk_bls12_381_g1_msm_resident(b200zk_ctx* ctx, uint64_t handle, const voi
   if (!ctx || !out || (!scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: null argument");
   DeviceGuard guard(ctx);
   auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || !it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: unknown handle");
+  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: unknown handle");
   if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: n exceeds the resident bases");
   return bls_msm_host_scalars(ctx, it->second, scalars, n, flags, ctx->stream, out);
 }
@@ -410,7 +389,7 @@ int b200zk_kzg_blob_to_commitment(b200zk_ctx* ctx, uint64_t setup_handle, const 
   if (!ctx || (n_blobs && (!blobs || !commitments))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: null argument");
   DeviceGuard guard(ctx);
   auto it = ctx->bases.find(setup_handle);
-  if (it == ctx->bases.end() || !it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: unknown setup handle");
+  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: unknown setup handle");
   if (it->second.n != 4096) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: the setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
   for (size_t b = 0; b < n_blobs; ++b) {
     int rc = bls_msm_host_scalars(ctx, it->second, blobs + b * 4096 * 32, 4096, B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW, ctx->stream, commitments + 48 * b);

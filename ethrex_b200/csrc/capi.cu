@@ -218,6 +218,7 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   if (ctx->ws_cnt2.p) cudaFree(ctx->ws_cnt2.p);
   if (ctx->kzg_roots.p) cudaFree(ctx->kzg_roots.p);
   if (ctx->ws_kzg.p) cudaFree(ctx->ws_kzg.p);
+  if (ctx->ws_pairing.p) cudaFree(ctx->ws_pairing.p);
   if (ctx->kzg_roots_ready) cudaEventDestroy(ctx->kzg_roots_ready);
   DevBuf* bufs[] = {&ctx->ws_hist, &ctx->ws_offsets, &ctx->ws_cursor, &ctx->ws_blocksums, &ctx->ws_idx, &ctx->ws_buckets, &ctx->ws_chunkS,
                     &ctx->ws_chunkV, &ctx->ws_result, &ctx->ws_points, &ctx->ws_scalars, &ctx->ws_ntt, &ctx->ws_misc, &ctx->ws_out, &ctx->ws_segoff, &ctx->ws_segbucket, &ctx->ws_digits, &ctx->ws_q0, &ctx->ws_q1, &ctx->ws_prefix, &ctx->ws_info, &ctx->ws_pairoff0, &ctx->ws_pairoff1};
@@ -307,6 +308,7 @@ int b200zk_bases_precompute(b200zk_ctx* ctx, uint64_t handle, uint32_t window_bi
   if (it == ctx->bases.end()) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: unknown handle");
   if (window_bits && (window_bits < 2 || window_bits > 24)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: window must be 0 or 2..24");
   BasesEntry& e = it->second;
+  if (e.bls && e.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: BLS12-381 G2 handles are pairing inputs, not MSM bases");
   if (e.table_c) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: handle already precomputed");
   const uint32_t c = window_bits ? window_bits : precompute_window(e.n);
   const uint32_t W = ((e.bls ? 256u : 255u) + c - 1) / c;  // ScalarBits<F>: BLS12-381's group order has one more bit

@@ -40,7 +40,9 @@ struct BasesEntry {
   void* d = nullptr;
   size_t n = 0;
   bool g2 = false;
-  bool bls = false;      // BLS12-381 G1 points (Fp381 Montgomery, 96 B affine): the KZG trusted setup
+  bool bls = false;      // BLS12-381 points: G1 (Fp381 Montgomery, 96 B affine), the KZG trusted setup; with g2 set, G2
+                         // (Fp2 over Fp381, 192 B affine), followed by the prepared Miller-loop lines of points 0 and 1
+  bool g2_gen0 = false;  // BLS12-381 G2: point 0 is the generator (so point 1 is [tau]2 of a KZG setup)
   uint32_t table_c = 0;  // != 0: d holds W = ceil(255/c) windows of n points: 2^(c*w) * P_i at w*n + i
 };
 
@@ -70,6 +72,7 @@ struct b200zk_ctx {
   // partial sums and encoded results of one call
   b200zk::DevBuf kzg_roots, ws_kzg;
   cudaEvent_t kzg_roots_ready = nullptr;
+  b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
@@ -266,5 +269,10 @@ int groth16_assemble_zk_dev(b200zk_ctx* ctx, const void* d_partials, size_t coun
 int bn254_g1_add_batch(b200zk_ctx* ctx, const uint8_t* a, const uint8_t* b, size_t count, uint8_t* out, uint8_t* status);
 int bn254_g1_mul_batch(b200zk_ctx* ctx, const uint8_t* points, const uint8_t* scalars, size_t count, uint8_t* out, uint8_t* status);
 int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint32_t* pair_offsets, size_t count, uint8_t* result, uint8_t* status);
+// EIP-4844 (bls381.cu): the Fiat-Shamir challenge of one blob, the digest-to-field reduction, and y = p(z) of n blobs on the
+// device (the quotient goes to d_q, n x 4096 x 32 bytes of scratch)
+void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]);
+void hash_to_bls_field(const uint8_t digest[32], uint8_t out_be[32]);
+int kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st);
 
 }  // namespace b200zk

@@ -14,6 +14,10 @@ commitment in.  KzgSettings also accepts a context object that serves only the t
 `bls12_381_g1_msm_resident`); for such an object the proof's scalar-field work is done here in Python integers.  The
 trusted setup is an INPUT (4096 compressed G1 points in c-kzg's g1_lagrange_brp order): the reference gets it from inside the
 c-kzg / kzg-rs crates, which are not in the tree, so no setup is bundled here.  Cell proofs (wrapper version 1) are out of scope.
+
+Verification (verify_kzg_proof, verify_blob_kzg_proof, verify_blob_kzg_proof_batch) needs the setup's G2 points as well
+(`g2_monomial`: at least [1]2 and [tau]2, 96-byte compressed) and a `Context`: the pairing runs on the device
+(`b200zk_kzg_verify_proof_batch`, `b200zk_kzg_verify_blob_proof_batch`).
 """
 from __future__ import annotations
 
@@ -50,18 +54,26 @@ def roots_of_unity_brp():
 class KzgSettings:
     """The trusted setup resident in HBM (the reference's `c_kzg::ethereum_kzg_settings(KZG_PRECOMPUTE)`, kzg.rs:262)."""
 
-    def __init__(self, ctx, g1_lagrange_brp: bytes, precompute: bool = True):
+    def __init__(self, ctx, g1_lagrange_brp: bytes, precompute: bool = True, g2_monomial: bytes | None = None):
         if len(g1_lagrange_brp) != 48 * FIELD_ELEMENTS_PER_BLOB:
             raise ValueError("the setup is 4096 compressed G1 points (48 bytes each) in g1_lagrange_brp order")
+        if g2_monomial is not None and (len(g2_monomial) % 96 or len(g2_monomial) < 2 * 96):
+            raise ValueError("g2_monomial is at least 2 compressed G2 points (96 bytes each): [1]2, [tau]2, ...")
         self.ctx = ctx
+        self.g2_handle = 0
         self.handle = ctx.bls12_381_g1_bases_upload(g1_lagrange_brp, FIELD_ELEMENTS_PER_BLOB)
         if precompute:
             ctx.bases_precompute(self.handle, 0)
+        if g2_monomial is not None:
+            self.g2_handle = ctx.bls12_381_g2_bases_upload(g2_monomial, len(g2_monomial) // 96)
 
     def close(self):
         if self.handle:
             self.ctx.bases_free(self.handle)
             self.handle = 0
+        if self.g2_handle:
+            self.ctx.bases_free(self.g2_handle)
+            self.g2_handle = 0
 
     # ---- kzg.rs:259-272
     def blob_to_kzg_commitment(self, blob: bytes) -> bytes:
@@ -145,3 +157,41 @@ class KzgSettings:
             pairs = [self.blob_to_kzg_commitment_and_proof(b) for b in blobs]
             return [c for c, _ in pairs], [p for _, p in pairs]
         return self.ctx.kzg_blob_to_commitment_and_proof(self.handle, b"".join(blobs)) if blobs else ([], [])
+
+    # ---- verification: provider.rs:463-544, kzg.rs:168-192
+    def _verifier(self) -> int:
+        if not hasattr(self.ctx, "kzg_verify_proof_batch"):
+            raise TypeError("KZG verification runs on the device: KzgSettings needs a Context")
+        if not self.g2_handle:
+            raise ValueError("KZG verification needs the setup's G2 points: pass g2_monomial")
+        return self.g2_handle
+
+    def verify_kzg_proof(self, commitment: bytes, z, y, proof: bytes) -> bool:
+        """c-kzg verify_kzg_proof: does `proof` open `commitment` to y at z?  z, y: ints or 32-byte big-endian.  Raises
+        ValueError on malformed input (c-kzg's C_KZG_BADARGS): z or y >= r, or an invalid commitment or proof."""
+        h = self._verifier()
+        zb, yb = (v.to_bytes(32, "big") if isinstance(v, int) else bytes(v) for v in (z, y))
+        if len(commitment) != 48 or len(proof) != 48 or len(zb) != 32 or len(yb) != 32:
+            raise ValueError("commitment and proof are 48 bytes, z and y 32 bytes")
+        res, st = self.ctx.kzg_verify_proof_batch(h, commitment, zb, yb, proof)
+        if st[0] in (2, 3):
+            raise ValueError("field element out of range" if st[0] == 2 else "invalid commitment or proof")
+        return res[0] == 1
+
+    def verify_blob_kzg_proof(self, blob: bytes, commitment: bytes, proof: bytes) -> bool:
+        """c-kzg verify_blob_kzg_proof: a batch of one"""
+        return self.verify_blob_kzg_proof_batch([blob], [commitment], [proof])
+
+    def verify_blob_kzg_proof_batch(self, blobs, commitments, proofs) -> bool:
+        """c-kzg verify_blob_kzg_proof_batch: one answer for the batch; ValueError on malformed input"""
+        h = self._verifier()
+        if not len(blobs) == len(commitments) == len(proofs):
+            raise ValueError("blobs, commitments and proofs differ in length")
+        if any(len(b) != BYTES_PER_BLOB for b in blobs) or any(len(c) != 48 for c in commitments) or any(len(p) != 48 for p in proofs):
+            raise ValueError("a blob is 131072 bytes, a commitment and a proof 48 bytes")
+        try:
+            return self.ctx.kzg_verify_blob_proof_batch(h, b"".join(blobs), b"".join(commitments), b"".join(proofs))
+        except B200Error as e:
+            if e.status in (2, 3):
+                raise ValueError(str(e)) from e
+            raise

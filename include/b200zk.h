@@ -329,6 +329,45 @@ int b200zk_kzg_blob_to_commitment_and_proof(b200zk_ctx* ctx, uint64_t setup_hand
 int b200zk_kzg_compute_proof(b200zk_ctx* ctx, uint64_t setup_handle, const uint8_t* blobs, size_t n_blobs,
                              const uint8_t* z, uint8_t* proofs, uint8_t* y);
 
+/* ---- the BLS12-381 pairing and EIP-4844 KZG verification ----------------------------------------------------------
+ * The three reference calls that rest on a BLS12-381 pairing:
+ *   bls12_381_pairing_check   Crypto::bls12_381_pairing_check (EIP-2537 pairing precompile 0x0f), provider.rs:642-672
+ *   kzg_verify_proof          Crypto::verify_kzg_proof (POINT_EVALUATION precompile 0x0a), provider.rs:463-507
+ *   kzg_verify_blob_proof     Crypto::verify_blob_kzg_proof / kzg::verify_kzg_proof_batch (blob transactions),
+ *                             provider.rs:509-544, crates/common/crypto/kzg.rs:168-192
+ * The pairing is the optimal ate pairing with line coefficients prepared per G2 point; a check asks whether a product of
+ * pairings is one.
+ *
+ * G2 bases: n points in the 96-byte compressed ZCash form (the trusted setup's g2_monomial): x.c1 | x.c0 big-endian, flag
+ * bits in byte 0 (bit 7 compressed, bit 6 infinity, bit 5 the larger y: y.c1 > (p-1)/2, or y.c1 = 0 and y.c0 > (p-1)/2).
+ * B200ZK_POINTS_COMPRESSED is required (status 4 otherwise).  Status 2: x.c0 or x.c1 >= p; 3: bad flag bits, not on the
+ * twist y^2 = x^3 + 4(1 + u), or not in the order-r subgroup (checked here, unlike G1 bases: a non-subgroup [tau]2 would
+ * make the verifier unsound).  The handle is freed by b200zk_bases_free; every MSM entry point, b200zk_bases_precompute
+ * and the BLS12-381 G1 / KZG prove calls refuse it with status 4. */
+int b200zk_bls12_381_g2_bases_upload(b200zk_ctx* ctx, const void* points, size_t n, uint32_t flags, uint64_t* handle);
+/* The EIP-2537 pairing check, `count` checks per call.  Check i covers pairs [pair_offsets[i], pair_offsets[i+1]) of
+ * `pairs`, 384 bytes each: G1 (128 B, x | y) then G2 (256 B, x.c0 | x.c1 | y.c0 | y.c1); every Fp is 64 bytes, 16 zero
+ * bytes then 48 bytes big-endian; all-zero is the identity.  Per check: status[i] = 2 when a coordinate is >= p or a
+ * padding byte is nonzero (checked for every point of the check before any curve check), 3 when a point is not on its
+ * curve or not in the order-r subgroup (G1 and G2 both); result[i] = 1 when the product of its pairings is one (an empty
+ * check, and pairs with an identity side, contribute 1), 0 otherwise or when status[i] != 0. */
+int b200zk_bls12_381_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 384 B each */, const uint32_t* pair_offsets /* count+1 */,
+                                         size_t count, uint8_t* result /* count */, uint8_t* status /* count */);
+/* KZG verification against a G2 setup handle: a BLS12-381 G2 handle of at least 2 points whose point 0 is the G2 generator;
+ * point 1 is [tau]2.  Anything else returns 4.
+ * c-kzg verify_kzg_proof for n independent items: commitment and proof 48-byte compressed G1, z and y 32-byte big-endian.
+ * Per item: status[i] = 2 when z or y >= r or a coordinate >= p, 3 when a commitment or proof has bad flag bits, is off the
+ * curve or not in the order-r subgroup (c-kzg validate_kzg_g1; the identity is valid); result[i] = 1 when the proof is
+ * valid.  A failed item reports 0 and does not affect the others. */
+int b200zk_kzg_verify_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint8_t* commitments /* 48 n */, const uint8_t* z /* 32 n */,
+                                  const uint8_t* y /* 32 n */, const uint8_t* proofs /* 48 n */, size_t n, uint8_t* result /* n */,
+                                  uint8_t* status /* n */);
+/* c-kzg verify_blob_kzg_proof_batch: one answer for n (blob, commitment, proof) triples, *valid = 1 or 0.  Bad input is an
+ * error, not 0: a blob element >= r returns 2, a malformed or non-subgroup commitment or proof 2 or 3 as above; then
+ * *valid is not written and b200zk_last_error names the blob.  n = 0 returns 0 with *valid = 1. */
+int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint8_t* blobs, const uint8_t* commitments,
+                                       const uint8_t* proofs, size_t n, int* valid);
+
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:
  *   bn254_g1_add         crates/common/crypto/provider.rs:201-234   (levm ecadd,     crates/vm/levm/src/precompiles.rs:692-716)

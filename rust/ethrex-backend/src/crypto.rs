@@ -1,5 +1,5 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
-//! (`crates/common/crypto/provider.rs:201-330`) on the GPU.  The trait is one item per call; a provider that wants
+//! (`crates/common/crypto/provider.rs:201-330`) and its BLS12-381 pairing check (`provider.rs:642-672`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
 //!
@@ -58,6 +58,25 @@ impl Crypto for B200Crypto {
         match res.first() {
             Some(Ok(v)) => Ok(*v),
             Some(Err(bad)) => Err(item_error(*bad, "G1/G2 not on BN254 curve")),
+            None => Err(CryptoError::Other("b200zk returned no result".to_string())),
+        }
+    }
+
+    /// The trait passes 48-byte big-endian coordinates (G2: x.c0, x.c1, y.c0, y.c1); the device call takes the EIP-2537
+    /// 64-byte form, so each is re-padded with 16 leading zero bytes.  No setup is needed.
+    fn bls12_381_pairing_check(&self, pairs: &[(([u8; 48], [u8; 48]), ([u8; 48], [u8; 48], [u8; 48], [u8; 48]))]) -> Result<bool, CryptoError> {
+        let mut calldata = Vec::with_capacity(pairs.len().saturating_mul(384));
+        for ((x, y), (x0, x1, y0, y1)) in pairs {
+            for fp in [x, y, x0, x1, y0, y1] {
+                calldata.extend_from_slice(&[0u8; 16]);
+                calldata.extend_from_slice(fp);
+            }
+        }
+        let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+        let res = gpu.bls12_381_pairing_check_batch(&[calldata.as_slice()]).map_err(device_error)?;
+        match res.first() {
+            Some(Ok(v)) => Ok(*v),
+            Some(Err(bad)) => Err(item_error(*bad, "G1/G2 not on the BLS12-381 curve or not in the subgroup")),
             None => Err(CryptoError::Other("b200zk returned no result".to_string())),
         }
     }

@@ -309,6 +309,89 @@ impl B200zk {
             })
             .collect())
     }
+
+    /// Several EIP-2537 pairing checks in one launch.  `checks[i]` is the precompile's calldata (k x 384 bytes:
+    /// G1 128 B | G2 256 B, every Fp as 16 zero bytes + 48 bytes big-endian).  Per check `Ok(true/false)` or the input error.
+    pub fn bls12_381_pairing_check_batch(&mut self, checks: &[&[u8]]) -> Result<Vec<Result<bool, ItemStatus>>, BackendError> {
+        let mut blob = Vec::new();
+        let mut offsets = Vec::with_capacity(checks.len().saturating_add(1));
+        offsets.push(0u32);
+        for cd in checks {
+            if cd.len() % 384 != 0 {
+                return Err(BackendError::serialization("bls12_381_pairing_check_batch: calldata must be a multiple of 384 bytes"));
+            }
+            blob.extend_from_slice(cd);
+            let pairs = u32::try_from(blob.len() / 384).map_err(|_| BackendError::serialization("bls12_381_pairing_check_batch: too many pairs"))?;
+            offsets.push(pairs);
+        }
+        let count = checks.len();
+        let mut res = vec![0u8; count];
+        let mut st = vec![0u8; count];
+        // SAFETY: `offsets` has count + 1 entries, `blob` holds offsets[count] pairs, outputs hold `count` bytes.
+        let status = unsafe {
+            sys::b200zk_bls12_381_pairing_check_batch(self.ctx.as_ptr(), blob.as_ptr(), offsets.as_ptr(), count, res.as_mut_ptr(), st.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(res
+            .into_iter()
+            .zip(st)
+            .map(|(r, s)| match ItemStatus::from_code(s) {
+                ItemStatus::Ok | ItemStatus::OkIdentity => Ok(r == 1),
+                bad => Err(bad),
+            })
+            .collect())
+    }
+
+    /// Upload a KZG setup's G2 points (96-byte compressed, `g2_monomial` order: [1]2, [tau]2, ...), subgroup-checked.
+    /// The handle is what the two KZG verify calls take; free it with `bases_free`.
+    pub fn bls12_381_g2_bases_upload(&mut self, points: &[u8]) -> Result<u64, BackendError> {
+        if points.len() % 96 != 0 {
+            return Err(BackendError::serialization("bls12_381_g2_bases_upload: points are 96 bytes each"));
+        }
+        let mut handle = 0u64;
+        // SAFETY: `points` holds len/96 compressed points; `handle` is a valid out pointer.
+        let status = unsafe { sys::b200zk_bls12_381_g2_bases_upload(self.ctx.as_ptr(), points.as_ptr().cast(), points.len() / 96, sys::B200ZK_POINTS_COMPRESSED, &mut handle) };
+        check(self, status)?;
+        Ok(handle)
+    }
+
+    /// c-kzg `verify_kzg_proof` for n items (commitments and proofs n x 48 bytes, z and y n x 32 bytes big-endian):
+    /// per item `Ok(valid)` or the input error (c-kzg's BADARGS).
+    pub fn kzg_verify_proof_batch(&mut self, g2_setup: u64, commitments: &[u8], z: &[u8], y: &[u8], proofs: &[u8]) -> Result<Vec<Result<bool, ItemStatus>>, BackendError> {
+        let n = commitments.len() / 48;
+        if commitments.len() % 48 != 0 || proofs.len() != 48 * n || z.len() != 32 * n || y.len() != 32 * n {
+            return Err(BackendError::serialization("kzg_verify_proof_batch: need 48 + 32 + 32 + 48 bytes per item"));
+        }
+        let mut res = vec![0u8; n];
+        let mut st = vec![0u8; n];
+        // SAFETY: every input holds n items of its size, outputs hold n bytes.
+        let status = unsafe {
+            sys::b200zk_kzg_verify_proof_batch(self.ctx.as_ptr(), g2_setup, commitments.as_ptr(), z.as_ptr(), y.as_ptr(), proofs.as_ptr(), n, res.as_mut_ptr(), st.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(res
+            .into_iter()
+            .zip(st)
+            .map(|(r, s)| match ItemStatus::from_code(s) {
+                ItemStatus::Ok | ItemStatus::OkIdentity => Ok(r == 1),
+                bad => Err(bad),
+            })
+            .collect())
+    }
+
+    /// c-kzg `verify_blob_kzg_proof_batch`: one answer for n (blob, commitment, proof) triples; malformed input is an error.
+    pub fn kzg_verify_blob_proof_batch(&mut self, g2_setup: u64, blobs: &[u8], commitments: &[u8], proofs: &[u8]) -> Result<bool, BackendError> {
+        const BLOB: usize = 4096 * 32;
+        let n = blobs.len() / BLOB;
+        if blobs.len() % BLOB != 0 || commitments.len() != 48 * n || proofs.len() != 48 * n {
+            return Err(BackendError::serialization("kzg_verify_blob_proof_batch: need 131072 + 48 + 48 bytes per blob"));
+        }
+        let mut valid: core::ffi::c_int = 0;
+        // SAFETY: every input holds n items of its size; `valid` is a valid out pointer.
+        let status = unsafe { sys::b200zk_kzg_verify_blob_proof_batch(self.ctx.as_ptr(), g2_setup, blobs.as_ptr(), commitments.as_ptr(), proofs.as_ptr(), n, &mut valid) };
+        check(self, status)?;
+        Ok(valid == 1)
+    }
 }
 
 impl Drop for B200zk {
