@@ -110,6 +110,10 @@ SIGNATURES = {
     "b200zk_bls12_381_pairing_check_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_kzg_verify_proof_batch": (_int, [_ctx, _u64, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_kzg_verify_blob_proof_batch": (_int, [_ctx, _u64, _vp, _vp, _vp, _sz, C.POINTER(_int)]),
+    "b200zk_bls12_381_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_bls12_381_g2_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_bls12_381_g1_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_bls12_381_g2_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_g1_mul_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_pairing_check_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

@@ -370,6 +370,49 @@ class Context:
                                                               count, res, st), "b200zk_bls12_381_pairing_check_batch")
         return list(res.raw[:count]), list(st.raw[:count])
 
+    # ------------------------------------------------------------------ EIP-2537 addition and MSM (precompiles 0x0b-0x0e)
+    # Twins of Crypto::bls12_381_{g1,g2}_{add,msm} (/root/reference/crates/common/crypto/provider.rs:549-640); EIP-2537
+    # encodings and per-item status as in include/b200zk.h.
+    def _bls12_add(self, fn, what: str, a, b, size: int):
+        if len(a) != len(b) or len(a) % size:
+            raise B200Error.serialization(f"{what}: inputs must be equal multiples of {size} bytes")
+        count = len(a) // size
+        out, st = C.create_string_buffer(max(1, size * count)), C.create_string_buffer(max(1, count))
+        pa, k1 = _host_ptr(a)
+        pb, k2 = _host_ptr(b)
+        self._check(fn(self._h, pa, pb, count, out, st), what)
+        return out.raw[:size * count], list(st.raw[:count])
+
+    def _bls12_msm(self, fn, what: str, calls, pair: int, size: int):
+        offs, blob = [0], bytearray()
+        for cd in calls:
+            if len(cd) % pair:
+                raise B200Error.serialization(f"{what}: calldata must be a multiple of {pair} bytes")
+            blob += cd
+            offs.append(len(blob) // pair)
+        count = len(calls)
+        offsets = np.asarray(offs, dtype=np.uint32)
+        out, st = C.create_string_buffer(max(1, size * count)), C.create_string_buffer(max(1, count))
+        pairs = np.frombuffer(bytes(blob) or b"\0", dtype=np.uint8)
+        self._check(fn(self._h, pairs.ctypes.data_as(C.c_void_p), offsets.ctypes.data_as(C.c_void_p), count, out, st), what)
+        return [out.raw[size * i:size * (i + 1)] for i in range(count)], list(st.raw[:count])
+
+    def bls12_381_g1_add_batch(self, a: bytes, b: bytes):
+        """a, b: count x 128 bytes (EIP-2537 G1) each -> (count x 128 result bytes, [status])"""
+        return self._bls12_add(F.lib.b200zk_bls12_381_g1_add_batch, "b200zk_bls12_381_g1_add_batch", a, b, 128)
+
+    def bls12_381_g2_add_batch(self, a: bytes, b: bytes):
+        """a, b: count x 256 bytes (EIP-2537 G2) each -> (count x 256 result bytes, [status])"""
+        return self._bls12_add(F.lib.b200zk_bls12_381_g2_add_batch, "b200zk_bls12_381_g2_add_batch", a, b, 256)
+
+    def bls12_381_g1_msm_batch(self, calls):
+        """calls: list of G1MSM calldata byte strings (k x 160 bytes each) -> ([128-byte output per call], [status])"""
+        return self._bls12_msm(F.lib.b200zk_bls12_381_g1_msm_batch, "b200zk_bls12_381_g1_msm_batch", calls, 160, 128)
+
+    def bls12_381_g2_msm_batch(self, calls):
+        """calls: list of G2MSM calldata byte strings (k x 288 bytes each) -> ([256-byte output per call], [status])"""
+        return self._bls12_msm(F.lib.b200zk_bls12_381_g2_msm_batch, "b200zk_bls12_381_g2_msm_batch", calls, 288, 256)
+
     def kzg_verify_proof_batch(self, g2_setup: int, commitments, z, y, proofs) -> tuple:
         """n items: commitments and proofs n x 48 bytes, z and y n x 32-byte big-endian -> ([result 0/1], [status])"""
         n = _host_len(commitments) // 48

@@ -1,6 +1,9 @@
-// bls12.cuh -- BLS12-381 pieces shared by bls381.cu (commitments, proofs) and bls_pairing.cu (the pairing, KZG
-// verification): big-endian byte loaders, the 48-byte compressed G1 decoding, and Fp2 = Fp[u]/(u^2 + 1) over Fp381 with
-// Fq2's interface, so curve.cuh's XYZZ formulas (and xyzz_scalar_mul) instantiate over the twist unchanged.
+// bls12.cuh -- BLS12-381 pieces shared by bls381.cu (commitments, proofs), bls_pairing.cu (the pairing, KZG verification)
+// and bls_ops.cu (EIP-2537 addition and MSM): big-endian byte loaders and stores, the 48-byte compressed G1 decoding, the
+// EIP-2537 64-byte field element, Fp2 = Fp[u]/(u^2 + 1) over Fp381 with Fq2's interface, so curve.cuh's XYZZ formulas (and
+// xyzz_scalar_mul) instantiate over the twist unchanged, the r P = O subgroup checks, and the workspace carver of the
+// pairing-family calls.  The build has no -rdc: each translation unit keeps its own device copy of the __noinline__
+// functions, and `inline` lets the host linker merge their host-side stubs.
 #pragma once
 #include "common.cuh"
 
@@ -108,6 +111,48 @@ struct Fp2_381 {
 
 template <> struct CurveB<Fp2_381> {
   static B2_D Fp2_381 b() { Fp381 four = Fp381::zero(); four.v[0] = 4; four = Fp381::to_mont(four); return {four, four}; }  // 4 (1 + u)
+};
+
+// ---- subgroup checks: r P = O (no endomorphism shortcuts) -------------------------------------------------------------
+__device__ __noinline__ inline bool g1_in_subgroup(const Affine<Fp381>& p) {
+  uint32_t k[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
+  return xyzz_scalar_mul<Fp381>(k, p).is_inf();
+}
+__device__ __noinline__ inline bool g2_in_subgroup(const Affine<Fp2_381>& q) {
+  uint32_t k[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
+  return xyzz_scalar_mul<Fp2_381>(k, q).is_inf();
+}
+
+// EIP-2537 field element: 16 zero bytes, then 48 bytes big-endian below p
+B2_D bool load_fp64(const uint8_t* src, Fp381* out) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(src);
+  const uint32_t pad = __ldg(w) | __ldg(w + 1) | __ldg(w + 2) | __ldg(w + 3);
+  *out = load_be48(src + 16, 0xffffffffu);
+  return pad == 0 && Fp381::less(*out, Fp381::modulus());
+}
+
+// canonical limbs -> 48 bytes big-endian (out 4-byte aligned); load_be48's inverse
+B2_D void store_be48(uint8_t* out, const Fp381& canonical) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(out);
+#pragma unroll
+  for (int k = 0; k < 12; ++k) w[11 - k] = __byte_perm(canonical.v[k], 0, 0x0123);
+}
+
+// ---- host side ----------------------------------------------------------------------------------------------------------
+// carves one call's buffers out of ws_pairing: run the same sequence of take() once with base = nullptr to size it
+struct Carve {
+  uint8_t* base = nullptr;
+  size_t off = 0;
+  template <class T> T* take(size_t count) {
+    off = (off + 255) & ~(size_t)255;
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
 };
 
 }  // namespace b200zk

@@ -221,28 +221,6 @@ __device__ __noinline__ Fp12b miller_prepared(const BlsLine* L, const Affine<Fp3
   return f12_conj(f);
 }
 
-// ---- subgroup checks: r P = O (no endomorphism shortcuts) -------------------------------------------------------------
-__device__ __noinline__ bool g1_in_subgroup(const Affine<Fp381>& p) {
-  uint32_t k[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
-  return xyzz_scalar_mul<Fp381>(k, p).is_inf();
-}
-__device__ __noinline__ bool g2_in_subgroup(const Affine<F2>& q) {
-  uint32_t k[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
-  return xyzz_scalar_mul<F2>(k, q).is_inf();
-}
-
-// EIP-2537 field element: 16 zero bytes, then 48 bytes big-endian below p
-B2_D bool load_fp64(const uint8_t* src, Fp381* out) {
-  const uint32_t* w = reinterpret_cast<const uint32_t*>(src);
-  const uint32_t pad = __ldg(w) | __ldg(w + 1) | __ldg(w + 2) | __ldg(w + 3);
-  *out = load_be48(src + 16, 0xffffffffu);
-  return pad == 0 && Fp381::less(*out, Fp381::modulus());
-}
-
 // ---- kernels ----------------------------------------------------------------------------------------------------------
 // one thread per (G1, G2) pair of EIP-2537 bytes (128 + 256): range and padding (status 2), then curve and subgroup of
 // both points (status 3); kTrivial when a side is the identity
@@ -420,18 +398,6 @@ __global__ void __launch_bounds__(32) kzg_blob_fold(const XYZZ<Fp381>* terms, si
 }
 
 // ---- host side ----------------------------------------------------------------------------------------------------------
-// carves one call's buffers out of ws_pairing: run the same sequence of take() once with base = nullptr to size it
-struct Carve {
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <class T> T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-};
-
 size_t g2_lines_offset(size_t n) { return (n * sizeof(Affine<F2>) + 255) & ~(size_t)255; }
 const BlsLine* g2_setup_lines(const BasesEntry& e) { return reinterpret_cast<const BlsLine*>((const uint8_t*)e.d + g2_lines_offset(e.n)); }
 

@@ -368,6 +368,36 @@ int b200zk_kzg_verify_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint
 int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint8_t* blobs, const uint8_t* commitments,
                                        const uint8_t* proofs, size_t n, int* valid);
 
+/* ---- EIP-2537 G1/G2 addition and multi-scalar multiplication -------------------------------------------------------
+ * The Prague precompiles 0x0b-0x0e, `count` independent items per call, HOST buffers:
+ *   bls12_381_g1_add  Crypto::bls12_381_g1_add, provider.rs:549-562 (levm BLS12_G1ADD, precompiles.rs:1056-1107)
+ *   bls12_381_g1_msm  Crypto::bls12_381_g1_msm, provider.rs:566-593 (levm BLS12_G1MSM, precompiles.rs:1109-1165)
+ *   bls12_381_g2_add  Crypto::bls12_381_g2_add, provider.rs:596-609 (levm BLS12_G2ADD, precompiles.rs:1167-1244)
+ *   bls12_381_g2_msm  Crypto::bls12_381_g2_msm, provider.rs:613-640 (levm BLS12_G2MSM, precompiles.rs:1246-1315)
+ * Encodings as the pairing check: every Fp is 64 bytes, 16 zero bytes then 48 bytes big-endian; G1 = x | y (128 B), G2 =
+ * x.c0 | x.c1 | y.c0 | y.c1 (256 B); all-zero is the identity.  An MSM pair is a point followed by a 32-byte big-endian
+ * scalar (G1 160 B, G2 288 B); MSM call i covers pairs [pair_offsets[i], pair_offsets[i+1]).
+ * The return value reports infrastructure errors only; input errors are per item in status[i], with the table of the
+ * BN254 batches (the provider's parse_bls12_g1 / _g2 / _scalar, provider.rs:724-795):
+ *   0 ok, 1 ok and the result is the identity,
+ *   2 a coordinate >= p or a nonzero padding byte (checked for every point of the item before any curve check, so 2
+ *     outranks 3 within an item),
+ *   3 a point is off its curve; for the MSM calls also a point outside the order-r subgroup.
+ * Addition checks no subgroup (EIP-2537 and the provider ask only for the curve).  The MSM checks every non-identity point,
+ * including those whose scalar is zero (the provider's is_torsion_free).  Scalars are any 256-bit value: k P = (k mod r) P
+ * for a subgroup point, so a scalar >= r is not an error.  An empty MSM call returns the identity with status 1, as the
+ * provider does (levm refuses empty calldata before it).  out[i] is the precompile's own output (padded EIP-2537, the
+ * identity all zero); a failed item's output is all zero.  count = 0 returns 0; null pointers, pair_offsets[0] != 0 or
+ * decreasing offsets return 4 with b200zk_last_error set. */
+int b200zk_bls12_381_g1_add_batch(b200zk_ctx* ctx, const uint8_t* a /* count*128 */, const uint8_t* b /* count*128 */, size_t count,
+                                  uint8_t* out /* count*128 */, uint8_t* status /* count */);
+int b200zk_bls12_381_g2_add_batch(b200zk_ctx* ctx, const uint8_t* a /* count*256 */, const uint8_t* b /* count*256 */, size_t count,
+                                  uint8_t* out /* count*256 */, uint8_t* status /* count */);
+int b200zk_bls12_381_g1_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 160 B each */, const uint32_t* pair_offsets /* count+1 */,
+                                  size_t count, uint8_t* out /* count*128 */, uint8_t* status /* count */);
+int b200zk_bls12_381_g2_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 288 B each */, const uint32_t* pair_offsets /* count+1 */,
+                                  size_t count, uint8_t* out /* count*256 */, uint8_t* status /* count */);
+
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:
  *   bn254_g1_add         crates/common/crypto/provider.rs:201-234   (levm ecadd,     crates/vm/levm/src/precompiles.rs:692-716)

@@ -1,5 +1,6 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
-//! (`crates/common/crypto/provider.rs:201-330`) and its BLS12-381 pairing check (`provider.rs:642-672`) on the GPU.  The trait is one item per call; a provider that wants
+//! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`) and its
+//! BLS12-381 pairing check (`provider.rs:642-672`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
 //!
@@ -80,4 +81,85 @@ impl Crypto for B200Crypto {
             None => Err(CryptoError::Other("b200zk returned no result".to_string())),
         }
     }
+
+    fn bls12_381_g1_add(&self, a: ([u8; 48], [u8; 48]), b: ([u8; 48], [u8; 48])) -> Result<[u8; 96], CryptoError> {
+        let (pa, pb) = (pad_g1(&a), pad_g1(&b));
+        let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+        let (out, st) = gpu.bls12_381_g1_add_batch(&pa, &pb).map_err(device_error)?;
+        match st.first().copied() {
+            Some(ItemStatus::Ok | ItemStatus::OkIdentity) => Ok(unpad::<96>(&out)),
+            Some(bad) => Err(item_error(bad, "G1 point not on curve")),
+            None => Err(CryptoError::Other("b200zk returned no status".to_string())),
+        }
+    }
+
+    fn bls12_381_g1_msm(&self, pairs: &[(([u8; 48], [u8; 48]), [u8; 32])]) -> Result<[u8; 96], CryptoError> {
+        let mut calldata = Vec::with_capacity(pairs.len().saturating_mul(160));
+        for (point, scalar) in pairs {
+            calldata.extend_from_slice(&pad_g1(point));
+            calldata.extend_from_slice(scalar);
+        }
+        let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+        let res = gpu.bls12_381_g1_msm_batch(&[calldata.as_slice()]).map_err(device_error)?;
+        match res.first() {
+            Some(Ok(out)) => Ok(unpad::<96>(out)),
+            Some(Err(bad)) => Err(item_error(*bad, "G1 point not on curve or not in subgroup")),
+            None => Err(CryptoError::Other("b200zk returned no result".to_string())),
+        }
+    }
+
+    fn bls12_381_g2_add(&self, a: ([u8; 48], [u8; 48], [u8; 48], [u8; 48]), b: ([u8; 48], [u8; 48], [u8; 48], [u8; 48])) -> Result<[u8; 192], CryptoError> {
+        let (pa, pb) = (pad_g2(&a), pad_g2(&b));
+        let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+        let (out, st) = gpu.bls12_381_g2_add_batch(&pa, &pb).map_err(device_error)?;
+        match st.first().copied() {
+            Some(ItemStatus::Ok | ItemStatus::OkIdentity) => Ok(unpad::<192>(&out)),
+            Some(bad) => Err(item_error(bad, "G2 point not on curve")),
+            None => Err(CryptoError::Other("b200zk returned no status".to_string())),
+        }
+    }
+
+    fn bls12_381_g2_msm(&self, pairs: &[(([u8; 48], [u8; 48], [u8; 48], [u8; 48]), [u8; 32])]) -> Result<[u8; 192], CryptoError> {
+        let mut calldata = Vec::with_capacity(pairs.len().saturating_mul(288));
+        for (point, scalar) in pairs {
+            calldata.extend_from_slice(&pad_g2(point));
+            calldata.extend_from_slice(scalar);
+        }
+        let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+        let res = gpu.bls12_381_g2_msm_batch(&[calldata.as_slice()]).map_err(device_error)?;
+        match res.first() {
+            Some(Ok(out)) => Ok(unpad::<192>(out)),
+            Some(Err(bad)) => Err(item_error(*bad, "G2 point not on curve or not in subgroup")),
+            None => Err(CryptoError::Other("b200zk returned no result".to_string())),
+        }
+    }
+}
+
+/// The trait's 48-byte coordinates -> the EIP-2537 64-byte form the device takes (16 leading zero bytes each).
+fn pad_fps<const N: usize>(fps: [&[u8; 48]; N]) -> Vec<u8> {
+    let mut out = Vec::with_capacity(64 * N);
+    for fp in fps {
+        out.extend_from_slice(&[0u8; 16]);
+        out.extend_from_slice(fp);
+    }
+    out
+}
+
+fn pad_g1((x, y): &([u8; 48], [u8; 48])) -> Vec<u8> {
+    pad_fps([x, y])
+}
+
+/// G2 in the trait's and EIP-2537's order: x.c0, x.c1, y.c0, y.c1.
+fn pad_g2((x0, x1, y0, y1): &([u8; 48], [u8; 48], [u8; 48], [u8; 48])) -> Vec<u8> {
+    pad_fps([x0, x1, y0, y1])
+}
+
+/// The device's padded output -> the trait's unpadded form (serialize_bls12_g1 / _g2: 48-byte coordinates in the same
+/// order, the identity all zero).  Every 64-byte slot starts with 16 zero bytes, so dropping them loses nothing.
+fn unpad<const N: usize>(padded: &[u8]) -> [u8; N] {
+    let mut out = [0u8; N];
+    for (dst, src) in out.chunks_mut(48).zip(padded.chunks(64)) {
+        dst.copy_from_slice(&src[16..64]);
+    }
+    out
 }

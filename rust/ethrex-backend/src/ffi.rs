@@ -342,6 +342,84 @@ impl B200zk {
             .collect())
     }
 
+    /// `count` independent EIP-2537 G1ADD items: `a`, `b` = count x 128 bytes.  Returns (count x 128 result bytes, per-item status).
+    pub fn bls12_381_g1_add_batch(&mut self, a: &[u8], b: &[u8]) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        self.bls12_381_add_batch(a, b, 128, "bls12_381_g1_add_batch: inputs must be equal multiples of 128 bytes", sys::b200zk_bls12_381_g1_add_batch)
+    }
+
+    /// `count` independent EIP-2537 G2ADD items: `a`, `b` = count x 256 bytes.  Returns (count x 256 result bytes, per-item status).
+    pub fn bls12_381_g2_add_batch(&mut self, a: &[u8], b: &[u8]) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        self.bls12_381_add_batch(a, b, 256, "bls12_381_g2_add_batch: inputs must be equal multiples of 256 bytes", sys::b200zk_bls12_381_g2_add_batch)
+    }
+
+    /// Several EIP-2537 G1MSM calls in one launch.  `calls[i]` is the precompile's calldata (k x 160 bytes: G1 128 B |
+    /// 32-byte big-endian scalar).  Per call `Ok(128 output bytes)` or the input error; an empty call is the identity.
+    pub fn bls12_381_g1_msm_batch(&mut self, calls: &[&[u8]]) -> Result<Vec<Result<Vec<u8>, ItemStatus>>, BackendError> {
+        self.bls12_381_msm_batch(calls, 160, 128, "bls12_381_g1_msm_batch", sys::b200zk_bls12_381_g1_msm_batch)
+    }
+
+    /// Several EIP-2537 G2MSM calls in one launch.  `calls[i]` is the precompile's calldata (k x 288 bytes: G2 256 B |
+    /// 32-byte big-endian scalar).  Per call `Ok(256 output bytes)` or the input error; an empty call is the identity.
+    pub fn bls12_381_g2_msm_batch(&mut self, calls: &[&[u8]]) -> Result<Vec<Result<Vec<u8>, ItemStatus>>, BackendError> {
+        self.bls12_381_msm_batch(calls, 288, 256, "bls12_381_g2_msm_batch", sys::b200zk_bls12_381_g2_msm_batch)
+    }
+
+    fn bls12_381_add_batch(
+        &mut self,
+        a: &[u8],
+        b: &[u8],
+        size: usize,
+        what: &'static str,
+        f: unsafe extern "C" fn(*mut sys::b200zk_ctx, *const u8, *const u8, usize, *mut u8, *mut u8) -> std::os::raw::c_int,
+    ) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        if a.len() != b.len() || a.len() % size != 0 {
+            return Err(BackendError::serialization(what));
+        }
+        let count = a.len() / size;
+        let mut out = vec![0u8; a.len()];
+        let mut st = vec![0u8; count];
+        // SAFETY: all four buffers hold `count` items of the documented sizes and outlive the synchronous call.
+        let status = unsafe { f(self.ctx.as_ptr(), a.as_ptr(), b.as_ptr(), count, out.as_mut_ptr(), st.as_mut_ptr()) };
+        check(self, status)?;
+        Ok((out, st.into_iter().map(ItemStatus::from_code).collect()))
+    }
+
+    fn bls12_381_msm_batch(
+        &mut self,
+        calls: &[&[u8]],
+        pair: usize,
+        size: usize,
+        what: &'static str,
+        f: unsafe extern "C" fn(*mut sys::b200zk_ctx, *const u8, *const u32, usize, *mut u8, *mut u8) -> std::os::raw::c_int,
+    ) -> Result<Vec<Result<Vec<u8>, ItemStatus>>, BackendError> {
+        let mut blob = Vec::new();
+        let mut offsets = Vec::with_capacity(calls.len().saturating_add(1));
+        offsets.push(0u32);
+        for cd in calls {
+            if cd.len() % pair != 0 {
+                return Err(BackendError::serialization(format!("{what}: calldata must be a multiple of {pair} bytes")));
+            }
+            blob.extend_from_slice(cd);
+            let pairs = u32::try_from(blob.len() / pair).map_err(|_| BackendError::serialization(format!("{what}: too many pairs")))?;
+            offsets.push(pairs);
+        }
+        let count = calls.len();
+        let mut out = vec![0u8; count.saturating_mul(size)];
+        let mut st = vec![0u8; count];
+        // SAFETY: `offsets` has count + 1 entries, `blob` holds offsets[count] pairs, `out` holds count x size bytes and
+        // `st` count bytes.
+        let status = unsafe { f(self.ctx.as_ptr(), blob.as_ptr(), offsets.as_ptr(), count, out.as_mut_ptr(), st.as_mut_ptr()) };
+        check(self, status)?;
+        Ok(out
+            .chunks(size)
+            .zip(st)
+            .map(|(o, s)| match ItemStatus::from_code(s) {
+                ItemStatus::Ok | ItemStatus::OkIdentity => Ok(o.to_vec()),
+                bad => Err(bad),
+            })
+            .collect())
+    }
+
     /// Upload a KZG setup's G2 points (96-byte compressed, `g2_monomial` order: [1]2, [tau]2, ...), subgroup-checked.
     /// The handle is what the two KZG verify calls take; free it with `bases_free`.
     pub fn bls12_381_g2_bases_upload(&mut self, points: &[u8]) -> Result<u64, BackendError> {
