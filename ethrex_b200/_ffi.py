@@ -27,6 +27,7 @@ G16_INPUTS_DEVICE = 1 << 8
 G16_H_COEFFS = 1 << 9
 SCALARS_RAW = 1 << 10
 POINTS_COMPRESSED = 1 << 11
+ECRECOVER_LOW_S = 1  # b200zk_secp256k1_ecrecover_batch: reject s > n/2 (EIP-2)
 
 _vp, _sz, _u32, _u64, _int = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int
 _ctx = C.c_void_p
@@ -114,6 +115,7 @@ SIGNATURES = {
     "b200zk_bls12_381_g2_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g1_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g2_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_secp256k1_ecrecover_batch": (_int, [_ctx, _vp, _vp, _sz, _u32, _vp, _vp]),
     "b200zk_bn254_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_g1_mul_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_pairing_check_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

@@ -413,6 +413,22 @@ class Context:
         """calls: list of G2MSM calldata byte strings (k x 288 bytes each) -> ([256-byte output per call], [status])"""
         return self._bls12_msm(F.lib.b200zk_bls12_381_g2_msm_batch, "b200zk_bls12_381_g2_msm_batch", calls, 288, 256)
 
+    # ------------------------------------------------------------------ secp256k1 signer recovery (ECRECOVER)
+    def secp256k1_ecrecover_batch(self, sigs, msgs, low_s: bool = False):
+        """sigs: count x 65 bytes (r | s | recid), msgs: count x 32-byte hashes -> (count x 32 bytes, [status]).
+        Item i's 32 bytes are keccak256 of the recovered public key (the address is bytes 12..32), zero when status[i]
+        != 0 (2 InvalidSignature, 3 RecoveryFailed, 4 InvalidRecoveryId).  low_s: EIP-2's s <= n/2, as recover_signer."""
+        ns, nm = _host_len(sigs), _host_len(msgs)
+        if ns % 65 or nm % 32 or ns // 65 != nm // 32:
+            raise B200Error.serialization("b200zk_secp256k1_ecrecover_batch: sigs must be count x 65 bytes and msgs count x 32 bytes")
+        count = ns // 65
+        sp, k1 = _host_ptr(sigs) if count else (None, None)
+        mp, k2 = _host_ptr(msgs) if count else (None, None)
+        out, st = C.create_string_buffer(max(1, 32 * count)), C.create_string_buffer(max(1, count))
+        self._check(F.lib.b200zk_secp256k1_ecrecover_batch(self._h, sp, mp, count, F.ECRECOVER_LOW_S if low_s else 0, out, st),
+                    "b200zk_secp256k1_ecrecover_batch")
+        return out.raw[:32 * count], list(st.raw[:count])
+
     def kzg_verify_proof_batch(self, g2_setup: int, commitments, z, y, proofs) -> tuple:
         """n items: commitments and proofs n x 48 bytes, z and y n x 32-byte big-endian -> ([result 0/1], [status])"""
         n = _host_len(commitments) // 48

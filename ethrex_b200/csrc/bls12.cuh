@@ -142,17 +142,4 @@ B2_D void store_be48(uint8_t* out, const Fp381& canonical) {
   for (int k = 0; k < 12; ++k) w[11 - k] = __byte_perm(canonical.v[k], 0, 0x0123);
 }
 
-// ---- host side ----------------------------------------------------------------------------------------------------------
-// carves one call's buffers out of ws_pairing: run the same sequence of take() once with base = nullptr to size it
-struct Carve {
-  uint8_t* base = nullptr;
-  size_t off = 0;
-  template <class T> T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-};
-
 }  // namespace b200zk

@@ -72,7 +72,12 @@ struct b200zk_ctx {
   // partial sums and encoded results of one call
   b200zk::DevBuf kzg_roots, ws_kzg;
   cudaEvent_t kzg_roots_ready = nullptr;
-  b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values
+  b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
+                              // also the inputs and outputs of the EIP-2537 (bls_ops.cu) and ECRECOVER (secp256k1.cu) batches
+  // ECRECOVER (secp256k1.cu): d G for d = 1 .. 4095 as affine secp256k1 points (256 KB), built once per context on first use;
+  // consumers on other streams wait on secp_gtab_ready
+  b200zk::DevBuf secp_gtab;
+  cudaEvent_t secp_gtab_ready = nullptr;
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
@@ -150,6 +155,18 @@ struct NvtxRange {
 };
 
 inline cudaStream_t pick_stream(b200zk_ctx* ctx, void* stream) { return stream ? (cudaStream_t)stream : ctx->stream; }
+
+// carves one call's buffers out of a workspace: run the same sequence of take() once with base = nullptr to size it
+struct Carve {
+  uint8_t* base = nullptr;
+  size_t off = 0;
+  template <class T> T* take(size_t count) {
+    off = (off + 255) & ~(size_t)255;
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += count * sizeof(T);
+    return p;
+  }
+};
 
 // every kernel launch in the library goes through this macro so gpu_launches is a count, not a guess
 #define B2_LAUNCH(ctx, kernel, grid, block, smem, st, ...)                                   \

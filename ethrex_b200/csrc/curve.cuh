@@ -7,6 +7,8 @@
 // Formulas: EFD shortw/xyzz madd-2008-s, add-2008-s, dbl-2008-s-1, mdbl-2008-s-1 (a = 0).  The affine
 // result of an MSM is independent of the coordinate system, so bit-exactness against the reference's
 // Jacobian arithmetic (ark-ec 0.5.0 short_weierstrass::Projective) only depends on the final normalisation.
+// The templates are __host__ __device__: a field type whose operations are too (secp256k1.cuh) runs them on the host,
+// which is how its tests check them without a device; the device-only fields only ever instantiate them in kernels.
 #pragma once
 #include "field.cuh"
 
@@ -14,22 +16,22 @@ namespace b200zk {
 
 template <class F> struct Affine {
   F x, y;
-  B2_D bool is_inf() const { return x.is_zero() && y.is_zero(); }
+  B2_HD bool is_inf() const { return x.is_zero() && y.is_zero(); }
 };
 
 template <class F> struct XYZZ {
   F x, y, zz, zzz;
-  static B2_D XYZZ identity() { return {F::zero(), F::zero(), F::zero(), F::zero()}; }
-  B2_D bool is_inf() const { return zz.is_zero(); }
+  static B2_HD XYZZ identity() { return {F::zero(), F::zero(), F::zero(), F::zero()}; }
+  B2_HD bool is_inf() const { return zz.is_zero(); }
 };
 
-template <class F> B2_D XYZZ<F> xyzz_from_affine(const Affine<F>& p) {
+template <class F> B2_HD XYZZ<F> xyzz_from_affine(const Affine<F>& p) {
   if (p.is_inf()) return XYZZ<F>::identity();
   return {p.x, p.y, F::one(), F::one()};
 }
 
 // 2*(x1, y1) for an affine point (mdbl-2008-s-1, a = 0)
-template <class F> B2_D XYZZ<F> xyzz_mdbl(const F& x1, const F& y1) {
+template <class F> B2_HD XYZZ<F> xyzz_mdbl(const F& x1, const F& y1) {
   F U = F::dbl(y1), V = F::sqr(U), W = F::mul(U, V), S = F::mul(x1, V);
   F xx = F::sqr(x1), M = F::add(F::dbl(xx), xx);
   XYZZ<F> r;
@@ -40,7 +42,7 @@ template <class F> B2_D XYZZ<F> xyzz_mdbl(const F& x1, const F& y1) {
 }
 
 // 2*P (dbl-2008-s-1, a = 0)
-template <class F> B2_D XYZZ<F> xyzz_dbl(const XYZZ<F>& p) {
+template <class F> B2_HD XYZZ<F> xyzz_dbl(const XYZZ<F>& p) {
   if (p.is_inf()) return p;
   F U = F::dbl(p.y), V = F::sqr(U), W = F::mul(U, V), S = F::mul(p.x, V);
   F xx = F::sqr(p.x), M = F::add(F::dbl(xx), xx);
@@ -52,7 +54,7 @@ template <class F> B2_D XYZZ<F> xyzz_dbl(const XYZZ<F>& p) {
 }
 
 // acc += (x2, y2)  (madd-2008-s; identity, doubling and cancellation handled)
-template <class F> B2_D void xyzz_add_mixed(XYZZ<F>& acc, const F& x2, const F& y2) {
+template <class F> B2_HD void xyzz_add_mixed(XYZZ<F>& acc, const F& x2, const F& y2) {
   if (x2.is_zero() && y2.is_zero()) return;
   if (acc.is_inf()) { acc.x = x2; acc.y = y2; acc.zz = F::one(); acc.zzz = F::one(); return; }
   F U2 = F::mul(x2, acc.zz), S2 = F::mul(y2, acc.zzz);
@@ -71,7 +73,7 @@ template <class F> B2_D void xyzz_add_mixed(XYZZ<F>& acc, const F& x2, const F& 
 }
 
 // acc += q  (add-2008-s with the exceptional cases)
-template <class F> B2_D void xyzz_add(XYZZ<F>& acc, const XYZZ<F>& q) {
+template <class F> B2_HD void xyzz_add(XYZZ<F>& acc, const XYZZ<F>& q) {
   if (q.is_inf()) return;
   if (acc.is_inf()) { acc = q; return; }
   F U1 = F::mul(acc.x, q.zz), U2 = F::mul(q.x, acc.zz);
@@ -90,7 +92,7 @@ template <class F> B2_D void xyzz_add(XYZZ<F>& acc, const XYZZ<F>& q) {
   acc.zzz = F::mul(F::mul(acc.zzz, q.zzz), PPP);
 }
 
-template <class F> B2_D Affine<F> xyzz_to_affine(const XYZZ<F>& p) {
+template <class F> B2_HD Affine<F> xyzz_to_affine(const XYZZ<F>& p) {
   if (p.is_inf()) return {F::zero(), F::zero()};
   F t = F::inv(F::mul(p.zz, p.zzz));
   F zz_inv = F::mul(t, p.zzz), zzz_inv = F::mul(t, p.zz);
@@ -98,7 +100,7 @@ template <class F> B2_D Affine<F> xyzz_to_affine(const XYZZ<F>& p) {
 }
 
 // k * P, k = 256-bit little-endian limbs (double-and-add, MSB first).  Setup / utility use only.
-template <class F> B2_D XYZZ<F> xyzz_scalar_mul(const uint32_t* k, const Affine<F>& p) {
+template <class F> B2_HD XYZZ<F> xyzz_scalar_mul(const uint32_t* k, const Affine<F>& p) {
   XYZZ<F> acc = XYZZ<F>::identity();
   for (int i = 255; i >= 0; --i) {
     acc = xyzz_dbl(acc);
@@ -124,7 +126,7 @@ template <> struct CurveB<Fq2> {
     return {Fq::to_mont(a), Fq::to_mont(c)};
   }
 };
-template <class F> B2_D bool affine_on_curve(const Affine<F>& p) {
+template <class F> B2_HD bool affine_on_curve(const Affine<F>& p) {
   if (p.is_inf()) return true;
   F lhs = F::sqr(p.y), rhs = F::add(F::mul(F::sqr(p.x), p.x), CurveB<F>::b());
   return lhs == rhs;

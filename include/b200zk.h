@@ -398,6 +398,29 @@ int b200zk_bls12_381_g1_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 160 B
 int b200zk_bls12_381_g2_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 288 B each */, const uint32_t* pair_offsets /* count+1 */,
                                   size_t count, uint8_t* out /* count*256 */, uint8_t* status /* count */);
 
+/* ---- secp256k1 signer recovery (ECRECOVER) -------------------------------------------------------------------------
+ * `count` independent items per call, HOST buffers:
+ *   secp256k1_ecrecover  Crypto::secp256k1_ecrecover, provider.rs:63-88 (levm ECRECOVER 0x01, precompiles.rs:456-510)
+ *   recover_signer       Crypto::recover_signer, provider.rs:153-171 (transaction senders, EIP-7702 authorities): pass
+ *                        B200ZK_ECRECOVER_LOW_S and take the address from bytes 12..32 of out[i]
+ * Item i: sigs[65 i ..] = r (32 B big-endian) | s (32 B big-endian) | recid (1 B), msgs[32 i ..] = the 32-byte message
+ * hash.  out[32 i ..] = keccak256(X | Y) of the recovered public key (X, Y 32-byte big-endian).  The checks run in this
+ * order and the first failure sets status[i] (a failed item's output is all zero):
+ *   2 InvalidSignature    with B200ZK_ECRECOVER_LOW_S: s > n/2 (EIP-2)
+ *   4 InvalidRecoveryId   recid > 3
+ *   2 InvalidSignature    r >= n or s >= n
+ *   3 RecoveryFailed      r = 0 or s = 0; recid 2 or 3 with r >= p - n (otherwise x = r + n); no curve point has
+ *                         abscissa x (x^3 + 7 is not a square); Q = r^-1 (s R - z G) is the identity
+ *   0 ok
+ * R is the point with abscissa x and y parity recid & 1, z the hash as a 256-bit integer reduced mod n.  This is the
+ * libsecp256k1 path, the reference's default build; its k256 fallback (provider.rs:90-151) rejects recids 2 and 3.  Real
+ * callers pass 0 or 1 (the precompile maps v = 27 / 28, transactions carry a y-parity bit).
+ * count = 0 returns 0; null pointers or unknown flag bits return 4 with b200zk_last_error set.  The table of G multiples
+ * the call reads is built on the device on the context's first call (256 KB, kept until b200zk_destroy). */
+#define B200ZK_ECRECOVER_LOW_S 1u /* reject s > n/2 with status 2 (EIP-2, Crypto::recover_signer) */
+int b200zk_secp256k1_ecrecover_batch(b200zk_ctx* ctx, const uint8_t* sigs /* count*65 */, const uint8_t* msgs /* count*32 */,
+                                     size_t count, uint32_t flags, uint8_t* out /* count*32 */, uint8_t* status /* count */);
+
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:
  *   bn254_g1_add         crates/common/crypto/provider.rs:201-234   (levm ecadd,     crates/vm/levm/src/precompiles.rs:692-716)

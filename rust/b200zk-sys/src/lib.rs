@@ -41,6 +41,8 @@ pub const B200ZK_G16_INPUTS_DEVICE: u32 = 1 << 8;
 pub const B200ZK_G16_H_COEFFS: u32 = 1 << 9;
 pub const B200ZK_SCALARS_RAW: u32 = 1 << 10;
 pub const B200ZK_POINTS_COMPRESSED: u32 = 1 << 11;
+/// b200zk_secp256k1_ecrecover_batch: reject s > n/2 with status 2 (EIP-2, `Crypto::recover_signer`)
+pub const B200ZK_ECRECOVER_LOW_S: u32 = 1;
 
 /// `struct b200zk_groth16_pk` (include/b200zk.h): columns 0..4 = A_g1, B_g1 (handle 0 = absent), B_g2, L_g1, H_g1.
 #[repr(C)]
@@ -141,6 +143,7 @@ unsafe extern "C" {
     pub fn b200zk_bls12_381_g2_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g1_msm_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g2_msm_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;
+    pub fn b200zk_secp256k1_ecrecover_batch(ctx: *mut b200zk_ctx, sigs: *const u8, msgs: *const u8, count: usize, flags: u32, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bn254_g1_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bn254_g1_mul_batch(ctx: *mut b200zk_ctx, points: *const u8, scalars: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bn254_pairing_check_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, result: *mut u8, status: *mut u8) -> c_int;

@@ -1,15 +1,16 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
 //! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`) and its
-//! BLS12-381 pairing check (`provider.rs:642-672`) on the GPU.  The trait is one item per call; a provider that wants
+//! BLS12-381 pairing check (`provider.rs:642-672`) and its secp256k1 signer recovery (`provider.rs:63-171`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
 //!
 //! Error mapping follows the reference: the levm wrappers reject coordinates >= p before the curve call
 //! (`crates/vm/levm/src/precompiles.rs:801-820`, `PrecompileError::CoordinateExceedsFieldModulus`), the provider
 //! reports points off the curve as `CryptoError::InvalidPoint`.
+use ethrex_common::Address;
 use ethrex_crypto::{Crypto, CryptoError};
 
-use crate::ffi::{global, ItemStatus};
+use crate::ffi::{global, ItemStatus, RecoverStatus};
 
 #[derive(Debug, Default, Clone, Copy)]
 pub struct B200Crypto;
@@ -25,7 +26,62 @@ fn item_error(status: ItemStatus, what: &'static str) -> CryptoError {
     }
 }
 
+fn recover_error(status: RecoverStatus) -> CryptoError {
+    match status {
+        RecoverStatus::InvalidSignature => CryptoError::InvalidSignature,
+        RecoverStatus::RecoveryFailed => CryptoError::RecoveryFailed,
+        RecoverStatus::InvalidRecoveryId => CryptoError::InvalidRecoveryId,
+        other => CryptoError::Other(format!("b200zk ecrecover status {other:?}")),
+    }
+}
+
+/// keccak256 of each recovered public key, one device call for all items
+fn ecrecover_batch(items: &[([u8; 65], [u8; 32])], low_s: bool) -> Result<Vec<Result<[u8; 32], CryptoError>>, CryptoError> {
+    let mut sigs = Vec::with_capacity(items.len().saturating_mul(65));
+    let mut msgs = Vec::with_capacity(items.len().saturating_mul(32));
+    for (sig, msg) in items {
+        sigs.extend_from_slice(sig);
+        msgs.extend_from_slice(msg);
+    }
+    let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;
+    let res = gpu.secp256k1_ecrecover_batch(&sigs, &msgs, low_s).map_err(device_error)?;
+    Ok(res.into_iter().map(|r| r.map_err(recover_error)).collect())
+}
+
+fn address_of(hash: &[u8; 32]) -> Address {
+    Address::from_slice(hash.split_at(12).1)
+}
+
+/// Transaction senders in one device call: the drop-in for the `par_iter` of `Block::get_transactions_with_sender`
+/// (`crates/common/types/block.rs:323-333`).  Each item is what `Crypto::recover_signer` takes (a 65-byte r | s | recid
+/// signature and the 32-byte signing hash), with its EIP-2 low-s rule; the results are in item order.
+pub fn recover_signers_batch(items: &[([u8; 65], [u8; 32])]) -> Vec<Result<Address, CryptoError>> {
+    match ecrecover_batch(items, true) {
+        Ok(res) => res.into_iter().map(|r| r.map(|h| address_of(&h))).collect(),
+        Err(e) => items.iter().map(|_| Err(CryptoError::Other(e.to_string()))).collect(),
+    }
+}
+
 impl Crypto for B200Crypto {
+    /// Follows the reference's default (libsecp256k1) path, recids 2 and 3 included; see include/b200zk.h.
+    fn secp256k1_ecrecover(&self, sig: &[u8; 64], recid: u8, msg: &[u8; 32]) -> Result<[u8; 32], CryptoError> {
+        let mut full = [0u8; 65];
+        let (head, tail) = full.split_at_mut(64);
+        head.copy_from_slice(sig);
+        tail.copy_from_slice(&[recid]);
+        ecrecover_batch(&[(full, *msg)], false)?
+            .into_iter()
+            .next()
+            .unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
+    }
+
+    fn recover_signer(&self, sig: &[u8; 65], msg: &[u8; 32]) -> Result<Address, CryptoError> {
+        recover_signers_batch(&[(*sig, *msg)])
+            .into_iter()
+            .next()
+            .unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
+    }
+
     fn bn254_g1_add(&self, p1: &[u8], p2: &[u8]) -> Result<[u8; 64], CryptoError> {
         let (a, b) = (p1.get(..64).ok_or(CryptoError::InvalidInput("G1 point must be 64 bytes"))?, p2.get(..64).ok_or(CryptoError::InvalidInput("G1 point must be 64 bytes"))?);
         let mut gpu = global().map_err(device_error)?.lock().map_err(device_error)?;

@@ -249,6 +249,29 @@ impl ItemStatus {
     }
 }
 
+/// Per-item outcome of `b200zk_secp256k1_ecrecover_batch` (include/b200zk.h): the reference's `CryptoError` cases of
+/// `Crypto::secp256k1_ecrecover` / `recover_signer`.  Its codes mean something else than [`ItemStatus`]'s.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum RecoverStatus {
+    Ok,
+    InvalidSignature,
+    RecoveryFailed,
+    InvalidRecoveryId,
+    Unknown(u8),
+}
+
+impl RecoverStatus {
+    fn from_code(code: u8) -> Self {
+        match code {
+            0 => Self::Ok,
+            2 => Self::InvalidSignature,
+            3 => Self::RecoveryFailed,
+            4 => Self::InvalidRecoveryId,
+            other => Self::Unknown(other),
+        }
+    }
+}
+
 impl B200zk {
     /// `count` independent ecAdd items: `a`, `b` = count x 64 bytes.  Returns (count x 64 result bytes, per-item status).
     pub fn bn254_g1_add_batch(&mut self, a: &[u8], b: &[u8]) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
@@ -362,6 +385,32 @@ impl B200zk {
     /// 32-byte big-endian scalar).  Per call `Ok(256 output bytes)` or the input error; an empty call is the identity.
     pub fn bls12_381_g2_msm_batch(&mut self, calls: &[&[u8]]) -> Result<Vec<Result<Vec<u8>, ItemStatus>>, BackendError> {
         self.bls12_381_msm_batch(calls, 288, 256, "bls12_381_g2_msm_batch", sys::b200zk_bls12_381_g2_msm_batch)
+    }
+
+    /// `count` independent ECRECOVER items: `sigs` = count x 65 bytes (r | s | recid, r and s big-endian), `msgs` =
+    /// count x 32-byte hashes.  `low_s` rejects s > n/2 (EIP-2, as `Crypto::recover_signer`).  Per item
+    /// `Ok(keccak256 of the recovered public key)` (the address is bytes 12..32) or its status.
+    pub fn secp256k1_ecrecover_batch(&mut self, sigs: &[u8], msgs: &[u8], low_s: bool) -> Result<Vec<Result<[u8; 32], RecoverStatus>>, BackendError> {
+        if sigs.len() % 65 != 0 || msgs.len() % 32 != 0 || sigs.len() / 65 != msgs.len() / 32 {
+            return Err(BackendError::serialization("secp256k1_ecrecover_batch: sigs must be count x 65 bytes and msgs count x 32 bytes"));
+        }
+        let count = sigs.len() / 65;
+        let mut out = vec![0u8; msgs.len()];
+        let mut st = vec![0u8; count];
+        let flags = if low_s { sys::B200ZK_ECRECOVER_LOW_S } else { 0 };
+        // SAFETY: `sigs` holds count x 65 bytes, `msgs` and `out` count x 32, `st` count.
+        let status = unsafe {
+            sys::b200zk_secp256k1_ecrecover_batch(self.ctx.as_ptr(), sigs.as_ptr(), msgs.as_ptr(), count, flags, out.as_mut_ptr(), st.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(out
+            .chunks_exact(32)
+            .zip(st)
+            .map(|(h, s)| match RecoverStatus::from_code(s) {
+                RecoverStatus::Ok => <[u8; 32]>::try_from(h).map_err(|_| RecoverStatus::Unknown(s)),
+                bad => Err(bad),
+            })
+            .collect())
     }
 
     fn bls12_381_add_batch(
