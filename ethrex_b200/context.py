@@ -429,6 +429,19 @@ class Context:
                     "b200zk_secp256k1_ecrecover_batch")
         return out.raw[:32 * count], list(st.raw[:count])
 
+    # ------------------------------------------------------------------ P-256 signature verification (P256VERIFY)
+    def secp256r1_verify_batch(self, inputs) -> list:
+        """inputs: count x 160 bytes, the P256VERIFY calldata h | r | s | qx | qy each -> [bool] per item (EIP-7951:
+        True when the signature verifies; malformed or off-curve items are False)."""
+        n = _host_len(inputs)
+        if n % 160:
+            raise B200Error.serialization("b200zk_secp256r1_verify_batch: inputs must be count x 160 bytes")
+        count = n // 160
+        ip, keep = _host_ptr(inputs) if count else (None, None)
+        res = C.create_string_buffer(max(1, count))
+        self._check(F.lib.b200zk_secp256r1_verify_batch(self._h, ip, count, res), "b200zk_secp256r1_verify_batch")
+        return [b == 1 for b in res.raw[:count]]
+
     def kzg_verify_proof_batch(self, g2_setup: int, commitments, z, y, proofs) -> tuple:
         """n items: commitments and proofs n x 48 bytes, z and y n x 32-byte big-endian -> ([result 0/1], [status])"""
         n = _host_len(commitments) // 48

@@ -222,6 +222,8 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   if (ctx->kzg_roots_ready) cudaEventDestroy(ctx->kzg_roots_ready);
   if (ctx->secp_gtab.p) cudaFree(ctx->secp_gtab.p);
   if (ctx->secp_gtab_ready) cudaEventDestroy(ctx->secp_gtab_ready);
+  if (ctx->p256_gtab.p) cudaFree(ctx->p256_gtab.p);
+  if (ctx->p256_gtab_ready) cudaEventDestroy(ctx->p256_gtab_ready);
   DevBuf* bufs[] = {&ctx->ws_hist, &ctx->ws_offsets, &ctx->ws_cursor, &ctx->ws_blocksums, &ctx->ws_idx, &ctx->ws_buckets, &ctx->ws_chunkS,
                     &ctx->ws_chunkV, &ctx->ws_result, &ctx->ws_points, &ctx->ws_scalars, &ctx->ws_ntt, &ctx->ws_misc, &ctx->ws_out, &ctx->ws_segoff, &ctx->ws_segbucket, &ctx->ws_digits, &ctx->ws_q0, &ctx->ws_q1, &ctx->ws_prefix, &ctx->ws_info, &ctx->ws_pairoff0, &ctx->ws_pairoff1};
   for (DevBuf* b : bufs) if (b->p) cudaFree(b->p);

@@ -73,11 +73,16 @@ struct b200zk_ctx {
   b200zk::DevBuf kzg_roots, ws_kzg;
   cudaEvent_t kzg_roots_ready = nullptr;
   b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
-                              // also the inputs and outputs of the EIP-2537 (bls_ops.cu) and ECRECOVER (secp256k1.cu) batches
+                              // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu) and
+                              // P256VERIFY (secp256r1.cu) batches
   // ECRECOVER (secp256k1.cu): d G for d = 1 .. 4095 as affine secp256k1 points (256 KB), built once per context on first use;
   // consumers on other streams wait on secp_gtab_ready
   b200zk::DevBuf secp_gtab;
   cudaEvent_t secp_gtab_ready = nullptr;
+  // P256VERIFY (secp256r1.cu): the same table for the P-256 generator (affine, Montgomery form, 256 KB), waited on through
+  // p256_gtab_ready
+  b200zk::DevBuf p256_gtab;
+  cudaEvent_t p256_gtab_ready = nullptr;
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};

@@ -4,7 +4,8 @@
 // EIP-196/197 convention of /root/reference/crates/common/crypto/provider.rs:201-330).  Accumulators use
 // extended Jacobian "XYZZ" coordinates (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2; ZZ = 0 = identity): the mixed
 // addition costs 8M+2S and needs no inversion, which is what the bucket-accumulation kernel is made of.
-// Formulas: EFD shortw/xyzz madd-2008-s, add-2008-s, dbl-2008-s-1, mdbl-2008-s-1 (a = 0).  The affine
+// Formulas: EFD shortw/xyzz madd-2008-s, add-2008-s, dbl-2008-s-1, mdbl-2008-s-1 (a = 0; CurveA below adds a = -3
+// for P-256, which only the doublings and the curve equation see).  The affine
 // result of an MSM is independent of the coordinate system, so bit-exactness against the reference's
 // Jacobian arithmetic (ark-ec 0.5.0 short_weierstrass::Projective) only depends on the final normalisation.
 // The templates are __host__ __device__: a field type whose operations are too (secp256k1.cuh) runs them on the host,
@@ -30,10 +31,22 @@ template <class F> B2_HD XYZZ<F> xyzz_from_affine(const Affine<F>& p) {
   return {p.x, p.y, F::one(), F::one()};
 }
 
-// 2*(x1, y1) for an affine point (mdbl-2008-s-1, a = 0)
+// the a coefficient of y^2 = x^3 + a x + b: 0 unless a curve specialises it.  The doublings and affine_on_curve support
+// a = 0 and a = -3 (P-256, secp256r1.cuh); for a = 0 they compile to exactly the a-free formulas.
+template <class F> struct CurveA { static constexpr int a = 0; };
+
+// 2*(x1, y1) for an affine point (mdbl-2008-s-1); M = 3 x^2 + a
 template <class F> B2_HD XYZZ<F> xyzz_mdbl(const F& x1, const F& y1) {
+  static_assert(CurveA<F>::a == 0 || CurveA<F>::a == -3, "curve.cuh doubles only for a = 0 or a = -3");
   F U = F::dbl(y1), V = F::sqr(U), W = F::mul(U, V), S = F::mul(x1, V);
-  F xx = F::sqr(x1), M = F::add(F::dbl(xx), xx);
+  F M;
+  if constexpr (CurveA<F>::a == -3) {  // 3 (x - 1)(x + 1)
+    F t = F::mul(F::sub(x1, F::one()), F::add(x1, F::one()));
+    M = F::add(F::dbl(t), t);
+  } else {
+    F xx = F::sqr(x1);
+    M = F::add(F::dbl(xx), xx);
+  }
   XYZZ<F> r;
   r.x = F::sub(F::sqr(M), F::dbl(S));
   r.y = F::mul2_sub(M, F::sub(S, r.x), W, y1);
@@ -41,11 +54,19 @@ template <class F> B2_HD XYZZ<F> xyzz_mdbl(const F& x1, const F& y1) {
   return r;
 }
 
-// 2*P (dbl-2008-s-1, a = 0)
+// 2*P (dbl-2008-s-1); M = 3 X^2 + a ZZ^2
 template <class F> B2_HD XYZZ<F> xyzz_dbl(const XYZZ<F>& p) {
+  static_assert(CurveA<F>::a == 0 || CurveA<F>::a == -3, "curve.cuh doubles only for a = 0 or a = -3");
   if (p.is_inf()) return p;
   F U = F::dbl(p.y), V = F::sqr(U), W = F::mul(U, V), S = F::mul(p.x, V);
-  F xx = F::sqr(p.x), M = F::add(F::dbl(xx), xx);
+  F M;
+  if constexpr (CurveA<F>::a == -3) {  // 3 (X - ZZ)(X + ZZ)
+    F t = F::mul(F::sub(p.x, p.zz), F::add(p.x, p.zz));
+    M = F::add(F::dbl(t), t);
+  } else {
+    F xx = F::sqr(p.x);
+    M = F::add(F::dbl(xx), xx);
+  }
   XYZZ<F> r;
   r.x = F::sub(F::sqr(M), F::dbl(S));
   r.y = F::mul2_sub(M, F::sub(S, r.x), W, p.y);
@@ -127,8 +148,11 @@ template <> struct CurveB<Fq2> {
   }
 };
 template <class F> B2_HD bool affine_on_curve(const Affine<F>& p) {
+  static_assert(CurveA<F>::a == 0 || CurveA<F>::a == -3, "curve.cuh checks the curve equation only for a = 0 or a = -3");
   if (p.is_inf()) return true;
-  F lhs = F::sqr(p.y), rhs = F::add(F::mul(F::sqr(p.x), p.x), CurveB<F>::b());
+  F lhs = F::sqr(p.y), rhs;
+  if constexpr (CurveA<F>::a == -3) rhs = F::add(F::mul(F::sub(F::sqr(p.x), F::add(F::dbl(F::one()), F::one())), p.x), CurveB<F>::b());  // (x^2 - 3) x + b
+  else rhs = F::add(F::mul(F::sqr(p.x), p.x), CurveB<F>::b());
   return lhs == rhs;
 }
 

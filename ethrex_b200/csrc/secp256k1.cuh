@@ -341,7 +341,7 @@ B2_HD void keccak256_64(const uint8_t* in, uint8_t* out) {
   for (int i = 0; i < 32; ++i) out[i] = (uint8_t)(st[i >> 3] >> (8 * (i & 7)));
 }
 
-// ---- recovery -------------------------------------------------------------------------------------------------------------
+// ---- recovery; its G table, wNAF and ladder below are shared with P-256 (secp256r1.cuh) -----------------------------------
 constexpr uint32_t kSecpLowS = 1;  // B200ZK_ECRECOVER_LOW_S
 enum : uint32_t { kEcrecOk = 0, kEcrecInvalidSignature = 2, kEcrecRecoveryFailed = 3, kEcrecInvalidRecoveryId = 4 };
 // fixed-base window of the G term: 12-bit digits of u1, 22 mixed additions.  Measured against 4 and 8 bits (DESIGN.md
@@ -351,13 +351,16 @@ constexpr int kSecpGTable = (1 << kSecpGWindow) - 1;         // table[d - 1] = d
 constexpr int kSecpRWindow = 5;                              // wNAF width of the R term: digits odd, |d| < 16
 constexpr int kSecpRTable = 1 << (kSecpRWindow - 2);         // R, 3R, .., 15R
 
-// the affine table the G term reads: table[d - 1] = d G
+// an entry of the affine table the G term reads: table[d - 1] = d G
+template <class F> B2_HD Affine<F> ecdsa_g_multiple(const Affine<F>& g, uint32_t d) {
+  const uint32_t k[8] = {d, 0, 0, 0, 0, 0, 0, 0};
+  return xyzz_to_affine(xyzz_scalar_mul(k, g));
+}
 B2_HD Affine<SecpFp> secp_g_multiple(uint32_t d) {
   Affine<SecpFp> g;
   secp::load_const(g.x.v, secp::GX);
   secp::load_const(g.y.v, secp::GY);
-  const uint32_t k[8] = {d, 0, 0, 0, 0, 0, 0, 0};
-  return xyzz_to_affine(xyzz_scalar_mul(k, g));
+  return ecdsa_g_multiple(g, d);
 }
 
 // width-5 NAF of k < 2^256: k = sum naf[i] 2^i, every nonzero digit odd with |digit| < 16; 257 digits
@@ -386,29 +389,30 @@ B2_HD void secp_wnaf(const uint32_t* k, int8_t* naf) {
 
 // u1 G + u2 R in one MSB-first loop: one shared doubling per bit (257 steps, the first on the identity, so at most 256
 // doublings), an XYZZ addition of +-(odd multiple of R) per nonzero wNAF digit of u2, and a mixed addition of
-// gtab[w - 1] per nonzero window w of u1 at the window's lowest bit
-B2_HD XYZZ<SecpFp> secp_lincomb(const uint32_t* u1, const uint32_t* u2, const Affine<SecpFp>& r, const Affine<SecpFp>* gtab) {
-  XYZZ<SecpFp> rt[kSecpRTable];
+// gtab[w - 1] per nonzero window w of u1 at the window's lowest bit.  r is a curve point other than the identity; the
+// curve enters only through the field F (and its CurveA / CurveB).
+template <class F> B2_HD XYZZ<F> secp_lincomb(const uint32_t* u1, const uint32_t* u2, const Affine<F>& r, const Affine<F>* gtab) {
+  XYZZ<F> rt[kSecpRTable];
   rt[0] = xyzz_from_affine(r);
-  const XYZZ<SecpFp> r2 = xyzz_mdbl(r.x, r.y);
+  const XYZZ<F> r2 = xyzz_mdbl(r.x, r.y);
   for (int i = 1; i < kSecpRTable; ++i) { rt[i] = rt[i - 1]; xyzz_add(rt[i], r2); }
   int8_t naf[257];
   secp_wnaf(u2, naf);
-  XYZZ<SecpFp> acc = XYZZ<SecpFp>::identity();
+  XYZZ<F> acc = XYZZ<F>::identity();
 #pragma unroll 1
   for (int i = 256; i >= 0; --i) {
     acc = xyzz_dbl(acc);
     const int d = naf[i];
     if (d) {
-      XYZZ<SecpFp> q = rt[(d < 0 ? -d : d) >> 1];
-      if (d < 0) q.y = SecpFp::neg(q.y);
+      XYZZ<F> q = rt[(d < 0 ? -d : d) >> 1];
+      if (d < 0) q.y = F::neg(q.y);
       xyzz_add(acc, q);
     }
     if (i % kSecpGWindow == 0 && i < 256) {
       const uint64_t two = u1[i >> 5] | (i < 224 ? (uint64_t)u1[(i >> 5) + 1] << 32 : 0);  // a window may cross a limb
       const uint32_t w = (uint32_t)(two >> (i & 31)) & ((1u << kSecpGWindow) - 1);
       if (w) {
-        const Affine<SecpFp> g = gtab[w - 1];
+        const Affine<F> g = gtab[w - 1];
         xyzz_add_mixed(acc, g.x, g.y);
       }
     }

@@ -1,0 +1,72 @@
+// secp256r1.cu -- batched P256VERIFY on the device: Crypto::secp256r1_verify of the reference
+// (crates/common/crypto/provider.rs:415-459, levm p_256_verify, EIP-7951), `count` independent items per call, one thread
+// per item.  The arithmetic, the curve and the rules of each check are in secp256r1.cuh; this file holds the kernels, the
+// per-context table of G multiples and the C entry point.
+#include "common.cuh"
+#include "secp256r1.cuh"
+
+namespace b200zk {
+namespace {
+
+constexpr int kVerifyThreads = 128;
+
+// table[d - 1] = d G for d = 1 .. 4095, one thread per entry; built once per context
+__global__ void __launch_bounds__(256) secp256r1_gtab_build(Affine<P256Fp>* table) {
+  const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x + 1;
+  if (d > kSecpGTable) return;
+  table[d - 1] = p256_g_multiple(d);
+}
+
+// one thread per item: 160 input bytes, one result byte (1 = verified)
+__global__ void __launch_bounds__(kVerifyThreads) secp256r1_verify_kernel(const uint8_t* __restrict__ inputs, size_t n,
+                                                                           const Affine<P256Fp>* __restrict__ gtab, uint8_t* __restrict__ result) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  result[i] = p256_verify(inputs + 160 * i, gtab) ? 1 : 0;
+}
+
+// the G table, built on first use; later calls on any stream wait on its event
+int p256_gtab(b200zk_ctx* ctx, cudaStream_t st, const Affine<P256Fp>** table) {
+  if (!ctx->p256_gtab.p) {
+    B2_TRY(ensure(ctx, ctx->p256_gtab, kSecpGTable * sizeof(Affine<P256Fp>)));
+    B2_LAUNCH(ctx, secp256r1_gtab_build, (kSecpGTable + 255) / 256, 256, 0, st, (Affine<P256Fp>*)ctx->p256_gtab.p);
+    if (cudaEventCreateWithFlags(&ctx->p256_gtab_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(ctx->p256_gtab_ready, st));
+    else { cudaGetLastError(); ctx->p256_gtab_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
+  } else if (ctx->p256_gtab_ready) {
+    B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->p256_gtab_ready, 0));
+  }
+  *table = (const Affine<P256Fp>*)ctx->p256_gtab.p;
+  return B200ZK_OK;
+}
+
+}  // namespace
+}  // namespace b200zk
+
+using namespace b200zk;
+
+extern "C" {
+
+int b200zk_secp256r1_verify_batch(b200zk_ctx* ctx, const uint8_t* inputs, size_t count, uint8_t* result) {
+  if (!ctx) return B200ZK_ERR_INVALID_ARG;
+  if (count && (!inputs || !result)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "secp256r1_verify_batch: null argument");
+  NvtxRange nvtx("b200zk:secp256r1_verify_batch");
+  DeviceGuard guard(ctx);
+  if (!count) return B200ZK_OK;
+  cudaStream_t st = ctx->stream;
+  const Affine<P256Fp>* gtab;
+  B2_TRY(p256_gtab(ctx, st, &gtab));
+  uint8_t *din, *dres;
+  Carve c;
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+    din = c.take<uint8_t>(160 * count); dres = c.take<uint8_t>(count);
+  }
+  B2_CUDA(ctx, cudaMemcpyAsync(din, inputs, 160 * count, cudaMemcpyHostToDevice, st));
+  B2_LAUNCH(ctx, secp256r1_verify_kernel, (unsigned)((count + kVerifyThreads - 1) / kVerifyThreads), kVerifyThreads, 0, st,
+            (const uint8_t*)din, count, gtab, dres);
+  B2_CUDA(ctx, cudaMemcpyAsync(result, dres, count, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  return B200ZK_OK;
+}
+
+}  // extern "C"

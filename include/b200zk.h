@@ -421,6 +421,23 @@ int b200zk_bls12_381_g2_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 288 B
 int b200zk_secp256k1_ecrecover_batch(b200zk_ctx* ctx, const uint8_t* sigs /* count*65 */, const uint8_t* msgs /* count*32 */,
                                      size_t count, uint32_t flags, uint8_t* out /* count*32 */, uint8_t* status /* count */);
 
+/* ---- secp256r1 (P-256) signature verification (P256VERIFY) ---------------------------------------------------------
+ * `count` independent items per call, HOST buffers:
+ *   secp256r1_verify  Crypto::secp256r1_verify, provider.rs:415-459 (levm P256VERIFY 0x0100, precompiles.rs:987-1043,
+ *                     EIP-7951; on every L2 and on L1 from Osaka)
+ * Item i: inputs[160 i ..] = the precompile's calldata h | r | s | qx | qy, five 32-byte big-endian words (the message
+ * hash, the signature, the public key).  result[i] = 1 when the signature verifies, 0 otherwise; as in the trait there is
+ * no per-item status.  The rules, in order (p256 0.13.2's verify_prehash as the provider calls it, and EIP-7951):
+ *   0  r or s outside [1, n - 1] (provider.rs:432-434)
+ *   0  qx >= p or qy >= p (non-canonical encodings are rejected, never reduced)
+ *   0  (qx, qy) not on y^2 = x^3 - 3x + b, (0, 0) included; the cofactor is 1, so there is no subgroup check
+ *   0  R' = (z s^-1) G + (r s^-1) Q is the identity, z = h mod n (the hash as a 256-bit integer)
+ *   1  iff x(R') mod n = r
+ * High s is accepted: (r, s) and (r, n - s) both verify.  The 160-byte length check and the gas stay with the caller.
+ * count = 0 returns 0; null pointers return 4 with b200zk_last_error set.  The table of G multiples the call reads is
+ * built on the device on the context's first call (256 KB, kept until b200zk_destroy). */
+int b200zk_secp256r1_verify_batch(b200zk_ctx* ctx, const uint8_t* inputs /* count*160 */, size_t count, uint8_t* result /* count */);
+
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:
  *   bn254_g1_add         crates/common/crypto/provider.rs:201-234   (levm ecadd,     crates/vm/levm/src/precompiles.rs:692-716)

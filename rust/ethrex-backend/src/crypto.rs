@@ -1,6 +1,7 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
 //! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`) and its
-//! BLS12-381 pairing check (`provider.rs:642-672`) and its secp256k1 signer recovery (`provider.rs:63-171`) on the GPU.  The trait is one item per call; a provider that wants
+//! BLS12-381 pairing check (`provider.rs:642-672`), its secp256k1 signer recovery (`provider.rs:63-171`) and its P-256
+//! signature verification (`provider.rs:415-459`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
 //!
@@ -62,7 +63,32 @@ pub fn recover_signers_batch(items: &[([u8; 65], [u8; 32])]) -> Vec<Result<Addre
     }
 }
 
+/// P256VERIFY (EIP-7951) for a block's calls in one device call.  Each item is what `Crypto::secp256r1_verify` takes:
+/// the 32-byte message hash, r | s and qx | qy; the results are in item order.  The trait has no error channel, so a
+/// device error makes every item `false`.
+pub fn verify_p256_batch(items: &[([u8; 32], [u8; 64], [u8; 64])]) -> Vec<bool> {
+    let mut inputs = Vec::with_capacity(items.len().saturating_mul(160));
+    for (msg, sig, pk) in items {
+        inputs.extend_from_slice(msg);
+        inputs.extend_from_slice(sig);
+        inputs.extend_from_slice(pk);
+    }
+    let res = global()
+        .map_err(device_error)
+        .and_then(|g| g.lock().map_err(device_error))
+        .and_then(|mut gpu| gpu.secp256r1_verify_batch(&inputs).map_err(device_error));
+    match res {
+        Ok(v) if v.len() == items.len() => v,
+        _ => vec![false; items.len()],
+    }
+}
+
 impl Crypto for B200Crypto {
+    /// The rules and their order are in include/b200zk.h (p256's `verify_prehash` as the reference calls it, EIP-7951).
+    fn secp256r1_verify(&self, msg: &[u8; 32], sig: &[u8; 64], pk: &[u8; 64]) -> bool {
+        verify_p256_batch(&[(*msg, *sig, *pk)]).first().copied().unwrap_or(false)
+    }
+
     /// Follows the reference's default (libsecp256k1) path, recids 2 and 3 included; see include/b200zk.h.
     fn secp256k1_ecrecover(&self, sig: &[u8; 64], recid: u8, msg: &[u8; 32]) -> Result<[u8; 32], CryptoError> {
         let mut full = [0u8; 65];

@@ -413,6 +413,20 @@ impl B200zk {
             .collect())
     }
 
+    /// `count` independent P256VERIFY items (EIP-7951): `inputs` = count x 160 bytes, the precompile's calldata
+    /// h | r | s | qx | qy (32-byte big-endian words).  Per item `true` when the signature verifies.
+    pub fn secp256r1_verify_batch(&mut self, inputs: &[u8]) -> Result<Vec<bool>, BackendError> {
+        if inputs.len() % 160 != 0 {
+            return Err(BackendError::serialization("secp256r1_verify_batch: inputs must be count x 160 bytes"));
+        }
+        let count = inputs.len() / 160;
+        let mut res = vec![0u8; count];
+        // SAFETY: `inputs` holds count x 160 bytes and `res` count, both outliving the synchronous call.
+        let status = unsafe { sys::b200zk_secp256r1_verify_batch(self.ctx.as_ptr(), inputs.as_ptr(), count, res.as_mut_ptr()) };
+        check(self, status)?;
+        Ok(res.into_iter().map(|r| r == 1).collect())
+    }
+
     fn bls12_381_add_batch(
         &mut self,
         a: &[u8],
