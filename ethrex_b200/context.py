@@ -464,6 +464,28 @@ class Context:
                     "b200zk_kzg_verify_blob_proof_batch")
         return valid.value == 1
 
+    # ------------------------------------------------------------------ EIP-7594 cells (PeerDAS, wrapper version 1)
+    def kzg_compute_cells(self, blobs) -> list:
+        """blobs: k x 131072 bytes -> k lists of 128 cells, 2048 bytes each (64 x 32-byte big-endian elements)"""
+        k = self._blob_count(blobs)
+        bp, keep = _host_ptr(blobs) if k else (None, None)
+        out = C.create_string_buffer(max(1, 262144 * k))
+        self._check(F.lib.b200zk_kzg_compute_cells(self._h, bp, k, out), "b200zk_kzg_compute_cells")
+        raw = out.raw
+        return [[raw[262144 * b + 2048 * c:262144 * b + 2048 * (c + 1)] for c in range(128)] for b in range(k)]
+
+    def kzg_verify_cell_proof_batch(self, g1_setup: int, g2_setup: int, blobs, commitments, proofs) -> bool:
+        """blobs: k x 131072 bytes, commitments k x 48 bytes, proofs k x 128 x 48 bytes (blob-major, cell index inner) ->
+        one bool for every cell of every blob"""
+        k = self._blob_count(blobs)
+        _need(commitments, 48 * k, "b200zk_kzg_verify_cell_proof_batch commitments")
+        _need(proofs, 128 * 48 * k, "b200zk_kzg_verify_cell_proof_batch proofs")
+        bufs = [_host_ptr(b) if _host_len(b) else (None, None) for b in (blobs, commitments, proofs)]
+        valid = C.c_int(-1)
+        self._check(F.lib.b200zk_kzg_verify_cell_proof_batch(self._h, g1_setup, g2_setup, *[p for p, _ in bufs], k, C.byref(valid)),
+                    "b200zk_kzg_verify_cell_proof_batch")
+        return valid.value == 1
+
     # ------------------------------------------------------------------ NTT root of unity (SURVEY.md section 8c)
     NTT_ROOT_ARK, NTT_ROOT_HALO2 = 0, 1
 

@@ -26,6 +26,12 @@ B2_D Fr381 load_be32(const uint8_t* in) {  // 32-byte big-endian integer -> cano
   return v;
 }
 
+B2_D void store_be32(uint8_t* out, const Fr381& canonical) {  // load_be32's inverse (out 4-byte aligned)
+  uint32_t* o = reinterpret_cast<uint32_t*>(out);
+#pragma unroll
+  for (int k = 0; k < 8; ++k) o[k] = __byte_perm(canonical.v[7 - k], 0, 0x0123);
+}
+
 B2_D Fp381 fp381_half() {
   Fp381 h;
 #pragma unroll

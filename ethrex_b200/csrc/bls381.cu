@@ -65,12 +65,6 @@ constexpr uint32_t kBlobN = 4096;      // FIELD_ELEMENTS_PER_BLOB
 constexpr uint32_t kEvalThreads = 256;  // one CTA per blob, 16 elements per thread: element k * 256 + t belongs to thread t
 constexpr size_t kEvalSmem = (kBlobN + 2 * kEvalThreads) * 32;  // per-element products / inverses + a 512-node product tree
 
-B2_D void store_be32(uint8_t* out, const Fr381& canonical) {
-  uint32_t* o = reinterpret_cast<uint32_t*>(out);
-#pragma unroll
-  for (int k = 0; k < 8; ++k) o[k] = __byte_perm(canonical.v[7 - k], 0, 0x0123);
-}
-
 // roots[i] = w^brp(i), i < 4096, w = 7^((r-1)/4096) (c-kzg's g1_lagrange_brp order); roots[4096] = 1/4096 = r - (r-1)/4096.
 // Montgomery form.  One thread per entry, each deriving w from its definition: a one-off per context.
 __global__ void __launch_bounds__(256) kzg_roots_build(void* __restrict__ roots) {

@@ -397,6 +397,20 @@ __global__ void __launch_bounds__(32) kzg_blob_fold(const XYZZ<Fp381>* terms, si
   pst[1] = p2.is_inf() ? kTrivial : 0;
 }
 
+// verify_cell_kzg_proof_batch from its three MSMs (parts: sum r^k pi_k | the commitments' and r^k h_k^64 pi_k terms |
+// [sum r^k I_k(tau)]1): P[0] = parts[1] - parts[2], paired with G2; P[1] = -parts[0], paired with [tau^64]2
+__global__ void __launch_bounds__(32) kzg_cell_fold(const XYZZ<Fp381>* parts, Affine<Fp381>* P, uint8_t* pst) {
+  if (blockIdx.x || threadIdx.x) return;
+  XYZZ<Fp381> b = parts[1], i = parts[2];
+  i.y = Fp381::neg(i.y);
+  xyzz_add(b, i);
+  const Affine<Fp381> p1 = xyzz_to_affine(b), p2 = affine_neg(xyzz_to_affine(parts[0]));
+  P[0] = p1;
+  P[1] = p2;
+  pst[0] = p1.is_inf() ? kTrivial : 0;
+  pst[1] = p2.is_inf() ? kTrivial : 0;
+}
+
 // ---- host side ----------------------------------------------------------------------------------------------------------
 size_t g2_lines_offset(size_t n) { return (n * sizeof(Affine<F2>) + 255) & ~(size_t)255; }
 const BlsLine* g2_setup_lines(const BasesEntry& e) { return reinterpret_cast<const BlsLine*>((const uint8_t*)e.d + g2_lines_offset(e.n)); }
@@ -615,6 +629,107 @@ int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const
   B2_LAUNCH(ctx, kzg_blob_terms, (unsigned)((n + 63) / 64), 64, 0, st, (const Affine<Fp381>*)pts, (const uint8_t*)zb, (const uint8_t*)yb, (const uint8_t*)rho, n, terms);
   B2_LAUNCH(ctx, kzg_blob_fold, 1, 32, 0, st, (const XYZZ<Fp381>*)terms, n, P, pst);
   B2_TRY(pairing_run(ctx, P, g2_setup_lines(*e), 2, pst, 2, offs, 1, f, res, sts, st));
+  uint8_t h_res = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(&h_res, res, 1, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  *valid = h_res ? 1 : 0;
+  return B200ZK_OK;
+}
+
+int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const uint8_t* blobs, const uint8_t* commitments,
+                                       const uint8_t* proofs, size_t n, int* valid) {
+  static const char* what = "kzg_verify_cell_proof_batch";
+  constexpr size_t kN = 4096, kBlob = kN * 32, kCells = 128, kExt = 2 * kBlob, kCell = kExt / kCells;
+  if (!ctx || !valid || (n && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: null argument");
+  NvtxRange nvtx("b200zk:kzg_verify_cell_proof_batch");
+  DeviceGuard guard(ctx);
+  auto g1 = ctx->bases.find(g1_setup);
+  if (g1 == ctx->bases.end() || !g1->second.bls || g1->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: unknown G1 setup handle");
+  if (g1->second.n != kN) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G1 setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
+  const BasesEntry* e = nullptr;
+  B2_TRY(kzg_g2_setup(ctx, g2_setup, what, &e));
+  if (e->n < 65) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G2 setup must hold at least 65 points ([tau^64]2 is point 64)");
+  if (!n) { *valid = 1; return B200ZK_OK; }
+  const size_t m = kCells * n;  // cells and proofs
+  cudaStream_t st = ctx->stream;
+  uint8_t *d_blobs, *cells, *in, *pt_st, *rbe, *pst, *res, *sts;
+  void *weights, *partial, *s_proof, *s_lin, *s_setup;
+  Affine<Fp381>*pts, *P;
+  Affine<F2>* q2;
+  XYZZ<Fp381>* parts;
+  BlsLine* lines;
+  Fp12b* f;
+  uint32_t* offs;
+  Carve c;
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+    d_blobs = c.take<uint8_t>(kBlob * n); cells = c.take<uint8_t>(kExt * n); in = c.take<uint8_t>(48 * (n + m));
+    pts = c.take<Affine<Fp381>>(n + m); pt_st = c.take<uint8_t>(n + m); rbe = c.take<uint8_t>(32);
+    weights = c.take<uint4>(2 * 65); partial = c.take<uint4>(2 * 64 * n); s_proof = c.take<uint4>(2 * m); s_lin = c.take<uint4>(2 * (n + m));
+    s_setup = c.take<uint4>(2 * kN); parts = c.take<XYZZ<Fp381>>(3); q2 = c.take<Affine<F2>>(2); lines = c.take<BlsLine>(2 * kLines);
+    P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<Fp12b>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
+  }
+  char msg[160];
+  // 1. every blob element < r (c-kzg blob_to_polynomial inside compute_cells): an error, not a false
+  B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, kBlob * n, cudaMemcpyHostToDevice, st));
+  size_t bad = 0;
+  B2_TRY(bls_scalars_check(ctx, d_blobs, kN * n, true, st, &bad));
+  if (bad < kN * n) {
+    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kN, bad % kN);
+    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+  }
+  // 2. commitments, then proofs: c-kzg validate_kzg_g1 (decompression, subgroup)
+  B2_CUDA(ctx, cudaMemcpyAsync(in, commitments, 48 * n, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(in + 48 * n, proofs, 48 * m, cudaMemcpyHostToDevice, st));
+  B2_LAUNCH(ctx, bls_g1_decode_subgroup, (unsigned)((n + m + 63) / 64), 64, 0, st, (const uint8_t*)in, n + m, pts, pt_st);
+  B2_TRY(kzg_cells_run(ctx, d_blobs, n, cells, st));
+  std::vector<uint8_t> h_st(n + m), h_cells(kExt * n);
+  B2_CUDA(ctx, cudaMemcpyAsync(h_st.data(), pt_st, n + m, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(h_cells.data(), cells, kExt * n, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  for (size_t k = 0; k < n + m; ++k) {
+    if (!h_st[k]) continue;
+    if (k < n) snprintf(msg, sizeof msg, "%s: the commitment of blob %zu ", what, k);
+    else snprintf(msg, sizeof msg, "%s: the proof of blob %zu, cell %zu ", what, (k - n) / kCells, (k - n) % kCells);
+    const std::string text = std::string(msg) + (h_st[k] == B200ZK_ERR_NOT_IN_FIELD ? "has a coordinate >= p" : "has malformed flag bits, is not on the curve or not in the order-r subgroup");
+    return fail(ctx, h_st[k], text.c_str());
+  }
+  // 3. r = hash_to_bls_field(SHA-256("RCKZGCBATCH__V1_" | 4096, 64, n, 128 n as u64 BE | the commitments | for each cell:
+  //    its commitment index and cell index as u64 BE, its 64 elements, its proof)): the spec's compute_verify_cell_kzg_
+  //    proof_batch_challenge, with the commitments listed per blob rather than deduplicated
+  static const uint8_t kDomain[16] = {'R', 'C', 'K', 'Z', 'G', 'C', 'B', 'A', 'T', 'C', 'H', '_', '_', 'V', '1', '_'};
+  auto put64 = [](uint8_t* o, uint64_t v) { for (int k = 0; k < 8; ++k) o[7 - k] = (uint8_t)(v >> (8 * k)); };
+  uint8_t lens[32];
+  put64(lens, kN); put64(lens + 8, kCell / 32); put64(lens + 16, n); put64(lens + 24, m);
+  Sha256 h;
+  h.update(kDomain, 16);
+  h.update(lens, 32);
+  h.update(commitments, 48 * n);
+  for (size_t k = 0; k < m; ++k) {
+    uint8_t idx[16];
+    put64(idx, k / kCells); put64(idx + 8, k % kCells);
+    h.update(idx, 16);
+    h.update(&h_cells[(k / kCells) * kExt + (k % kCells) * kCell], kCell);
+    h.update(proofs + 48 * k, 48);
+  }
+  uint8_t digest[32], h_r[32];
+  h.final(digest);
+  hash_to_bls_field(digest, h_r);
+  // 4. the scalars on the device; 5. three MSMs: sum r^k pi_k, the commitments' and r^k h_k^64 pi_k terms, and
+  //    [sum r^k I_k(tau)]1 over the Lagrange setup; 6. one 2-pair check against (G2, [tau^64]2)
+  B2_CUDA(ctx, cudaMemcpyAsync(rbe, h_r, 32, cudaMemcpyHostToDevice, st));
+  B2_TRY(kzg_cell_scalars_run(ctx, d_blobs, n, rbe, weights, partial, s_proof, s_lin, s_setup, st));
+  B2_TRY(msm_run_bls(ctx, pts + n, s_proof, m, 0, st, parts));
+  B2_TRY(msm_run_bls(ctx, pts, s_lin, n + m, 0, st, parts + 1));
+  B2_TRY(msm_run_bls(ctx, g1->second.d, s_setup, kN, 0, st, parts + 2, g1->second.table_c, g1->second.n));
+  B2_LAUNCH(ctx, kzg_cell_fold, 1, 32, 0, st, (const XYZZ<Fp381>*)parts, P, pst);
+  const Affine<F2>* g2pts = (const Affine<F2>*)e->d;
+  B2_CUDA(ctx, cudaMemcpyAsync(q2, g2pts, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(q2 + 1, g2pts + 64, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
+  B2_LAUNCH(ctx, bls_g2_prepare, 1, 64, 0, st, (const Affine<F2>*)q2, (const uint8_t*)nullptr, (size_t)2, lines);
+  const uint32_t h_offs[2] = {0, 2};
+  B2_CUDA(ctx, cudaMemcpyAsync(offs, h_offs, 8, cudaMemcpyHostToDevice, st));
+  B2_TRY(pairing_run(ctx, P, lines, 2, pst, 2, offs, 1, f, res, sts, st));
   uint8_t h_res = 0;
   B2_CUDA(ctx, cudaMemcpyAsync(&h_res, res, 1, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));

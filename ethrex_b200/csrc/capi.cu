@@ -220,6 +220,8 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   if (ctx->ws_kzg.p) cudaFree(ctx->ws_kzg.p);
   if (ctx->ws_pairing.p) cudaFree(ctx->ws_pairing.p);
   if (ctx->kzg_roots_ready) cudaEventDestroy(ctx->kzg_roots_ready);
+  if (ctx->kzg_cells_tw.p) cudaFree(ctx->kzg_cells_tw.p);
+  if (ctx->kzg_cells_tw_ready) cudaEventDestroy(ctx->kzg_cells_tw_ready);
   if (ctx->secp_gtab.p) cudaFree(ctx->secp_gtab.p);
   if (ctx->secp_gtab_ready) cudaEventDestroy(ctx->secp_gtab_ready);
   if (ctx->p256_gtab.p) cudaFree(ctx->p256_gtab.p);

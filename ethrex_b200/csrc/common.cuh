@@ -66,12 +66,16 @@ struct b200zk_ctx {
   b200zk::DevBuf ws_zinv;     // 1/(5^n - 1) of the last quotient domain, canonical limbs (cached per log_n)
   uint32_t zinv_log_n = 0xffffffffu;
   // cudaFuncSetAttribute (opt-in to > 48 KiB dynamic shared memory) is per DEVICE: remembered per context, not per process
-  bool attr_sort = false, attr_acc = false, attr_ntt512 = false, attr_ntt256 = false, attr_kzg = false;
+  bool attr_sort = false, attr_acc = false, attr_ntt512 = false, attr_ntt256 = false, attr_kzg = false, attr_kzg_cells = false;
   // EIP-4844 proofs (bls381.cu): the blob domain's 4096 roots of unity in bit-reversed order, then 1/4096 (Fr381
   // Montgomery), built once per context; consumers on other streams wait on kzg_roots_ready.  ws_kzg: blobs, z, quotients,
   // partial sums and encoded results of one call
   b200zk::DevBuf kzg_roots, ws_kzg;
   cudaEvent_t kzg_roots_ready = nullptr;
+  // EIP-7594 cells (kzg_cells.cu): w^i for the 8192nd root w, i < 8192, then 1/4096 (Fr381 Montgomery), built once per
+  // context; consumers on other streams wait on kzg_cells_tw_ready
+  b200zk::DevBuf kzg_cells_tw;
+  cudaEvent_t kzg_cells_tw_ready = nullptr;
   b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
                               // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu) and
                               // P256VERIFY (secp256r1.cu) batches
@@ -296,5 +300,12 @@ int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint3
 void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]);
 void hash_to_bls_field(const uint8_t digest[32], uint8_t out_be[32]);
 int kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st);
+// EIP-7594 (kzg_cells.cu): the 128 cells of n blobs (checked < r), n x 8192 x 32 bytes big-endian; and from the challenge
+// r (32-byte big-endian, < r) the scalars of the batched cell-proof check, canonical little-endian limbs: s_proof (128 n)
+// = r^k, s_lin (129 n) = the n commitments' sum_c r^(128 b + c), then r^k h_k^64; s_setup (4096) = sum_k r^k I_k on the
+// bit-reversed roots.  Scratch: weights 65 x 32 bytes, partial n x 64 x 32 bytes
+int kzg_cells_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, uint8_t* d_cells, cudaStream_t st);
+int kzg_cell_scalars_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, const uint8_t* d_r_be, void* d_weights, void* d_partial,
+                         void* d_s_proof, void* d_s_lin, void* d_s_setup, cudaStream_t st);
 
 }  // namespace b200zk

@@ -13,11 +13,16 @@ library hashes the challenge itself.  `compute_challenge` below is the same hash
 commitment in.  KzgSettings also accepts a context object that serves only the two MSM calls (`kzg_blob_to_commitment`,
 `bls12_381_g1_msm_resident`); for such an object the proof's scalar-field work is done here in Python integers.  The
 trusted setup is an INPUT (4096 compressed G1 points in c-kzg's g1_lagrange_brp order): the reference gets it from inside the
-c-kzg / kzg-rs crates, which are not in the tree, so no setup is bundled here.  Cell proofs (wrapper version 1) are out of scope.
+c-kzg / kzg-rs crates, which are not in the tree, so no setup is bundled here.
 
 Verification (verify_kzg_proof, verify_blob_kzg_proof, verify_blob_kzg_proof_batch) needs the setup's G2 points as well
 (`g2_monomial`: at least [1]2 and [tau]2, 96-byte compressed) and a `Context`: the pairing runs on the device
 (`b200zk_kzg_verify_proof_batch`, `b200zk_kzg_verify_blob_proof_batch`).
+
+EIP-7594 cells (wrapper version 1, crates/common/crypto/kzg.rs:72-113 of the reference): `compute_cells` extends a blob to
+its 128 cells and `verify_cell_kzg_proof_batch` checks every cell proof of a bundle in one pairing check, both on the
+device (`b200zk_kzg_compute_cells`, `b200zk_kzg_verify_cell_proof_batch`); verification needs `g2_monomial` with all 65
+points ([tau^64]2 is point 64).  Computing cell proofs (FK20) is out of scope.
 """
 from __future__ import annotations
 
@@ -28,6 +33,9 @@ from .errors import B200Error
 BLS_MODULUS = 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001
 FIELD_ELEMENTS_PER_BLOB = 4096
 BYTES_PER_BLOB = 32 * FIELD_ELEMENTS_PER_BLOB
+FIELD_ELEMENTS_PER_CELL = 64
+CELLS_PER_EXT_BLOB = 128
+BYTES_PER_CELL = 32 * FIELD_ELEMENTS_PER_CELL
 FIAT_SHAMIR_PROTOCOL_DOMAIN = b"FSBLOBVERIFY_V1_"
 PRIMITIVE_ROOT_OF_UNITY = 7
 
@@ -191,6 +199,37 @@ class KzgSettings:
             raise ValueError("a blob is 131072 bytes, a commitment and a proof 48 bytes")
         try:
             return self.ctx.kzg_verify_blob_proof_batch(h, b"".join(blobs), b"".join(commitments), b"".join(proofs))
+        except B200Error as e:
+            if e.status in (2, 3):
+                raise ValueError(str(e)) from e
+            raise
+
+    # ---- EIP-7594 cells: kzg.rs:72-113, blobs_bundle.rs:152-173
+    def compute_cells(self, blob: bytes) -> list:
+        """c-kzg compute_cells: the blob's 128 cells of 2048 bytes; the first 64 are the blob itself.  ValueError when a
+        blob element is >= r."""
+        if not hasattr(self.ctx, "kzg_compute_cells"):
+            raise TypeError("compute_cells runs on the device: KzgSettings needs a Context")
+        if len(blob) != BYTES_PER_BLOB:
+            raise ValueError("a blob is 131072 bytes")
+        try:
+            return self.ctx.kzg_compute_cells(blob)[0]
+        except B200Error as e:
+            if e.status == 2:
+                raise ValueError(str(e)) from e
+            raise
+
+    def verify_cell_kzg_proof_batch(self, blobs, commitments, cell_proofs) -> bool:
+        """verify_cell_kzg_proof_batch over whole blobs, as the reference calls it: every cell of every blob, each
+        commitment once per blob, cell_proofs blob-major (128 per blob, cell index inner).  One answer; ValueError on
+        malformed input"""
+        h = self._verifier()
+        if not len(blobs) == len(commitments) or len(cell_proofs) != CELLS_PER_EXT_BLOB * len(blobs):
+            raise ValueError("need one commitment and 128 cell proofs per blob")
+        if any(len(b) != BYTES_PER_BLOB for b in blobs) or any(len(c) != 48 for c in commitments) or any(len(p) != 48 for p in cell_proofs):
+            raise ValueError("a blob is 131072 bytes, a commitment and a proof 48 bytes")
+        try:
+            return self.ctx.kzg_verify_cell_proof_batch(self.handle, h, b"".join(blobs), b"".join(commitments), b"".join(cell_proofs))
         except B200Error as e:
             if e.status in (2, 3):
                 raise ValueError(str(e)) from e

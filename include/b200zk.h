@@ -368,6 +368,35 @@ int b200zk_kzg_verify_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint
 int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint8_t* blobs, const uint8_t* commitments,
                                        const uint8_t* proofs, size_t n, int* valid);
 
+/* ---- EIP-7594 cells (PeerDAS, blob bundles of wrapper version 1) ---------------------------------------------------
+ *   kzg_compute_cells             c-kzg compute_cells, crates/common/crypto/kzg.rs:89-91
+ *   kzg_verify_cell_proof_batch   kzg::verify_cell_kzg_proof_batch, kzg.rs:72-113, reached from BlobsBundle::verify_kzg_proofs
+ *                                 (crates/common/types/blobs_bundle.rs:152-173) for every post-Osaka blob transaction
+ * A blob (4096 x 32-byte big-endian elements, each < r, else status 2 with b200zk_last_error naming the blob) lists p's
+ * values on the 4096 roots of unity in bit-reversed order, root 7^((r-1)/4096).  Its extension lists p on the 8192
+ * roots of unity in bit-reversed order, split into CELLS_PER_EXT_BLOB = 128 cells of FIELD_ELEMENTS_PER_CELL = 64
+ * elements (2048 bytes); cells 0..63 are the blob itself.  Computing cell proofs (FK20) is not offered.
+ * kzg_compute_cells: cells = n_blobs x 128 x 2048 bytes.  n_blobs = 0 returns 0; null pointers with n_blobs > 0: 4. */
+int b200zk_kzg_compute_cells(b200zk_ctx* ctx, const uint8_t* blobs, size_t n_blobs, uint8_t* cells /* n_blobs x 128 x 2048 B */);
+/* verify_cell_kzg_proof_batch over whole blobs, the shape the reference calls it with: every blob's 128 cells, cell
+ * indices 0..127, each commitment standing for its blob's 128 cells; proofs are blob-major, 128 per blob, cell index inner
+ * (48-byte compressed G1 each).  One answer, *valid = 1 or 0, from one two-pairing check of the universal equation
+ *   e(sum r^k pi_k, [tau^64]2) = e(sum_i (sum_(k in blob i) r^k) C_i - [sum r^k I_k(tau)]1 + sum r^k h_k^64 pi_k, [1]2)
+ * with I_k the interpolation polynomial of cell k on its coset h_k <w_64> and r the Fiat-Shamir challenge: SHA-256 of
+ * "RCKZGCBATCH__V1_", the sizes (4096, 64, n_blobs, 128 n_blobs as u64 big-endian), the commitments, then per cell its
+ * blob and cell index (u64 big-endian), its 64 elements and its proof, reduced mod r (the spec's construction; the
+ * commitments are not deduplicated, so r need not equal c-kzg's byte for byte).
+ * g1_setup: the 4096-point Lagrange-form G1 handle of the KZG calls above ([sum r^k I_k(tau)]1 is an MSM over it).
+ * g2_setup: a BLS12-381 G2 handle of at least 65 points whose point 0 is the G2 generator; point 64 is [tau^64]2 (c-kzg's
+ * setup ships 65 g2_monomial points for this).  Anything else returns 4.
+ * Bad input is an error and *valid is not written: a blob element >= r returns 2; a commitment or proof with a coordinate
+ * >= p returns 2; bad flag bits, a point off the curve or outside the order-r subgroup returns 3 (the identity is valid);
+ * b200zk_last_error names the blob (and cell).  Null pointers with n_blobs > 0 return 4.  n_blobs = 0 returns 0 with
+ * *valid = 1. */
+int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const uint8_t* blobs,
+                                       const uint8_t* commitments /* 48 n */, const uint8_t* proofs /* 128 x 48 n */, size_t n_blobs,
+                                       int* valid);
+
 /* ---- EIP-2537 G1/G2 addition and multi-scalar multiplication -------------------------------------------------------
  * The Prague precompiles 0x0b-0x0e, `count` independent items per call, HOST buffers:
  *   bls12_381_g1_add  Crypto::bls12_381_g1_add, provider.rs:549-562 (levm BLS12_G1ADD, precompiles.rs:1056-1107)

@@ -533,6 +533,39 @@ impl B200zk {
         check(self, status)?;
         Ok(valid == 1)
     }
+
+    /// c-kzg `compute_cells` for n blobs: n x 128 cells of 2048 bytes, blob-major; the first 64 cells of a blob are the
+    /// blob itself.  A blob element >= r is an error.
+    pub fn kzg_compute_cells(&mut self, blobs: &[u8]) -> Result<Vec<u8>, BackendError> {
+        const BLOB: usize = 4096 * 32;
+        let n = blobs.len() / BLOB;
+        if blobs.len() % BLOB != 0 {
+            return Err(BackendError::serialization("kzg_compute_cells: blobs must be n x 131072 bytes"));
+        }
+        let mut cells = vec![0u8; 2 * BLOB * n];
+        // SAFETY: `blobs` holds n blobs and `cells` 2 x 131072 bytes per blob.
+        let status = unsafe { sys::b200zk_kzg_compute_cells(self.ctx.as_ptr(), blobs.as_ptr(), n, cells.as_mut_ptr()) };
+        check(self, status)?;
+        Ok(cells)
+    }
+
+    /// `verify_cell_kzg_proof_batch` over whole blobs (every cell, each commitment once per blob, proofs blob-major with
+    /// 128 per blob): one answer; malformed input is an error.  `g1_setup` is the 4096-point Lagrange setup, `g2_setup`
+    /// the setup's 65 G2 points.
+    pub fn kzg_verify_cell_proof_batch(&mut self, g1_setup: u64, g2_setup: u64, blobs: &[u8], commitments: &[u8], proofs: &[u8]) -> Result<bool, BackendError> {
+        const BLOB: usize = 4096 * 32;
+        let n = blobs.len() / BLOB;
+        if blobs.len() % BLOB != 0 || commitments.len() != 48 * n || proofs.len() != 128 * 48 * n {
+            return Err(BackendError::serialization("kzg_verify_cell_proof_batch: need 131072 + 48 + 128 x 48 bytes per blob"));
+        }
+        let mut valid: core::ffi::c_int = 0;
+        // SAFETY: every input holds n blobs' worth of its items; `valid` is a valid out pointer.
+        let status = unsafe {
+            sys::b200zk_kzg_verify_cell_proof_batch(self.ctx.as_ptr(), g1_setup, g2_setup, blobs.as_ptr(), commitments.as_ptr(), proofs.as_ptr(), n, &mut valid)
+        };
+        check(self, status)?;
+        Ok(valid == 1)
+    }
 }
 
 impl Drop for B200zk {
