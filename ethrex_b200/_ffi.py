@@ -112,6 +112,7 @@ SIGNATURES = {
     "b200zk_kzg_verify_proof_batch": (_int, [_ctx, _u64, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_kzg_verify_blob_proof_batch": (_int, [_ctx, _u64, _vp, _vp, _vp, _sz, C.POINTER(_int)]),
     "b200zk_kzg_compute_cells": (_int, [_ctx, _vp, _sz, _vp]),
+    "b200zk_kzg_blob_to_commitment_and_cell_proofs": (_int, [_ctx, _u64, _u64, _vp, _sz, _vp, _vp]),
     "b200zk_kzg_verify_cell_proof_batch": (_int, [_ctx, _u64, _u64, _vp, _vp, _vp, _sz, C.POINTER(_int)]),
     "b200zk_bls12_381_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g2_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

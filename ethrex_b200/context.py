@@ -474,6 +474,16 @@ class Context:
         raw = out.raw
         return [[raw[262144 * b + 2048 * c:262144 * b + 2048 * (c + 1)] for c in range(128)] for b in range(k)]
 
+    def kzg_blob_to_commitment_and_cell_proofs(self, g1_lagrange: int, g1_monomial: int, blobs) -> tuple:
+        """blobs: k x 131072 bytes -> ([48-byte commitments], [48-byte cell proofs]), the proofs blob-major (128 per blob, cell
+        index inner).  g1_monomial: a 4096-point G1 handle of the setup's [tau^i]1 points."""
+        k = self._blob_count(blobs)
+        bp, keep = _host_ptr(blobs) if k else (None, None)
+        cm, pr = C.create_string_buffer(max(1, 48 * k)), C.create_string_buffer(max(1, 128 * 48 * k))
+        self._check(F.lib.b200zk_kzg_blob_to_commitment_and_cell_proofs(self._h, g1_lagrange, g1_monomial, bp, k, cm, pr),
+                    "b200zk_kzg_blob_to_commitment_and_cell_proofs")
+        return [cm.raw[48 * i:48 * i + 48] for i in range(k)], [pr.raw[48 * i:48 * i + 48] for i in range(128 * k)]
+
     def kzg_verify_cell_proof_batch(self, g1_setup: int, g2_setup: int, blobs, commitments, proofs) -> bool:
         """blobs: k x 131072 bytes, commitments k x 48 bytes, proofs k x 128 x 48 bytes (blob-major, cell index inner) ->
         one bool for every cell of every blob"""

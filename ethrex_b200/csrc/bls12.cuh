@@ -148,4 +148,17 @@ B2_D void store_be48(uint8_t* out, const Fp381& canonical) {
   for (int k = 0; k < 12; ++k) w[11 - k] = __byte_perm(canonical.v[k], 0, 0x0123);
 }
 
+// native affine -> the 48-byte compressed form, bls_g1_decompress's inverse; the identity is 0xc0 | 0..0 (out 4-byte aligned)
+B2_D void bls_g1_compress(uint8_t* out, const Affine<Fp381>& p) {
+  if (p.is_inf()) {
+    uint32_t* w = reinterpret_cast<uint32_t*>(out);
+#pragma unroll
+    for (int k = 0; k < 12; ++k) w[k] = 0;
+    out[0] = 0xc0;
+    return;
+  }
+  store_be48(out, Fp381::from_mont(p.x));
+  out[0] |= 0x80 | (Fp381::less(fp381_half(), Fp381::from_mont(p.y)) ? 0x20 : 0x00);
+}
+
 }  // namespace b200zk

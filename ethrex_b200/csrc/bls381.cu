@@ -281,8 +281,10 @@ int kzg_check_inputs(b200zk_ctx* ctx, const KzgLayout& L, size_t n, bool with_z,
   return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
 }
 
+}  // namespace
+
 // one 4096-point MSM per blob over the setup, each encoded into its own 128-byte slot of `enc`
-int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_t n, uint32_t flags, uint8_t* partials, uint8_t* enc, cudaStream_t st) {
+int b200zk::kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_t n, uint32_t flags, uint8_t* partials, uint8_t* enc, cudaStream_t st) {
   for (size_t b = 0; b < n; ++b) {
     B2_TRY(msm_run_bls(ctx, e.d, scalars + b * kBlobN * 32, kBlobN, flags, st, partials + b * KzgLayout::kPartial, e.table_c, e.n));
     B2_TRY(msm_encode_bls(ctx, partials + b * KzgLayout::kPartial, 1, 0, st, enc + b * KzgLayout::kEnc));
@@ -290,14 +292,8 @@ int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_
   return B200ZK_OK;
 }
 
-// z of every blob in L.z, checked: y into L.y, the proofs' encodings into enc
-int kzg_proofs(b200zk_ctx* ctx, const BasesEntry& e, const KzgLayout& L, size_t n, uint8_t* enc, cudaStream_t st) {
-  B2_TRY(kzg_eval_run(ctx, L.blobs, L.z, n, L.q, L.y, st));
-  return kzg_msms(ctx, e, L.q, n, 0 /* little-endian limbs */, L.partials + n * KzgLayout::kPartial, enc, st);
-}
-
 // the setup handle of a KZG call: a BLS12-381 G1 handle of exactly 4096 points
-int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e) {
+int b200zk::kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e) {
   auto it = ctx->bases.find(handle);
   std::string msg = what;
   if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": unknown setup handle").c_str());
@@ -306,6 +302,12 @@ int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEnt
   return B200ZK_OK;
 }
 
+namespace {
+// z of every blob in L.z, checked: y into L.y, the proofs' encodings into enc
+int kzg_proofs(b200zk_ctx* ctx, const BasesEntry& e, const KzgLayout& L, size_t n, uint8_t* enc, cudaStream_t st) {
+  B2_TRY(kzg_eval_run(ctx, L.blobs, L.z, n, L.q, L.y, st));
+  return kzg_msms(ctx, e, L.q, n, 0 /* little-endian limbs */, L.partials + n * KzgLayout::kPartial, enc, st);
+}
 }  // namespace
 
 // EIP-4844 compute_challenge: hash_to_bls_field(SHA-256("FSBLOBVERIFY_V1_" | 4096 as 16-byte big-endian | blob | commitment))

@@ -241,7 +241,11 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   for (auto& e : ctx->ev_up) if (e) cudaEventDestroy(e);
   if (ctx->stream_sort) cudaStreamDestroy(ctx->stream_sort);
   for (auto& kv : ctx->twiddles) { cudaFree(kv.second.d); if (kv.second.ready) cudaEventDestroy(kv.second.ready); }
-  for (auto& kv : ctx->bases) cudaFree(kv.second.d);
+  for (auto& kv : ctx->bases) {
+    cudaFree(kv.second.d);
+    if (kv.second.fk20) cudaFree(kv.second.fk20);
+    if (kv.second.fk20_ready) cudaEventDestroy(kv.second.fk20_ready);
+  }
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -338,6 +342,8 @@ int b200zk_bases_free(b200zk_ctx* ctx, uint64_t handle) { b200zk::DeviceGuard gu
   if (it == ctx->bases.end()) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_free: unknown handle");
   B2_CUDA(ctx, cudaDeviceSynchronize());
   cudaFree(it->second.d);
+  if (it->second.fk20) cudaFree(it->second.fk20);
+  if (it->second.fk20_ready) cudaEventDestroy(it->second.fk20_ready);
   ctx->bases.erase(it);
   return B200ZK_OK;
 }

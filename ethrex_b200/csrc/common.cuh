@@ -44,6 +44,10 @@ struct BasesEntry {
                          // (Fp2 over Fp381, 192 B affine), followed by the prepared Miller-loop lines of points 0 and 1
   bool g2_gen0 = false;  // BLS12-381 G2: point 0 is the generator (so point 1 is [tau]2 of a KZG setup)
   uint32_t table_c = 0;  // != 0: d holds W = ceil(255/c) windows of n points: 2^(c*w) * P_i at w*n + i
+  // a 4096-point BLS12-381 G1 monomial setup used for EIP-7594 cell proofs (kzg_cells.cu): its FK20 table, 64 x 128 native
+  // affine points, built on the handle's first such call and freed with it; consumers on other streams wait on fk20_ready
+  void* fk20 = nullptr;
+  cudaEvent_t fk20_ready = nullptr;
 };
 
 }  // namespace b200zk
@@ -300,6 +304,11 @@ int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint3
 void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]);
 void hash_to_bls_field(const uint8_t digest[32], uint8_t out_be[32]);
 int kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st);
+// the setup handle of a KZG call: a BLS12-381 G1 handle of exactly 4096 points, else status 4 naming `what`
+int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e);
+// one 4096-point MSM per blob over the setup (scalars n x 4096 x 32 bytes): XYZZ partial sums 192 B apart, each encoded into
+// its own 128-byte slot of enc (the 48-byte compressed point first)
+int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_t n, uint32_t flags, uint8_t* partials, uint8_t* enc, cudaStream_t st);
 // EIP-7594 (kzg_cells.cu): the 128 cells of n blobs (checked < r), n x 8192 x 32 bytes big-endian; and from the challenge
 // r (32-byte big-endian, < r) the scalars of the batched cell-proof check, canonical little-endian limbs: s_proof (128 n)
 // = r^k, s_lin (129 n) = the n commitments' sum_c r^(128 b + c), then r^k h_k^64; s_setup (4096) = sum_k r^k I_k on the

@@ -10,6 +10,7 @@
 // 256 KiB of the full extension never has to sit in one CTA.
 #include "bls12.cuh"
 #include <cstring>
+#include <vector>
 
 namespace b200zk {
 namespace {
@@ -173,6 +174,180 @@ __global__ void __launch_bounds__(256) kzg_cells_scalars(const void* __restrict_
   store_fe(s_lin, k, Fr381::from_mont(Fr381::mul(rq, tw_at(tw, kCellN * brp7((uint32_t)(q % kCells))))));
 }
 
+// ---- cell proofs by FK20 (c-kzg compute_cells_and_kzg_proofs) --------------------------------------------------------
+// pi_k = [q_k(tau)]1, q_k = (p - I_k) / (X^64 - s_k), is sum_(m=1..63) s_k^(m-1) T_m with the Toeplitz sums
+//   T_m = sum_(i <= 4095 - 64 m) c_(i + 64 m) [tau^i]1 = sum_b sum_(a <= 63 - m) C_b[a + m] S_b[a],
+// C_b[t] = c_(64 t + b), S_b[a] = [tau^(64 a + b)]1.  Per column b that is a circular convolution of length 128 of C_b
+// (zero-padded) with S''_b (S''_b[0] = S_b[0], S''_b[128 - a] = S_b[a] for a = 1..63, else O) that never wraps for m < 64, so
+//   table[b] = DFT(S''_b) (once per setup),  u = sum_b DFT(C_b) table[b],  T_m = DFT^-1(u)[m],
+// and the 128 proofs are one more DFT of (T_1 .. T_63, O ..), since s_k = w_128^brp7(k).  All DFTs have size 128 and root
+// w_128 = w_8192^64.  Forward DFTs are Gentleman-Sande (natural in, bit-reversed out) and the inverse is Cooley-Tukey
+// (bit-reversed in, natural out), as the NTTs above: the column DFTs and the table are both bit-reversed, the pointwise
+// sums need no permutation, and the last DFT leaves pi_k at position k.  tests/fk20_ref.py restates every step in scalars.
+constexpr uint32_t kDft = 128;            // the circulant's size
+constexpr uint32_t kColGroup = 16;        // columns per pass of kzg_fk20_columns: 4096 coefficients + 16 x 128 in shared memory
+constexpr size_t kColSmem = (kN + kColGroup * kDft) * 32;
+constexpr uint32_t kMsmWarps = 4;         // kzg_fk20_msm: one warp per (blob, position) MSM of 64 terms
+
+B2_D XYZZ<Fp381> xyzz_neg(const XYZZ<Fp381>& p) { return {p.x, Fp381::neg(p.y), p.zz, p.zzz}; }
+
+// k P for a canonical scalar k < r < 2^255 (double-and-add, MSB first): the twiddle products of the G1 DFTs
+B2_D XYZZ<Fp381> xyzz_mul_fr(const XYZZ<Fp381>& p, const Fr381& k) {
+  XYZZ<Fp381> acc = XYZZ<Fp381>::identity();
+#pragma unroll 1
+  for (int i = 254; i >= 0; --i) {
+    acc = xyzz_dbl(acc);
+    if ((k.v[i >> 5] >> (i & 31)) & 1) xyzz_add(acc, p);
+  }
+  return acc;
+}
+
+// In place over 128 XYZZ points in s, 64 threads (one butterfly each per stage), s written and synchronised by the caller.
+// Forward, Gentleman-Sande: natural order in, DFT[brp7(i)] at position i.  A butterfly of twiddle 1 (j = 0) multiplies nothing.
+B2_D void g1_dft_forward(void* s, const void* tw) {
+  for (uint32_t h = kDft / 2; h >= 1; h >>= 1) {
+    const uint32_t b = threadIdx.x, j = b & (h - 1), i0 = 2 * b - j, i1 = i0 + h;
+    XYZZ<Fp381> u = load_xyzz<Fp381>(s, i0);
+    const XYZZ<Fp381> v = load_xyzz<Fp381>(s, i1);
+    XYZZ<Fp381> d = xyzz_neg(v);
+    xyzz_add(d, u);
+    xyzz_add(u, v);
+    store_xyzz<Fp381>(s, i0, u);
+    if (j) d = xyzz_mul_fr(d, Fr381::from_mont(tw_at(tw, j * (kExtN / (2 * h)))));
+    store_xyzz<Fp381>(s, i1, d);
+    __syncthreads();
+  }
+}
+// Inverse, Cooley-Tukey, root w_128^-1, unscaled: bit-reversed order in, natural order out
+B2_D void g1_dft_inverse(void* s, const void* tw) {
+  for (uint32_t h = 1; h < kDft; h <<= 1) {
+    const uint32_t b = threadIdx.x, j = b & (h - 1), i0 = 2 * b - j, i1 = i0 + h;
+    XYZZ<Fp381> v = load_xyzz<Fp381>(s, i1);
+    if (j) v = xyzz_mul_fr(v, Fr381::from_mont(tw_at(tw, kExtN - j * (kExtN / (2 * h)))));
+    XYZZ<Fp381> u = load_xyzz<Fp381>(s, i0), d = xyzz_neg(v);
+    xyzz_add(d, u);
+    xyzz_add(u, v);
+    store_xyzz<Fp381>(s, i0, u);
+    store_xyzz<Fp381>(s, i1, d);
+    __syncthreads();
+  }
+}
+
+// One CTA of 64 threads per column b: table[128 b + i] = DFT(S''_b)[brp7(i)] as native affine points.  mono: the monomial
+// setup's points [tau^i]1 (native affine, the first 4096 entries of the handle whether or not it holds window tables).
+__global__ void __launch_bounds__(kDft / 2, 1) kzg_fk20_table(const void* __restrict__ mono, const void* __restrict__ tw, void* __restrict__ table) {
+  __shared__ uint4 s_pts[kDft * 12];  // 128 XYZZ points, 192 bytes each
+  const uint32_t b = blockIdx.x, t = threadIdx.x;
+  // k = t: S''[0] = S_b[0], then O; k = 64 + t: O at 64, then S_b[a] for a = 128 - k = 64 - t
+  store_xyzz<Fp381>(s_pts, t, t ? XYZZ<Fp381>::identity() : xyzz_from_affine(load_affine_nc<Fp381>(mono, b)));
+  store_xyzz<Fp381>(s_pts, kCellN + t, t ? xyzz_from_affine(load_affine_nc<Fp381>(mono, kCellN * (kCellN - t) + b)) : XYZZ<Fp381>::identity());
+  __syncthreads();
+  g1_dft_forward(s_pts, tw);
+  store_affine<Fp381>(table, (size_t)kDft * b + t, xyzz_to_affine(load_xyzz<Fp381>(s_pts, t)));
+  store_affine<Fp381>(table, (size_t)kDft * b + kCellN + t, xyzz_to_affine(load_xyzz<Fp381>(s_pts, kCellN + t)));
+}
+
+// One CTA per blob: the coefficients (the inverse NTT of kzg_cells_extend), then the 64 column DFTs, 16 columns per pass.
+// hat[64 (128 blob + i) + b] = DFT(C_b)[brp7(i)] / (4096 * 128), canonical limbs: the scalars of MSM (blob, i), with the
+// blob's 1/4096 and the inverse G1 DFT's 1/128 folded in.
+__global__ void __launch_bounds__(kThreads, 1) kzg_fk20_columns(const uint8_t* __restrict__ blobs, const void* __restrict__ tw, void* __restrict__ hat) {
+  extern __shared__ uint4 cells_smem[];
+  uint4* cols = cells_smem + 2 * kN;
+  load_blob(cells_smem, blobs + (size_t)blockIdx.x * kN * 32);
+  ntt_inverse_brp(cells_smem, tw);
+  const Fr381 ninv = tw_at(tw, kExtN);
+  Fr381 scale = Fr381::mul(ninv, ninv);  // 1/4096^2 = 1/(4096 * 128) / 32
+#pragma unroll 1
+  for (int k = 0; k < 5; ++k) scale = Fr381::dbl(scale);
+  void* out = (uint8_t*)hat + (size_t)blockIdx.x * kDft * kCellN * 32;
+#pragma unroll 1
+  for (uint32_t g = 0; g < kCellN; g += kColGroup) {
+    for (uint32_t e = threadIdx.x; e < kColGroup * kDft; e += kThreads) {
+      const uint32_t q = e / kDft, t = e % kDft;
+      store_fe(cols, e, t < kCellN ? load_fe<Fr381>(cells_smem, kCellN * t + g + q) : Fr381::zero());
+    }
+    __syncthreads();
+    for (uint32_t h = kDft / 2; h >= 1; h >>= 1) {
+      const uint32_t step = kExtN / (2 * h);
+#pragma unroll 1
+      for (uint32_t e = threadIdx.x; e < kColGroup * kDft / 2; e += kThreads) {
+        const uint32_t b = e % (kDft / 2), j = b & (h - 1), i0 = kDft * (e / (kDft / 2)) + 2 * b - j, i1 = i0 + h;
+        const Fr381 u = load_fe<Fr381>(cols, i0), v = load_fe<Fr381>(cols, i1);
+        store_fe(cols, i0, Fr381::add(u, v));
+        store_fe(cols, i1, Fr381::mul(Fr381::sub(u, v), tw_at(tw, j * step)));
+      }
+      __syncthreads();
+    }
+    for (uint32_t e = threadIdx.x; e < kColGroup * kDft; e += kThreads) {
+      const uint32_t q = e / kDft, i = e % kDft;
+      store_fe(out, (size_t)kCellN * i + g + q, Fr381::mul(load_fe<Fr381>(cols, e), scale));
+    }
+    __syncthreads();
+  }
+}
+
+B2_D Fp381 shfl_down_fp(const Fp381& a, uint32_t off) {
+  Fp381 r;
+#pragma unroll
+  for (int k = 0; k < 12; ++k) r.v[k] = __shfl_down_sync(0xffffffffu, a.v[k], off);
+  return r;
+}
+
+// One warp per MSM q = 128 blob + i: u[q] = sum_b hat[64 q + b] table[128 b + i], 64 terms.  Lane l takes b = 2l, 2l + 1
+// with one shared doubling chain (Shamir's trick: P1, P2 or P1 + P2 per bit pair), then the warp sums its 32 lanes.
+__global__ void __launch_bounds__(32 * kMsmWarps) kzg_fk20_msm(const void* __restrict__ table, const void* __restrict__ hat, size_t n_msm, void* __restrict__ u) {
+  const size_t q = (size_t)blockIdx.x * kMsmWarps + threadIdx.x / 32;
+  if (q >= n_msm) return;  // whole warps
+  __shared__ uint4 s_pts[32 * kMsmWarps * 3 * 6];  // per thread P1, P2, P1 + P2 (96-byte affine), out of the registers
+  const uint32_t lane = threadIdx.x % 32, i = (uint32_t)(q % kDft), b0 = 2 * lane, mine = 3 * threadIdx.x;
+  {
+    const Affine<Fp381> p1 = load_affine_nc<Fp381>(table, (size_t)kDft * b0 + i), p2 = load_affine_nc<Fp381>(table, (size_t)kDft * (b0 + 1) + i);
+    XYZZ<Fp381> s12 = xyzz_from_affine(p1);
+    xyzz_add_mixed(s12, p2.x, p2.y);
+    store_affine<Fp381>(s_pts, mine, p1);
+    store_affine<Fp381>(s_pts, mine + 1, p2);
+    store_affine<Fp381>(s_pts, mine + 2, xyzz_to_affine(s12));
+  }
+  const Fr381 k1 = load_fe_nc<Fr381>(hat, kCellN * q + b0), k2 = load_fe_nc<Fr381>(hat, kCellN * q + b0 + 1);
+  const Fp381* f = nullptr;
+  XYZZ<Fp381> acc = XYZZ<Fp381>::identity();
+#pragma unroll 1
+  for (int bit = 254; bit >= 0; --bit) {
+    acc = xyzz_dbl(acc);
+    const uint32_t sel = ((k1.v[bit >> 5] >> (bit & 31)) & 1) | (((k2.v[bit >> 5] >> (bit & 31)) & 1) << 1);
+    if (sel) {
+      const uint32_t at = mine + sel - 1;
+      xyzz_add_mixed(acc, load_field(s_pts, 2 * at, f), load_field(s_pts, 2 * at + 1, f));
+    }
+  }
+#pragma unroll 1
+  for (uint32_t off = 16; off; off >>= 1) {
+    const XYZZ<Fp381> o = {shfl_down_fp(acc.x, off), shfl_down_fp(acc.y, off), shfl_down_fp(acc.zz, off), shfl_down_fp(acc.zzz, off)};
+    xyzz_add(acc, o);
+  }
+  if (!lane) store_xyzz<Fp381>(u, q, acc);
+}
+
+// One CTA of 64 threads per blob: z = DFT^-1(u) (T_m = z[m]), v = (z[1] .. z[63], O ..), the 128 proofs DFT(v) in cell
+// order, normalised and compressed (48 bytes each, blob-major)
+__global__ void __launch_bounds__(kDft / 2, 1) kzg_fk20_proofs(const void* __restrict__ u, const void* __restrict__ tw, uint8_t* __restrict__ proofs) {
+  __shared__ uint4 s_pts[kDft * 12];
+  const uint32_t t = threadIdx.x;
+  const size_t base = (size_t)kDft * blockIdx.x;
+  store_xyzz<Fp381>(s_pts, t, load_xyzz<Fp381>(u, base + t));
+  store_xyzz<Fp381>(s_pts, kCellN + t, load_xyzz<Fp381>(u, base + kCellN + t));
+  __syncthreads();
+  g1_dft_inverse(s_pts, tw);
+  const XYZZ<Fp381> zt = t + 1 < kCellN ? load_xyzz<Fp381>(s_pts, t + 1) : XYZZ<Fp381>::identity();
+  __syncthreads();
+  store_xyzz<Fp381>(s_pts, t, zt);
+  store_xyzz<Fp381>(s_pts, kCellN + t, XYZZ<Fp381>::identity());
+  __syncthreads();
+  g1_dft_forward(s_pts, tw);
+  bls_g1_compress(proofs + 48 * (base + t), xyzz_to_affine(load_xyzz<Fp381>(s_pts, t)));
+  bls_g1_compress(proofs + 48 * (base + kCellN + t), xyzz_to_affine(load_xyzz<Fp381>(s_pts, kCellN + t)));
+}
+
 // the twiddle table, built on first use; later calls on any stream wait on its event
 int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
   if (!ctx->kzg_cells_tw.p) {
@@ -187,9 +362,24 @@ int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_extend, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+    B2_CUDA(ctx, cudaFuncSetAttribute(kzg_fk20_columns, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColSmem));
     ctx->attr_kzg_cells = true;
   }
   *tw = ctx->kzg_cells_tw.p;
+  return B200ZK_OK;
+}
+
+// the FK20 table of a monomial setup, built on the handle's first cell-proof call; later calls on any stream wait on its event
+int fk20_table(b200zk_ctx* ctx, BasesEntry& e, const void* tw, cudaStream_t st, const void** table) {
+  if (!e.fk20) {
+    B2_CUDA(ctx, cudaMalloc(&e.fk20, (size_t)kCellN * kDft * 96));
+    B2_LAUNCH(ctx, kzg_fk20_table, kCellN, kDft / 2, 0, st, (const void*)e.d, tw, e.fk20);
+    if (cudaEventCreateWithFlags(&e.fk20_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(e.fk20_ready, st));
+    else { cudaGetLastError(); e.fk20_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
+  } else if (e.fk20_ready) {
+    B2_CUDA(ctx, cudaStreamWaitEvent(st, e.fk20_ready, 0));
+  }
+  *table = e.fk20;
   return B200ZK_OK;
 }
 
@@ -243,6 +433,52 @@ int b200zk_kzg_compute_cells(b200zk_ctx* ctx, const uint8_t* blobs, size_t n_blo
   B2_TRY(kzg_cells_run(ctx, d_blobs, n_blobs, d_cells, st));
   B2_CUDA(ctx, cudaMemcpyAsync(cells, d_cells, n_blobs * kExtN * 32, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
+  return B200ZK_OK;
+}
+
+int b200zk_kzg_blob_to_commitment_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_lagrange, uint64_t g1_monomial, const uint8_t* blobs, size_t n_blobs,
+                                                  uint8_t* commitments, uint8_t* proofs) {
+  static const char* what = "kzg_blob_to_commitment_and_cell_proofs";
+  if (!ctx || (n_blobs && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment_and_cell_proofs: null argument");
+  NvtxRange nvtx("b200zk:kzg_blob_to_commitment_and_cell_proofs");
+  DeviceGuard guard(ctx);
+  const BasesEntry *lag = nullptr, *mono = nullptr;
+  B2_TRY(kzg_setup(ctx, g1_lagrange, "kzg_blob_to_commitment_and_cell_proofs (g1_lagrange)", &lag));
+  B2_TRY(kzg_setup(ctx, g1_monomial, "kzg_blob_to_commitment_and_cell_proofs (g1_monomial)", &mono));
+  if (!n_blobs) return B200ZK_OK;
+  cudaStream_t st = ctx->stream;
+  uint8_t *d_blobs, *d_hat, *d_u, *d_partials, *d_enc, *d_proofs;
+  Carve c;
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass) { B2_TRY(ensure(ctx, ctx->ws_kzg, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_kzg.p, 0}; }
+    d_blobs = c.take<uint8_t>(n_blobs * kN * 32);
+    d_hat = c.take<uint8_t>(n_blobs * kDft * kCellN * 32);
+    d_u = c.take<uint8_t>(n_blobs * kDft * 192);
+    d_partials = c.take<uint8_t>(n_blobs * 192);
+    d_enc = c.take<uint8_t>(n_blobs * 128);
+    d_proofs = c.take<uint8_t>(n_blobs * kCells * 48);
+  }
+  B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, n_blobs * kN * 32, cudaMemcpyHostToDevice, st));
+  size_t bad = 0;
+  B2_TRY(bls_scalars_check(ctx, d_blobs, n_blobs * kN, true, st, &bad));
+  if (bad < n_blobs * kN) {
+    char msg[160];
+    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kN, bad % kN);
+    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+  }
+  const void *tw = nullptr, *table = nullptr;
+  B2_TRY(cells_tw(ctx, st, &tw));
+  B2_TRY(fk20_table(ctx, ctx->bases[g1_monomial], tw, st, &table));
+  B2_LAUNCH(ctx, kzg_fk20_columns, (unsigned)n_blobs, kThreads, kColSmem, st, (const uint8_t*)d_blobs, tw, (void*)d_hat);
+  const size_t n_msm = n_blobs * kDft;
+  B2_LAUNCH(ctx, kzg_fk20_msm, (unsigned)((n_msm + kMsmWarps - 1) / kMsmWarps), 32 * kMsmWarps, 0, st, table, (const void*)d_hat, n_msm, (void*)d_u);
+  B2_LAUNCH(ctx, kzg_fk20_proofs, (unsigned)n_blobs, kDft / 2, 0, st, (const void*)d_u, tw, d_proofs);
+  B2_TRY(kzg_msms(ctx, *lag, d_blobs, n_blobs, B200ZK_SCALARS_BE, d_partials, d_enc, st));
+  std::vector<uint8_t> enc(n_blobs * 128);
+  B2_CUDA(ctx, cudaMemcpyAsync(enc.data(), d_enc, enc.size(), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(proofs, d_proofs, n_blobs * kCells * 48, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  for (size_t b = 0; b < n_blobs; ++b) memcpy(commitments + 48 * b, &enc[128 * b], 48);
   return B200ZK_OK;
 }
 

@@ -22,7 +22,9 @@ Verification (verify_kzg_proof, verify_blob_kzg_proof, verify_blob_kzg_proof_bat
 EIP-7594 cells (wrapper version 1, crates/common/crypto/kzg.rs:72-113 of the reference): `compute_cells` extends a blob to
 its 128 cells and `verify_cell_kzg_proof_batch` checks every cell proof of a bundle in one pairing check, both on the
 device (`b200zk_kzg_compute_cells`, `b200zk_kzg_verify_cell_proof_batch`); verification needs `g2_monomial` with all 65
-points ([tau^64]2 is point 64).  Computing cell proofs (FK20) is out of scope.
+points ([tau^64]2 is point 64).  `blob_to_commitment_and_cell_proofs` (kzg.rs:275-293, what `BlobsBundle::create_from_blobs`
+calls per blob for wrapper version 1) computes the commitment and the 128 cell proofs by FK20 on the device
+(`b200zk_kzg_blob_to_commitment_and_cell_proofs`); it needs `g1_monomial`, the setup's 4096 points [tau^i]1.
 """
 from __future__ import annotations
 
@@ -62,26 +64,30 @@ def roots_of_unity_brp():
 class KzgSettings:
     """The trusted setup resident in HBM (the reference's `c_kzg::ethereum_kzg_settings(KZG_PRECOMPUTE)`, kzg.rs:262)."""
 
-    def __init__(self, ctx, g1_lagrange_brp: bytes, precompute: bool = True, g2_monomial: bytes | None = None):
+    def __init__(self, ctx, g1_lagrange_brp: bytes, precompute: bool = True, g2_monomial: bytes | None = None,
+                 g1_monomial: bytes | None = None):
         if len(g1_lagrange_brp) != 48 * FIELD_ELEMENTS_PER_BLOB:
             raise ValueError("the setup is 4096 compressed G1 points (48 bytes each) in g1_lagrange_brp order")
         if g2_monomial is not None and (len(g2_monomial) % 96 or len(g2_monomial) < 2 * 96):
             raise ValueError("g2_monomial is at least 2 compressed G2 points (96 bytes each): [1]2, [tau]2, ...")
+        if g1_monomial is not None and len(g1_monomial) != 48 * FIELD_ELEMENTS_PER_BLOB:
+            raise ValueError("g1_monomial is 4096 compressed G1 points (48 bytes each): [tau^i]1 for i < 4096")
         self.ctx = ctx
         self.g2_handle = 0
+        self.g1_monomial_handle = 0
         self.handle = ctx.bls12_381_g1_bases_upload(g1_lagrange_brp, FIELD_ELEMENTS_PER_BLOB)
         if precompute:
             ctx.bases_precompute(self.handle, 0)
         if g2_monomial is not None:
             self.g2_handle = ctx.bls12_381_g2_bases_upload(g2_monomial, len(g2_monomial) // 96)
+        if g1_monomial is not None:
+            self.g1_monomial_handle = ctx.bls12_381_g1_bases_upload(g1_monomial, FIELD_ELEMENTS_PER_BLOB)
 
     def close(self):
-        if self.handle:
-            self.ctx.bases_free(self.handle)
-            self.handle = 0
-        if self.g2_handle:
-            self.ctx.bases_free(self.g2_handle)
-            self.g2_handle = 0
+        for name in ("handle", "g2_handle", "g1_monomial_handle"):
+            if getattr(self, name):
+                self.ctx.bases_free(getattr(self, name))
+                setattr(self, name, 0)
 
     # ---- kzg.rs:259-272
     def blob_to_kzg_commitment(self, blob: bytes) -> bytes:
@@ -214,6 +220,31 @@ class KzgSettings:
             raise ValueError("a blob is 131072 bytes")
         try:
             return self.ctx.kzg_compute_cells(blob)[0]
+        except B200Error as e:
+            if e.status == 2:
+                raise ValueError(str(e)) from e
+            raise
+
+    def blob_to_commitment_and_cell_proofs(self, blob: bytes):
+        """kzg::blob_to_commitment_and_cell_proofs (c-kzg compute_cells_and_kzg_proofs): (commitment, [128 cell proofs]),
+        48 bytes each.  ValueError when a blob element is >= r."""
+        if len(blob) != BYTES_PER_BLOB:
+            raise ValueError("a blob is 131072 bytes")
+        commitments, proofs = self.blobs_to_commitments_and_cell_proofs([blob])
+        return commitments[0], proofs
+
+    def blobs_to_commitments_and_cell_proofs(self, blobs) -> tuple:
+        """([commitments], [cell proofs]) for a batch of blobs in one device call; the proofs blob-major, 128 per blob"""
+        if not hasattr(self.ctx, "kzg_blob_to_commitment_and_cell_proofs"):
+            raise TypeError("cell proofs are computed on the device: KzgSettings needs a Context")
+        if not self.g1_monomial_handle:
+            raise ValueError("cell proofs need the setup's monomial G1 points: pass g1_monomial")
+        if any(len(b) != BYTES_PER_BLOB for b in blobs):
+            raise ValueError("a blob is 131072 bytes")
+        if not blobs:
+            return [], []
+        try:
+            return self.ctx.kzg_blob_to_commitment_and_cell_proofs(self.handle, self.g1_monomial_handle, b"".join(blobs))
         except B200Error as e:
             if e.status == 2:
                 raise ValueError(str(e)) from e

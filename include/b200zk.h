@@ -372,12 +372,27 @@ int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const
  *   kzg_compute_cells             c-kzg compute_cells, crates/common/crypto/kzg.rs:89-91
  *   kzg_verify_cell_proof_batch   kzg::verify_cell_kzg_proof_batch, kzg.rs:72-113, reached from BlobsBundle::verify_kzg_proofs
  *                                 (crates/common/types/blobs_bundle.rs:152-173) for every post-Osaka blob transaction
+ *   kzg_blob_to_commitment_and_cell_proofs
+ *                                 kzg::blob_to_commitment_and_cell_proofs (c-kzg compute_cells_and_kzg_proofs), kzg.rs:275-293,
+ *                                 called per blob by BlobsBundle::create_from_blobs for wrapper version 1 (blobs_bundle.rs:101-110)
  * A blob (4096 x 32-byte big-endian elements, each < r, else status 2 with b200zk_last_error naming the blob) lists p's
  * values on the 4096 roots of unity in bit-reversed order, root 7^((r-1)/4096).  Its extension lists p on the 8192
  * roots of unity in bit-reversed order, split into CELLS_PER_EXT_BLOB = 128 cells of FIELD_ELEMENTS_PER_CELL = 64
- * elements (2048 bytes); cells 0..63 are the blob itself.  Computing cell proofs (FK20) is not offered.
+ * elements (2048 bytes); cells 0..63 are the blob itself.
  * kzg_compute_cells: cells = n_blobs x 128 x 2048 bytes.  n_blobs = 0 returns 0; null pointers with n_blobs > 0: 4. */
 int b200zk_kzg_compute_cells(b200zk_ctx* ctx, const uint8_t* blobs, size_t n_blobs, uint8_t* cells /* n_blobs x 128 x 2048 B */);
+/* The commitment and the 128 cell proofs of each of n_blobs blobs, by FK20.  Cell k's proof is [q_k(tau)]1 with
+ * q_k = (p - I_k) / (X^64 - h_k^64), I_k = p mod (X^64 - h_k^64), h_k = w_8192^brp7(k) the first root of the cell's coset.
+ * g1_lagrange: the 4096-point Lagrange-form G1 handle of the KZG calls above (the commitment is an MSM over it).
+ * g1_monomial: a 4096-point BLS12-381 G1 handle (b200zk_bls12_381_g1_bases_upload) holding the setup's g1_monomial points
+ * [tau^i]1 in order; that both handles describe one tau is the setup's business.  The FK20 table derived from it (64 x 128
+ * points, 0.8 MB) is built on the handle's first call here, kept with the handle and freed by b200zk_bases_free.
+ * Rules: a G2 handle, an unknown handle or one of the wrong size returns 4, as do null pointers with n_blobs > 0;
+ * n_blobs = 0 returns 0; every blob element is checked < r before any MSM, and a failure returns 2, writes nothing and
+ * names the blob and element in b200zk_last_error; an identity commitment or proof is 0xc0 | 0..0 with status 0.
+ * commitments: n_blobs x 48 bytes; proofs: n_blobs x 128 x 48 bytes, blob-major with the cell index inner (compressed G1). */
+int b200zk_kzg_blob_to_commitment_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_lagrange, uint64_t g1_monomial, const uint8_t* blobs,
+                                                  size_t n_blobs, uint8_t* commitments /* 48 n */, uint8_t* proofs /* 128 x 48 n */);
 /* verify_cell_kzg_proof_batch over whole blobs, the shape the reference calls it with: every blob's 128 cells, cell
  * indices 0..127, each commitment standing for its blob's 128 cells; proofs are blob-major, 128 per blob, cell index inner
  * (48-byte compressed G1 each).  One answer, *valid = 1 or 0, from one two-pairing check of the universal equation

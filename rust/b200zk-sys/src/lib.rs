@@ -140,6 +140,7 @@ unsafe extern "C" {
     pub fn b200zk_kzg_verify_proof_batch(ctx: *mut b200zk_ctx, g2_setup: u64, commitments: *const u8, z: *const u8, y: *const u8, proofs: *const u8, n: usize, result: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_kzg_verify_blob_proof_batch(ctx: *mut b200zk_ctx, g2_setup: u64, blobs: *const u8, commitments: *const u8, proofs: *const u8, n: usize, valid: *mut c_int) -> c_int;
     pub fn b200zk_kzg_compute_cells(ctx: *mut b200zk_ctx, blobs: *const u8, n_blobs: usize, cells: *mut u8) -> c_int;
+    pub fn b200zk_kzg_blob_to_commitment_and_cell_proofs(ctx: *mut b200zk_ctx, g1_lagrange: u64, g1_monomial: u64, blobs: *const u8, n_blobs: usize, commitments: *mut u8, proofs: *mut u8) -> c_int;
     pub fn b200zk_kzg_verify_cell_proof_batch(ctx: *mut b200zk_ctx, g1_setup: u64, g2_setup: u64, blobs: *const u8, commitments: *const u8, proofs: *const u8, n_blobs: usize, valid: *mut c_int) -> c_int;
     pub fn b200zk_bls12_381_g1_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g2_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;

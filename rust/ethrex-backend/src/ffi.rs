@@ -549,6 +549,25 @@ impl B200zk {
         Ok(cells)
     }
 
+    /// `kzg::blob_to_commitment_and_cell_proofs` for n blobs: (n x 48 commitment bytes, n x 128 x 48 cell-proof bytes,
+    /// blob-major with the cell index inner).  `g1_lagrange` is the 4096-point Lagrange setup, `g1_monomial` the setup's
+    /// 4096 points [tau^i]1.  A blob element >= r is an error.
+    pub fn kzg_blob_to_commitment_and_cell_proofs(&mut self, g1_lagrange: u64, g1_monomial: u64, blobs: &[u8]) -> Result<(Vec<u8>, Vec<u8>), BackendError> {
+        const BLOB: usize = 4096 * 32;
+        let n = blobs.len() / BLOB;
+        if blobs.len() % BLOB != 0 {
+            return Err(BackendError::serialization("kzg_blob_to_commitment_and_cell_proofs: blobs must be n x 131072 bytes"));
+        }
+        let mut commitments = vec![0u8; 48 * n];
+        let mut proofs = vec![0u8; 128 * 48 * n];
+        // SAFETY: `blobs` holds n blobs, `commitments` 48 bytes and `proofs` 128 x 48 bytes per blob.
+        let status = unsafe {
+            sys::b200zk_kzg_blob_to_commitment_and_cell_proofs(self.ctx.as_ptr(), g1_lagrange, g1_monomial, blobs.as_ptr(), n, commitments.as_mut_ptr(), proofs.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok((commitments, proofs))
+    }
+
     /// `verify_cell_kzg_proof_batch` over whole blobs (every cell, each commitment once per blob, proofs blob-major with
     /// 128 per blob): one answer; malformed input is an error.  `g1_setup` is the 4096-point Lagrange setup, `g2_setup`
     /// the setup's 65 G2 points.
