@@ -232,7 +232,7 @@ int bls_msm_host_scalars(b200zk_ctx* ctx, const BasesEntry& e, const void* scala
   if (bad < n) return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, "bls12-381 scalar >= the group order");
   B2_TRY(ensure(ctx, ctx->ws_result, 512));
   B2_TRY(ensure(ctx, ctx->ws_out, 512));
-  B2_TRY(msm_run_bls(ctx, e.d, ctx->ws_scalars.p, n, flags & (B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW), st, ctx->ws_result.p, e.table_c, e.n));
+  B2_TRY(msm_run_bls(ctx, e.d.p, ctx->ws_scalars.p, n, flags & (B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW), st, ctx->ws_result.p, e.table_c, e.n));
   B2_TRY(msm_encode_bls(ctx, ctx->ws_result.p, 1, flags, st, ctx->ws_out.p));
   B2_CUDA(ctx, cudaMemcpyAsync(ctx->h_pinned, ctx->ws_out.p, 96 + 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
@@ -242,63 +242,46 @@ int bls_msm_host_scalars(b200zk_ctx* ctx, const BasesEntry& e, const void* scala
   return inf ? B200ZK_OK_INFINITY : B200ZK_OK;
 }
 
-// the root table (kzg_roots_build), built on first use; later calls on any stream wait on its event
+// the root table (kzg_roots_build), built on first use
 int kzg_roots(b200zk_ctx* ctx, cudaStream_t st, const void** roots) {
-  if (!ctx->kzg_roots.p) {
-    B2_TRY(ensure(ctx, ctx->kzg_roots, (kBlobN + 1) * 32));
-    B2_LAUNCH(ctx, kzg_roots_build, (kBlobN + 256) / 256, 256, 0, st, ctx->kzg_roots.p);
-    if (cudaEventCreateWithFlags(&ctx->kzg_roots_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(ctx->kzg_roots_ready, st));
-    else { cudaGetLastError(); ctx->kzg_roots_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
-  } else if (ctx->kzg_roots_ready) {
-    B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->kzg_roots_ready, 0));
-  }
-  *roots = ctx->kzg_roots.p;
-  return B200ZK_OK;
+  return once_table(ctx, ctx->kzg_roots, (kBlobN + 1) * 32, st, [&](void* t) -> int {
+    B2_LAUNCH(ctx, kzg_roots_build, (kBlobN + 256) / 256, 256, 0, st, t);
+    return B200ZK_OK;
+  }, roots);
 }
 
-// ws_kzg for n blobs: [blobs n x 128 KiB | z n x 32 (right behind the blobs: one range check covers both) | quotients
+// ws_kzg for n blobs: [blobs n x 128 KiB, then z n x 32 right behind them (one range check covers both) | quotients
 // n x 128 KiB | y n x 32 | 2n XYZZ partial sums | 2n encoded points (commitments, then proofs)]
 struct KzgLayout {
   uint8_t *blobs, *z, *q, *y, *partials, *enc;
   static constexpr size_t kPartial = 4 * 48, kEnc = 128;  // msm_encode writes 96 B + a u32 is_infinity flag
   int make(b200zk_ctx* ctx, size_t n) {
-    const size_t blob_bytes = n * kBlobN * 32;
-    B2_TRY(ensure(ctx, ctx->ws_kzg, 2 * blob_bytes + 2 * n * 32 + 2 * n * (kPartial + kEnc)));
-    blobs = (uint8_t*)ctx->ws_kzg.p; z = blobs + blob_bytes; q = z + n * 32; y = q + blob_bytes;
-    partials = y + n * 32; enc = partials + 2 * n * kPartial;
+    B2_TRY(carve(ctx, ctx->ws_kzg, [&](Carve& c) {
+      blobs = c.take<uint8_t>(n * (kBlobN + 1) * 32); q = c.take<uint8_t>(n * kBlobN * 32); y = c.take<uint8_t>(n * 32);
+      partials = c.take<uint8_t>(2 * n * kPartial); enc = c.take<uint8_t>(2 * n * kEnc);
+    }));
+    z = blobs + n * kBlobN * 32;
     return B200ZK_OK;
   }
 };
-
-int kzg_check_inputs(b200zk_ctx* ctx, const KzgLayout& L, size_t n, bool with_z, cudaStream_t st, const char* what) {
-  const size_t elems = n * kBlobN;
-  size_t bad = elems;
-  B2_TRY(bls_scalars_check(ctx, L.blobs, elems + (with_z ? n : 0), true, st, &bad));
-  if (bad >= elems + (with_z ? n : 0)) return B200ZK_OK;
-  char msg[160];
-  if (bad < elems) snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kBlobN, bad % kBlobN);
-  else snprintf(msg, sizeof msg, "%s: z of blob %zu is >= the BLS12-381 group order", what, bad - elems);
-  return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
-}
 
 }  // namespace
 
 // one 4096-point MSM per blob over the setup, each encoded into its own 128-byte slot of `enc`
 int b200zk::kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_t n, uint32_t flags, uint8_t* partials, uint8_t* enc, cudaStream_t st) {
   for (size_t b = 0; b < n; ++b) {
-    B2_TRY(msm_run_bls(ctx, e.d, scalars + b * kBlobN * 32, kBlobN, flags, st, partials + b * KzgLayout::kPartial, e.table_c, e.n));
+    B2_TRY(msm_run_bls(ctx, e.d.p, scalars + b * kBlobN * 32, kBlobN, flags, st, partials + b * KzgLayout::kPartial, e.table_c, e.n));
     B2_TRY(msm_encode_bls(ctx, partials + b * KzgLayout::kPartial, 1, 0, st, enc + b * KzgLayout::kEnc));
   }
   return B200ZK_OK;
 }
 
 // the setup handle of a KZG call: a BLS12-381 G1 handle of exactly 4096 points
-int b200zk::kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e) {
-  auto it = ctx->bases.find(handle);
+int b200zk::kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, BasesEntry** e) {
   std::string msg = what;
-  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": unknown setup handle").c_str());
-  if (it->second.n != kBlobN) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points").c_str());
-  *e = &it->second;
+  *e = find_bases(ctx, handle, Group::Bls12G1, (msg + ": unknown setup handle").c_str());
+  if (!*e) return B200ZK_ERR_INVALID_ARG;
+  if ((*e)->n != kBlobN) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points").c_str());
   return B200ZK_OK;
 }
 
@@ -359,36 +342,34 @@ int b200zk_bls12_381_g1_bases_upload(b200zk_ctx* ctx, const void* points, size_t
   const bool compressed = flags & B200ZK_POINTS_COMPRESSED;
   const size_t in_bytes = n * (compressed ? 48 : 96);
   BasesEntry e;
-  e.n = n; e.g2 = false; e.bls = true;
-  B2_CUDA(ctx, cudaMalloc(&e.d, n * 96 + 32));
+  e.n = n; e.group = Group::Bls12G1;
+  B2_CUDA(ctx, cudaMalloc(&e.d.p, n * 96 + 32));
   int rc = ensure(ctx, ctx->ws_ntt, in_bytes + 32);
   cudaError_t ce = cudaSuccess;
   if (rc <= B200ZK_OK_INFINITY && n) ce = cudaMemcpyAsync(ctx->ws_ntt.p, points, in_bytes, cudaMemcpyHostToDevice, ctx->stream);
-  if (rc <= B200ZK_OK_INFINITY && ce == cudaSuccess) rc = bls_points_to_native(ctx, ctx->ws_ntt.p, e.d, n, compressed, ctx->stream);
+  if (rc <= B200ZK_OK_INFINITY && ce == cudaSuccess) rc = bls_points_to_native(ctx, ctx->ws_ntt.p, e.d.p, n, compressed, ctx->stream);
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(ctx->stream);
-  if (rc > B200ZK_OK_INFINITY || ce != cudaSuccess) { cudaFree(e.d); return rc > B200ZK_OK_INFINITY ? rc : fail(ctx, B200ZK_ERR_CUDA, "bls bases upload", ce); }
-  *handle = ctx->next_handle++;
-  ctx->bases[*handle] = e;
-  return B200ZK_OK;
+  if (rc > B200ZK_OK_INFINITY) return rc;
+  if (ce != cudaSuccess) return fail(ctx, B200ZK_ERR_CUDA, "bls bases upload", ce);
+  return register_bases(ctx, std::move(e), handle);
 }
 
 int b200zk_bls12_381_g1_msm_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags, uint8_t out[48]) {
   if (!ctx || !out || (!scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: null argument");
   DeviceGuard guard(ctx);
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: n exceeds the resident bases");
-  return bls_msm_host_scalars(ctx, it->second, scalars, n, flags, ctx->stream, out);
+  const BasesEntry* e = find_bases(ctx, handle, Group::Bls12G1, "bls12_381_g1_msm_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_g1_msm_resident: n exceeds the resident bases");
+  return bls_msm_host_scalars(ctx, *e, scalars, n, flags, ctx->stream, out);
 }
 
 int b200zk_kzg_blob_to_commitment(b200zk_ctx* ctx, uint64_t setup_handle, const uint8_t* blobs, size_t n_blobs, uint8_t* commitments) {
   if (!ctx || (n_blobs && (!blobs || !commitments))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: null argument");
   DeviceGuard guard(ctx);
-  auto it = ctx->bases.find(setup_handle);
-  if (it == ctx->bases.end() || !it->second.bls || it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: unknown setup handle");
-  if (it->second.n != 4096) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment: the setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
+  BasesEntry* e = nullptr;
+  B2_TRY(kzg_setup(ctx, setup_handle, "kzg_blob_to_commitment", &e));
   for (size_t b = 0; b < n_blobs; ++b) {
-    int rc = bls_msm_host_scalars(ctx, it->second, blobs + b * 4096 * 32, 4096, B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW, ctx->stream, commitments + 48 * b);
+    int rc = bls_msm_host_scalars(ctx, *e, blobs + b * 4096 * 32, 4096, B200ZK_SCALARS_BE | B200ZK_SCALARS_RAW, ctx->stream, commitments + 48 * b);
     if (rc > B200ZK_OK_INFINITY) return rc;
   }
   return B200ZK_OK;
@@ -399,14 +380,14 @@ int b200zk_kzg_blob_to_commitment_and_proof(b200zk_ctx* ctx, uint64_t setup_hand
   if (!ctx || (n_blobs && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment_and_proof: null argument");
   NvtxRange nvtx("b200zk:kzg_blob_to_commitment_and_proof");
   DeviceGuard guard(ctx);
-  const BasesEntry* e = nullptr;
+  BasesEntry* e = nullptr;
   B2_TRY(kzg_setup(ctx, setup_handle, what, &e));
   if (!n_blobs) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
   KzgLayout L;
   B2_TRY(L.make(ctx, n_blobs));
   B2_CUDA(ctx, cudaMemcpyAsync(L.blobs, blobs, n_blobs * kBlobN * 32, cudaMemcpyHostToDevice, st));
-  B2_TRY(kzg_check_inputs(ctx, L, n_blobs, false, st, what));
+  B2_TRY(check_blobs(ctx, L.blobs, n_blobs, 0, st, what));
   // commitments, read back once: the challenge hashes them on the host
   B2_TRY(kzg_msms(ctx, *e, L.blobs, n_blobs, B200ZK_SCALARS_BE, L.partials, L.enc, st));
   std::vector<uint8_t> enc(2 * n_blobs * KzgLayout::kEnc), z(n_blobs * 32);
@@ -430,7 +411,7 @@ int b200zk_kzg_compute_proof(b200zk_ctx* ctx, uint64_t setup_handle, const uint8
   if (!ctx || (n_blobs && (!blobs || !z || !proofs || !y))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_compute_proof: null argument");
   NvtxRange nvtx("b200zk:kzg_compute_proof");
   DeviceGuard guard(ctx);
-  const BasesEntry* e = nullptr;
+  BasesEntry* e = nullptr;
   B2_TRY(kzg_setup(ctx, setup_handle, what, &e));
   if (!n_blobs) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
@@ -438,7 +419,7 @@ int b200zk_kzg_compute_proof(b200zk_ctx* ctx, uint64_t setup_handle, const uint8
   B2_TRY(L.make(ctx, n_blobs));
   B2_CUDA(ctx, cudaMemcpyAsync(L.blobs, blobs, n_blobs * kBlobN * 32, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(L.z, z, n_blobs * 32, cudaMemcpyHostToDevice, st));
-  B2_TRY(kzg_check_inputs(ctx, L, n_blobs, true, st, what));
+  B2_TRY(check_blobs(ctx, L.blobs, n_blobs, n_blobs, st, what));
   B2_TRY(kzg_proofs(ctx, *e, L, n_blobs, L.enc, st));
   std::vector<uint8_t> enc(n_blobs * KzgLayout::kEnc), ys(n_blobs * 32);
   B2_CUDA(ctx, cudaMemcpyAsync(enc.data(), L.enc, enc.size(), cudaMemcpyDeviceToHost, st));

@@ -141,11 +141,9 @@ int add_batch(b200zk_ctx* ctx, const char* what, const uint8_t* a, const uint8_t
   constexpr size_t kPt = point_bytes<F>();
   cudaStream_t st = ctx->stream;
   uint8_t *da, *db, *dout, *dst;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     da = c.take<uint8_t>(kPt * count); db = c.take<uint8_t>(kPt * count); dout = c.take<uint8_t>(kPt * count); dst = c.take<uint8_t>(count);
-  }
+  }));
   B2_CUDA(ctx, cudaMemcpyAsync(da, a, kPt * count, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(db, b, kPt * count, cudaMemcpyHostToDevice, st));
   B2_LAUNCH(ctx, bls_add<F>, (unsigned)((count + 63) / 64), 64, 0, st, (const uint8_t*)da, (const uint8_t*)db, count, dout, dst);
@@ -163,21 +161,17 @@ int msm_batch(b200zk_ctx* ctx, const char* what, const uint8_t* pairs, const uin
   NvtxRange nvtx(("b200zk:" + w).c_str());
   DeviceGuard guard(ctx);
   if (!count) return B200ZK_OK;
-  if (pair_offsets[0] != 0) return fail(ctx, B200ZK_ERR_INVALID_ARG, (w + ": pair_offsets[0] must be 0").c_str());
-  for (size_t i = 0; i < count; ++i)
-    if (pair_offsets[i + 1] < pair_offsets[i]) return fail(ctx, B200ZK_ERR_INVALID_ARG, (w + ": pair_offsets must be non-decreasing").c_str());
+  B2_TRY(check_offsets(ctx, pair_offsets, count, what));
   const size_t n = pair_offsets[count];
   constexpr size_t kPt = point_bytes<F>(), kPair = pair_bytes<F>();
   cudaStream_t st = ctx->stream;
   uint8_t *in, *pst, *dout, *dst;
   XYZZ<F>* terms;
   uint32_t* offs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     in = c.take<uint8_t>(kPair * n); terms = c.take<XYZZ<F>>(n); pst = c.take<uint8_t>(n); offs = c.take<uint32_t>(count + 1);
     dout = c.take<uint8_t>(kPt * count); dst = c.take<uint8_t>(count);
-  }
+  }));
   if (n) {
     B2_CUDA(ctx, cudaMemcpyAsync(in, pairs, kPair * n, cudaMemcpyHostToDevice, st));
     B2_LAUNCH(ctx, bls_msm_terms<F>, (unsigned)((n + 63) / 64), 64, 0, st, (const uint8_t*)in, n, terms, pst);

@@ -413,16 +413,15 @@ __global__ void __launch_bounds__(32) kzg_cell_fold(const XYZZ<Fp381>* parts, Af
 
 // ---- host side ----------------------------------------------------------------------------------------------------------
 size_t g2_lines_offset(size_t n) { return (n * sizeof(Affine<F2>) + 255) & ~(size_t)255; }
-const BlsLine* g2_setup_lines(const BasesEntry& e) { return reinterpret_cast<const BlsLine*>((const uint8_t*)e.d + g2_lines_offset(e.n)); }
+const BlsLine* g2_setup_lines(const BasesEntry& e) { return reinterpret_cast<const BlsLine*>((const uint8_t*)e.d.p + g2_lines_offset(e.n)); }
 
 // the G2 handle of a KZG verification: BLS12-381 G2, at least 2 points, point 0 the generator (point 1 is then [tau]2)
 int kzg_g2_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e) {
-  auto it = ctx->bases.find(handle);
   std::string msg = what;
-  if (it == ctx->bases.end() || !it->second.bls || !it->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": unknown BLS12-381 G2 setup handle").c_str());
-  if (it->second.n < 2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the G2 setup must hold at least 2 points").c_str());
-  if (!it->second.g2_gen0) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": point 0 of the G2 setup is not the G2 generator").c_str());
-  *e = &it->second;
+  *e = find_bases(ctx, handle, Group::Bls12G2, (msg + ": unknown BLS12-381 G2 setup handle").c_str());
+  if (!*e) return B200ZK_ERR_INVALID_ARG;
+  if ((*e)->n < 2) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the G2 setup must hold at least 2 points").c_str());
+  if (!(*e)->g2_gen0) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": point 0 of the G2 setup is not the G2 generator").c_str());
   return B200ZK_OK;
 }
 
@@ -447,17 +446,17 @@ int b200zk_bls12_381_g2_bases_upload(b200zk_ctx* ctx, const void* points, size_t
   DeviceGuard guard(ctx);
   cudaStream_t st = ctx->stream;
   BasesEntry e;
-  e.n = n; e.g2 = true; e.bls = true;
+  e.n = n; e.group = Group::Bls12G2;
   const size_t lines_off = g2_lines_offset(n);
   B2_TRY(ensure(ctx, ctx->ws_pairing, n * 96 + 256 + 16));
-  B2_CUDA(ctx, cudaMalloc(&e.d, lines_off + 2 * kLines * sizeof(BlsLine) + 32));
+  B2_CUDA(ctx, cudaMalloc(&e.d.p, lines_off + 2 * kLines * sizeof(BlsLine) + 32));
   unsigned long long* d_status = (unsigned long long*)((uint8_t*)ctx->ws_pairing.p + ((n * 96 + 255) & ~(size_t)255));
   unsigned long long h[2] = {(unsigned long long)n, (unsigned long long)n};
   int rc = B200ZK_OK;
   cudaError_t ce = cudaMemcpyAsync(d_status, h, 16, cudaMemcpyHostToDevice, st);
   if (ce == cudaSuccess && n) ce = cudaMemcpyAsync(ctx->ws_pairing.p, points, n * 96, cudaMemcpyHostToDevice, st);
   if (ce == cudaSuccess && n) {
-    bls_g2_decode<<<(unsigned)((n + 63) / 64), 64, 0, st>>>((const uint8_t*)ctx->ws_pairing.p, n, (Affine<F2>*)e.d, d_status);
+    bls_g2_decode<<<(unsigned)((n + 63) / 64), 64, 0, st>>>((const uint8_t*)ctx->ws_pairing.p, n, (Affine<F2>*)e.d.p, d_status);
     ctx->launches++;
     ce = cudaGetLastError();
   }
@@ -468,16 +467,15 @@ int b200zk_bls12_381_g2_bases_upload(b200zk_ctx* ctx, const void* points, size_t
   // the lines of points 0 and 1 (G2 and [tau]2 of a KZG setup), once per handle: the upload is synchronous, so they are
   // ready before the handle is returned
   if (ce == cudaSuccess && rc == B200ZK_OK && n >= 2) {
-    bls_g2_prepare<<<1, 64, 0, st>>>((const Affine<F2>*)e.d, nullptr, 2, (BlsLine*)((uint8_t*)e.d + lines_off));
+    bls_g2_prepare<<<1, 64, 0, st>>>((const Affine<F2>*)e.d.p, nullptr, 2, (BlsLine*)((uint8_t*)e.d.p + lines_off));
     ctx->launches++;
     ce = cudaGetLastError();
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
   }
-  if (rc != B200ZK_OK || ce != cudaSuccess) { cudaFree(e.d); return rc != B200ZK_OK ? rc : fail(ctx, B200ZK_ERR_CUDA, "bls12_381_g2_bases_upload", ce); }
+  if (rc != B200ZK_OK) return rc;
+  if (ce != cudaSuccess) return fail(ctx, B200ZK_ERR_CUDA, "bls12_381_g2_bases_upload", ce);
   e.g2_gen0 = n >= 1 && memcmp(points, kG2GenCompressed, 96) == 0;  // a valid point has one encoding
-  *handle = ctx->next_handle++;
-  ctx->bases[*handle] = e;
-  return B200ZK_OK;
+  return register_bases(ctx, std::move(e), handle);
 }
 
 int b200zk_bls12_381_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint32_t* pair_offsets, size_t count, uint8_t* result, uint8_t* status) {
@@ -486,9 +484,7 @@ int b200zk_bls12_381_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, 
   NvtxRange nvtx("b200zk:bls12_381_pairing_check_batch");
   DeviceGuard guard(ctx);
   if (!count) return B200ZK_OK;
-  if (pair_offsets[0] != 0) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_pairing_check_batch: pair_offsets[0] must be 0");
-  for (size_t i = 0; i < count; ++i)
-    if (pair_offsets[i + 1] < pair_offsets[i]) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bls12_381_pairing_check_batch: pair_offsets must be non-decreasing");
+  B2_TRY(check_offsets(ctx, pair_offsets, count, "bls12_381_pairing_check_batch"));
   const size_t n = pair_offsets[count];
   cudaStream_t st = ctx->stream;
   uint8_t *in, *pst, *res, *sts;
@@ -497,12 +493,10 @@ int b200zk_bls12_381_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, 
   BlsLine* lines;
   Fp12b* f;
   uint32_t* offs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     in = c.take<uint8_t>(384 * n); P = c.take<Affine<Fp381>>(n); Q = c.take<Affine<F2>>(n); pst = c.take<uint8_t>(n);
     lines = c.take<BlsLine>(kLines * n); f = c.take<Fp12b>(n); offs = c.take<uint32_t>(count + 1); res = c.take<uint8_t>(count); sts = c.take<uint8_t>(count);
-  }
+  }));
   if (n) B2_CUDA(ctx, cudaMemcpyAsync(in, pairs, 384 * n, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(offs, pair_offsets, (count + 1) * 4, cudaMemcpyHostToDevice, st));
   if (n) {
@@ -530,13 +524,11 @@ int b200zk_kzg_verify_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint
   Affine<Fp381>*pts, *P;
   Fp12b* f;
   uint32_t* offs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     in = c.take<uint8_t>(96 * n); zb = c.take<uint8_t>(32 * n); yb = c.take<uint8_t>(32 * n); pts = c.take<Affine<Fp381>>(2 * n);
     pt_st = c.take<uint8_t>(2 * n); P = c.take<Affine<Fp381>>(2 * n); pst = c.take<uint8_t>(2 * n); f = c.take<Fp12b>(2 * n);
     offs = c.take<uint32_t>(n + 1); res = c.take<uint8_t>(n); sts = c.take<uint8_t>(n);
-  }
+  }));
   std::vector<uint32_t> h_offs(n + 1);
   for (size_t i = 0; i <= n; ++i) h_offs[i] = (uint32_t)(2 * i);
   B2_CUDA(ctx, cudaMemcpyAsync(in, commitments, 48 * n, cudaMemcpyHostToDevice, st));
@@ -569,23 +561,16 @@ int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const
   XYZZ<Fp381>* terms;
   Fp12b* f;
   uint32_t* offs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(kBlob * n); zb = c.take<uint8_t>(32 * n); q = c.take<uint8_t>(kBlob * n); yb = c.take<uint8_t>(32 * n);
     in = c.take<uint8_t>(96 * n); pts = c.take<Affine<Fp381>>(2 * n); pt_st = c.take<uint8_t>(2 * n); rho = c.take<uint8_t>(32);
     terms = c.take<XYZZ<Fp381>>(2 * n); P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<Fp12b>(2);
     offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
-  }
+  }));
   char msg[160];
   // 1. every blob element < r (c-kzg blob_to_polynomial): an error, not a false
   B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, kBlob * n, cudaMemcpyHostToDevice, st));
-  size_t bad = 0;
-  B2_TRY(bls_scalars_check(ctx, d_blobs, 4096 * n, true, st, &bad));
-  if (bad < 4096 * n) {
-    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / 4096, bad % 4096);
-    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
-  }
+  B2_TRY(check_blobs(ctx, d_blobs, n, 0, st, what));
   // 2. commitments and proofs: c-kzg validate_kzg_g1 (decompression, subgroup)
   B2_CUDA(ctx, cudaMemcpyAsync(in, commitments, 48 * n, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(in + 48 * n, proofs, 48 * n, cudaMemcpyHostToDevice, st));
@@ -643,9 +628,9 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   if (!ctx || !valid || (n && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: null argument");
   NvtxRange nvtx("b200zk:kzg_verify_cell_proof_batch");
   DeviceGuard guard(ctx);
-  auto g1 = ctx->bases.find(g1_setup);
-  if (g1 == ctx->bases.end() || !g1->second.bls || g1->second.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: unknown G1 setup handle");
-  if (g1->second.n != kN) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G1 setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
+  const BasesEntry* g1 = find_bases(ctx, g1_setup, Group::Bls12G1, "kzg_verify_cell_proof_batch: unknown G1 setup handle");
+  if (!g1) return B200ZK_ERR_INVALID_ARG;
+  if (g1->n != kN) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G1 setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
   const BasesEntry* e = nullptr;
   B2_TRY(kzg_g2_setup(ctx, g2_setup, what, &e));
   if (e->n < 65) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G2 setup must hold at least 65 points ([tau^64]2 is point 64)");
@@ -660,24 +645,17 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   BlsLine* lines;
   Fp12b* f;
   uint32_t* offs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(kBlob * n); cells = c.take<uint8_t>(kExt * n); in = c.take<uint8_t>(48 * (n + m));
     pts = c.take<Affine<Fp381>>(n + m); pt_st = c.take<uint8_t>(n + m); rbe = c.take<uint8_t>(32);
     weights = c.take<uint4>(2 * 65); partial = c.take<uint4>(2 * 64 * n); s_proof = c.take<uint4>(2 * m); s_lin = c.take<uint4>(2 * (n + m));
     s_setup = c.take<uint4>(2 * kN); parts = c.take<XYZZ<Fp381>>(3); q2 = c.take<Affine<F2>>(2); lines = c.take<BlsLine>(2 * kLines);
     P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<Fp12b>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
-  }
+  }));
   char msg[160];
   // 1. every blob element < r (c-kzg blob_to_polynomial inside compute_cells): an error, not a false
   B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, kBlob * n, cudaMemcpyHostToDevice, st));
-  size_t bad = 0;
-  B2_TRY(bls_scalars_check(ctx, d_blobs, kN * n, true, st, &bad));
-  if (bad < kN * n) {
-    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kN, bad % kN);
-    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
-  }
+  B2_TRY(check_blobs(ctx, d_blobs, n, 0, st, what));
   // 2. commitments, then proofs: c-kzg validate_kzg_g1 (decompression, subgroup)
   B2_CUDA(ctx, cudaMemcpyAsync(in, commitments, 48 * n, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(in + 48 * n, proofs, 48 * m, cudaMemcpyHostToDevice, st));
@@ -721,9 +699,9 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   B2_TRY(kzg_cell_scalars_run(ctx, d_blobs, n, rbe, weights, partial, s_proof, s_lin, s_setup, st));
   B2_TRY(msm_run_bls(ctx, pts + n, s_proof, m, 0, st, parts));
   B2_TRY(msm_run_bls(ctx, pts, s_lin, n + m, 0, st, parts + 1));
-  B2_TRY(msm_run_bls(ctx, g1->second.d, s_setup, kN, 0, st, parts + 2, g1->second.table_c, g1->second.n));
+  B2_TRY(msm_run_bls(ctx, g1->d.p, s_setup, kN, 0, st, parts + 2, g1->table_c, g1->n));
   B2_LAUNCH(ctx, kzg_cell_fold, 1, 32, 0, st, (const XYZZ<Fp381>*)parts, P, pst);
-  const Affine<F2>* g2pts = (const Affine<F2>*)e->d;
+  const Affine<F2>* g2pts = (const Affine<F2>*)e->d.p;
   B2_CUDA(ctx, cudaMemcpyAsync(q2, g2pts, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(q2 + 1, g2pts + 64, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
   B2_LAUNCH(ctx, bls_g2_prepare, 1, 64, 0, st, (const Affine<F2>*)q2, (const uint8_t*)nullptr, (size_t)2, lines);

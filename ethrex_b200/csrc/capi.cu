@@ -13,6 +13,7 @@ using namespace b200zk;
 namespace {
 
 template <bool G2> struct Sizes {
+  static constexpr Group group = G2 ? Group::Bn254G2 : Group::Bn254G1;
   static constexpr size_t point = G2 ? 128 : 64;     // affine, native or BE
   static constexpr size_t partial = G2 ? 256 : 128;  // XYZZ
 };
@@ -81,49 +82,44 @@ template <bool G2>
 int bases_upload(b200zk_ctx* ctx, const void* points, size_t n, uint32_t flags, uint64_t* handle) {
   if (!ctx || !handle || (!points && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_upload: null argument");
   BasesEntry e;
-  e.n = n; e.g2 = G2;
-  B2_CUDA(ctx, cudaMalloc(&e.d, n * Sizes<G2>::point + 32));
-  int rc = upload_points<G2>(ctx, points, n, flags, ctx->stream, e.d, &ctx->ws_ntt);
-  if (rc > B200ZK_OK_INFINITY) { cudaFree(e.d); return rc; }
+  e.n = n; e.group = Sizes<G2>::group;
+  B2_CUDA(ctx, cudaMalloc(&e.d.p, n * Sizes<G2>::point + 32));
+  B2_TRY(upload_points<G2>(ctx, points, n, flags, ctx->stream, e.d.p, &ctx->ws_ntt));
   cudaError_t ce = cudaStreamSynchronize(ctx->stream);
-  if (ce != cudaSuccess) { cudaFree(e.d); return fail(ctx, B200ZK_ERR_CUDA, "bases upload", ce); }
-  *handle = ctx->next_handle++;
-  ctx->bases[*handle] = e;
-  return B200ZK_OK;
+  if (ce != cudaSuccess) return fail(ctx, B200ZK_ERR_CUDA, "bases upload", ce);
+  return register_bases(ctx, std::move(e), handle);
 }
 
 template <bool G2>
 int msm_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags, uint8_t* out) {
   if (!ctx || !out || (!scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || it->second.g2 != G2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident: n exceeds the resident bases");
+  const BasesEntry* e = find_bases(ctx, handle, Sizes<G2>::group, "msm_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident: n exceeds the resident bases");
   // host scalars go straight into the (chunk-pipelined) schedule: their upload overlaps the previous chunk's work
-  return msm_device<G2>(ctx, it->second.d, nullptr, n, flags & ~B200ZK_POINTS_BE, ctx->stream, out, it->second.table_c, it->second.n, scalars);
+  return msm_device<G2>(ctx, e->d.p, nullptr, n, flags & ~B200ZK_POINTS_BE, ctx->stream, out, e->table_c, e->n, scalars);
 }
 
 template <bool G2>
 int msm_resident_device(b200zk_ctx* ctx, uint64_t handle, const void* d_scalars, size_t n, uint32_t flags, void* stream, uint8_t* out) {
   if (!ctx || !out || (!d_scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident_device: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || it->second.g2 != G2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident_device: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident_device: n exceeds the resident bases");
-  return msm_device<G2>(ctx, it->second.d, d_scalars, n, flags & ~B200ZK_POINTS_BE, stream, out, it->second.table_c, it->second.n);
+  const BasesEntry* e = find_bases(ctx, handle, Sizes<G2>::group, "msm_resident_device: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_resident_device: n exceeds the resident bases");
+  return msm_device<G2>(ctx, e->d.p, d_scalars, n, flags & ~B200ZK_POINTS_BE, stream, out, e->table_c, e->n);
 }
 
 template <bool G2>
 int bases_from_device(b200zk_ctx* ctx, const void* d_points, size_t n, void* stream, uint64_t* handle) {
   if (!ctx || !handle || (!d_points && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_from_device: null argument");
   BasesEntry e;
-  e.n = n; e.g2 = G2;
+  e.n = n; e.group = Sizes<G2>::group;
   cudaStream_t st = pick_stream(ctx, stream);
-  B2_CUDA(ctx, cudaMalloc(&e.d, n * Sizes<G2>::point + 32));
-  cudaError_t ce = n ? cudaMemcpyAsync(e.d, d_points, n * Sizes<G2>::point, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
+  B2_CUDA(ctx, cudaMalloc(&e.d.p, n * Sizes<G2>::point + 32));
+  cudaError_t ce = n ? cudaMemcpyAsync(e.d.p, d_points, n * Sizes<G2>::point, cudaMemcpyDeviceToDevice, st) : cudaSuccess;
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
-  if (ce != cudaSuccess) { cudaFree(e.d); return fail(ctx, B200ZK_ERR_CUDA, "bases_from_device copy", ce); }
-  *handle = ctx->next_handle++;
-  ctx->bases[*handle] = e;
-  return B200ZK_OK;
+  if (ce != cudaSuccess) return fail(ctx, B200ZK_ERR_CUDA, "bases_from_device copy", ce);
+  return register_bases(ctx, std::move(e), handle);
 }
 
 template <bool G2>
@@ -211,29 +207,9 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   if (cudaGetDevice(&prev_device) != cudaSuccess) { cudaGetLastError(); prev_device = -1; }
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
-  for (auto& b : ctx->ws_g16) if (b.p) cudaFree(b.p);
-  if (ctx->ws_zinv.p) cudaFree(ctx->ws_zinv.p);
-  if (ctx->ws_key.p) cudaFree(ctx->ws_key.p);
-  if (ctx->ws_ctab.p) cudaFree(ctx->ws_ctab.p);
-  if (ctx->ws_cnt2.p) cudaFree(ctx->ws_cnt2.p);
-  if (ctx->kzg_roots.p) cudaFree(ctx->kzg_roots.p);
-  if (ctx->ws_kzg.p) cudaFree(ctx->ws_kzg.p);
-  if (ctx->ws_pairing.p) cudaFree(ctx->ws_pairing.p);
-  if (ctx->kzg_roots_ready) cudaEventDestroy(ctx->kzg_roots_ready);
-  if (ctx->kzg_cells_tw.p) cudaFree(ctx->kzg_cells_tw.p);
-  if (ctx->kzg_cells_tw_ready) cudaEventDestroy(ctx->kzg_cells_tw_ready);
-  if (ctx->secp_gtab.p) cudaFree(ctx->secp_gtab.p);
-  if (ctx->secp_gtab_ready) cudaEventDestroy(ctx->secp_gtab_ready);
-  if (ctx->p256_gtab.p) cudaFree(ctx->p256_gtab.p);
-  if (ctx->p256_gtab_ready) cudaEventDestroy(ctx->p256_gtab_ready);
-  DevBuf* bufs[] = {&ctx->ws_hist, &ctx->ws_offsets, &ctx->ws_cursor, &ctx->ws_blocksums, &ctx->ws_idx, &ctx->ws_buckets, &ctx->ws_chunkS,
-                    &ctx->ws_chunkV, &ctx->ws_result, &ctx->ws_points, &ctx->ws_scalars, &ctx->ws_ntt, &ctx->ws_misc, &ctx->ws_out, &ctx->ws_segoff, &ctx->ws_segbucket, &ctx->ws_digits, &ctx->ws_q0, &ctx->ws_q1, &ctx->ws_prefix, &ctx->ws_info, &ctx->ws_pairoff0, &ctx->ws_pairoff1};
-  for (DevBuf* b : bufs) if (b->p) cudaFree(b->p);
-  if (ctx->ws_totals.p) cudaFree(ctx->ws_totals.p);
-  if (ctx->ws_bitpart.p) cudaFree(ctx->ws_bitpart.p);
+  // the resident bases, the once-built tables and every workspace DevBuf free themselves (here and in `delete ctx`)
+  ctx->bases.clear();
   for (auto& sl : ctx->slot) {
-    DevBuf* sb[] = {&sl.hist, &sl.offsets, &sl.cursor, &sl.run_off, &sl.tsum, &sl.digits, &sl.idx, &sl.key, &sl.ctab, &sl.cnt2};
-    for (DevBuf* b : sb) if (b->p) cudaFree(b->p);
     if (sl.sorted) cudaEventDestroy(sl.sorted);
     if (sl.released) cudaEventDestroy(sl.released);
   }
@@ -241,11 +217,6 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   for (auto& e : ctx->ev_up) if (e) cudaEventDestroy(e);
   if (ctx->stream_sort) cudaStreamDestroy(ctx->stream_sort);
   for (auto& kv : ctx->twiddles) { cudaFree(kv.second.d); if (kv.second.ready) cudaEventDestroy(kv.second.ready); }
-  for (auto& kv : ctx->bases) {
-    cudaFree(kv.second.d);
-    if (kv.second.fk20) cudaFree(kv.second.fk20);
-    if (kv.second.fk20_ready) cudaEventDestroy(kv.second.fk20_ready);
-  }
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -314,37 +285,35 @@ int b200zk_g2_msm_resident_device(b200zk_ctx* ctx, uint64_t handle, const void* 
 
 int b200zk_bases_precompute(b200zk_ctx* ctx, uint64_t handle, uint32_t window_bits) { b200zk::DeviceGuard guard(ctx);
   if (!ctx) return B200ZK_ERR_INVALID_ARG;
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end()) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: unknown handle");
+  BasesEntry* found = find_bases(ctx, handle, "bases_precompute: unknown handle");
+  if (!found) return B200ZK_ERR_INVALID_ARG;
   if (window_bits && (window_bits < 2 || window_bits > 24)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: window must be 0 or 2..24");
-  BasesEntry& e = it->second;
-  if (e.bls && e.g2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: BLS12-381 G2 handles are pairing inputs, not MSM bases");
+  BasesEntry& e = *found;
+  if (e.group == Group::Bls12G2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: BLS12-381 G2 handles are pairing inputs, not MSM bases");
   if (e.table_c) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_precompute: handle already precomputed");
   const uint32_t c = window_bits ? window_bits : precompute_window(e.n);
-  const uint32_t W = ((e.bls ? 256u : 255u) + c - 1) / c;  // ScalarBits<F>: BLS12-381's group order has one more bit
-  const size_t pt = e.bls ? 96 : (e.g2 ? 128 : 64);
+  const GroupSizes sz = group_sizes(e.group);
+  const uint32_t W = (sz.scalar_bits + c - 1) / c;
+  const size_t pt = sz.point;
   if ((unsigned long long)e.n * W >= (1ull << 31)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "bases_precompute: table exceeds 31-bit indices");
-  void* table = nullptr;
-  B2_CUDA(ctx, cudaMalloc(&table, (size_t)W * e.n * pt + 32));
-  int rc = e.bls ? msm_precompute_bls(ctx, e.d, e.n, c, table, ctx->stream)
-                 : (e.g2 ? msm_precompute_g2(ctx, e.d, e.n, c, table, ctx->stream) : msm_precompute_g1(ctx, e.d, e.n, c, table, ctx->stream));
+  DevBuf table;
+  B2_CUDA(ctx, cudaMalloc(&table.p, (size_t)W * e.n * pt + 32));
+  int rc = e.group == Group::Bls12G1 ? msm_precompute_bls(ctx, e.d.p, e.n, c, table.p, ctx->stream)
+         : e.group == Group::Bn254G2 ? msm_precompute_g2(ctx, e.d.p, e.n, c, table.p, ctx->stream)
+                                     : msm_precompute_g1(ctx, e.d.p, e.n, c, table.p, ctx->stream);
   cudaError_t ce = cudaStreamSynchronize(ctx->stream);
-  if (rc > B200ZK_OK_INFINITY || ce != cudaSuccess) { cudaFree(table); return rc > B200ZK_OK_INFINITY ? rc : fail(ctx, B200ZK_ERR_CUDA, "bases_precompute", ce); }
-  cudaFree(e.d);
-  e.d = table;
+  if (rc > B200ZK_OK_INFINITY) return rc;
+  if (ce != cudaSuccess) return fail(ctx, B200ZK_ERR_CUDA, "bases_precompute", ce);
+  e.d = std::move(table);
   e.table_c = c;
   return B200ZK_OK;
 }
 
 int b200zk_bases_free(b200zk_ctx* ctx, uint64_t handle) { b200zk::DeviceGuard guard(ctx);
   if (!ctx) return B200ZK_ERR_INVALID_ARG;
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end()) return fail(ctx, B200ZK_ERR_INVALID_ARG, "bases_free: unknown handle");
+  if (!find_bases(ctx, handle, "bases_free: unknown handle")) return B200ZK_ERR_INVALID_ARG;
   B2_CUDA(ctx, cudaDeviceSynchronize());
-  cudaFree(it->second.d);
-  if (it->second.fk20) cudaFree(it->second.fk20);
-  if (it->second.fk20_ready) cudaEventDestroy(it->second.fk20_ready);
-  ctx->bases.erase(it);
+  ctx->bases.erase(handle);
   return B200ZK_OK;
 }
 int b200zk_g1_msm_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags, uint8_t out[64]) { b200zk::DeviceGuard guard(ctx); return msm_resident<false>(ctx, handle, scalars, n, flags, out); }
@@ -400,32 +369,32 @@ int b200zk_g2_msm_partial_device(b200zk_ctx* ctx, const void* d_points, const vo
 }
 int b200zk_g1_msm_partial_resident_device(b200zk_ctx* ctx, uint64_t handle, const void* d_scalars, size_t n, uint32_t flags, void* stream, void* d_partial128) { b200zk::DeviceGuard guard(ctx);
   if (!ctx || !d_partial128 || (!d_scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || it->second.g2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
-  return msm_run_g1(ctx, it->second.d, d_scalars, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial128, it->second.table_c, it->second.n);
+  const BasesEntry* e = find_bases(ctx, handle, Group::Bn254G1, "msm_partial_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
+  return msm_run_g1(ctx, e->d.p, d_scalars, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial128, e->table_c, e->n);
 }
 // host (pinned) scalars: their upload is chunk-pipelined with the accumulation; the partial stays on the device
 int b200zk_g1_msm_partial_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags, void* stream, void* d_partial128) { b200zk::DeviceGuard guard(ctx);
   if (!ctx || !d_partial128 || (!scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || it->second.g2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
-  return msm_run_g1(ctx, it->second.d, nullptr, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial128, it->second.table_c, it->second.n, scalars);
+  const BasesEntry* e = find_bases(ctx, handle, Group::Bn254G1, "msm_partial_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
+  return msm_run_g1(ctx, e->d.p, nullptr, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial128, e->table_c, e->n, scalars);
 }
 int b200zk_g2_msm_partial_resident(b200zk_ctx* ctx, uint64_t handle, const void* scalars, size_t n, uint32_t flags, void* stream, void* d_partial256) { b200zk::DeviceGuard guard(ctx);
   if (!ctx || !d_partial256 || (!scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || !it->second.g2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
-  return msm_run_g2(ctx, it->second.d, nullptr, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial256, it->second.table_c, it->second.n, scalars);
+  const BasesEntry* e = find_bases(ctx, handle, Group::Bn254G2, "msm_partial_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
+  return msm_run_g2(ctx, e->d.p, nullptr, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial256, e->table_c, e->n, scalars);
 }
 int b200zk_g2_msm_partial_resident_device(b200zk_ctx* ctx, uint64_t handle, const void* d_scalars, size_t n, uint32_t flags, void* stream, void* d_partial256) { b200zk::DeviceGuard guard(ctx);
   if (!ctx || !d_partial256 || (!d_scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: null argument");
-  auto it = ctx->bases.find(handle);
-  if (it == ctx->bases.end() || !it->second.g2 || it->second.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: unknown handle");
-  if (n > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
-  return msm_run_g2(ctx, it->second.d, d_scalars, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial256, it->second.table_c, it->second.n);
+  const BasesEntry* e = find_bases(ctx, handle, Group::Bn254G2, "msm_partial_resident: unknown handle");
+  if (!e) return B200ZK_ERR_INVALID_ARG;
+  if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_partial_resident: n exceeds the resident bases");
+  return msm_run_g2(ctx, e->d.p, d_scalars, n, flags & ~B200ZK_POINTS_BE, pick_stream(ctx, stream), d_partial256, e->table_c, e->n);
 }
 int b200zk_g1_fold_partials_device(b200zk_ctx* ctx, const void* d_partials, size_t count, uint32_t flags, void* stream, uint8_t out[64]) { b200zk::DeviceGuard guard(ctx); return fold_partials<false>(ctx, d_partials, count, flags, stream, out); }
 int b200zk_g2_fold_partials_device(b200zk_ctx* ctx, const void* d_partials, size_t count, uint32_t flags, void* stream, uint8_t out[128]) { b200zk::DeviceGuard guard(ctx); return fold_partials<true>(ctx, d_partials, count, flags, stream, out); }
@@ -436,31 +405,29 @@ int b200zk_msm_multi_resident_device(b200zk_ctx* ctx, const uint64_t* handles, s
   if (!ctx || (count && (!handles || !out || !status)) || (!d_scalars && n)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: null argument");
   if (!count) return B200ZK_OK;
   cudaStream_t st = pick_stream(ctx, stream);
-  const BasesEntry* first = nullptr;
+  std::vector<const BasesEntry*> cols(count);
   for (size_t i = 0; i < count; ++i) {
-    auto it = ctx->bases.find(handles[i]);
-    if (it == ctx->bases.end()) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: unknown handle");
-    const BasesEntry& e = it->second;
-    if (n > e.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: n exceeds the resident bases");
-    if (e.bls) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: BLS12-381 bases in a BN254 call");
-    if (!first) first = &e;
+    const BasesEntry* e = cols[i] = find_bases(ctx, handles[i], "msm_multi_resident_device: unknown handle");
+    if (!e) return B200ZK_ERR_INVALID_ARG;
+    if (n > e->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: n exceeds the resident bases");
+    if (e->group != Group::Bn254G1 && e->group != Group::Bn254G2) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: BLS12-381 bases in a BN254 call");
     // one sort serves every column only if they share the plan: same window tables (or none) over the same point count
-    if (e.table_c != first->table_c || (e.table_c && e.n != first->n))
+    if (e->table_c != cols[0]->table_c || (e->table_c && e->n != cols[0]->n))
       return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm_multi_resident_device: handles must share the precomputed window and the point count");
   }
   B2_TRY(ensure(ctx, ctx->ws_result, 256));
   B2_TRY(ensure(ctx, ctx->ws_out, 256));
   for (size_t i = 0; i < count; ++i) {
-    const BasesEntry& e = ctx->bases.find(handles[i])->second;
+    const BasesEntry& e = *cols[i];
     const int mode = (n >= 2) ? (i == 0 ? 1 : 2) : 0;  // n < 2: nothing worth sharing, and the tiny plans differ
     const uint32_t f = flags & ~(uint32_t)B200ZK_POINTS_BE;
     int rc;
-    if (e.g2) {
-      B2_TRY(msm_run_g2(ctx, e.d, d_scalars, n, f, st, ctx->ws_result.p, e.table_c, e.n, nullptr, mode));
+    if (e.group == Group::Bn254G2) {
+      B2_TRY(msm_run_g2(ctx, e.d.p, d_scalars, n, f, st, ctx->ws_result.p, e.table_c, e.n, nullptr, mode));
       B2_TRY(msm_encode_g2(ctx, ctx->ws_result.p, 1, flags, st, ctx->ws_out.p));
       rc = read_result(ctx, ctx->ws_out.p, 128, st, out + 128 * i);
     } else {
-      B2_TRY(msm_run_g1(ctx, e.d, d_scalars, n, f, st, ctx->ws_result.p, e.table_c, e.n, nullptr, mode));
+      B2_TRY(msm_run_g1(ctx, e.d.p, d_scalars, n, f, st, ctx->ws_result.p, e.table_c, e.n, nullptr, mode));
       B2_TRY(msm_encode_g1(ctx, ctx->ws_result.p, 1, flags, st, ctx->ws_out.p));
       rc = read_result(ctx, ctx->ws_out.p, 64, st, out + 128 * i);
     }

@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200zk.h"
@@ -18,9 +19,30 @@ template <> struct CurveB<Fp381> {
   static B2_D Fp381 b() { Fp381 four = Fp381::zero(); four.v[0] = 4; return Fp381::to_mont(four); }  // y^2 = x^3 + 4
 };
 
+// a device allocation that frees itself: grown by ensure(), move-only
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { reset(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { reset(); }
+  void reset() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+};
+
+// a table built on first use by once_table(); consumers on other streams wait on `ready`
+struct OnceTable {
+  DevBuf buf;
+  cudaEvent_t ready = nullptr;
+  bool built = false;  // set only once the build is enqueued and its event recorded
+  OnceTable() = default;
+  OnceTable(OnceTable&& o) noexcept : buf(std::move(o.buf)), ready(o.ready), built(o.built) { o.ready = nullptr; o.built = false; }
+  ~OnceTable() { if (ready) cudaEventDestroy(ready); }
 };
 
 struct TwiddleSet {   // per (log_n, direction): see ntt.cu
@@ -36,18 +58,30 @@ struct SortSlot {  // one of the two sort workspaces of the chunk-pipelined MSM
   cudaEvent_t sorted = nullptr, released = nullptr;
 };
 
+// Bls12G1: Fp381 Montgomery, 96 B affine, the KZG trusted setup; Bls12G2: Fp2 over Fp381, 192 B affine, followed by the
+// prepared Miller-loop lines of points 0 and 1
+enum class Group { Bn254G1, Bn254G2, Bls12G1, Bls12G2 };
+
+// native affine point bytes and scalar bits (ScalarBits<F>: BLS12-381's group order has one more bit) of a group
+struct GroupSizes { size_t point; uint32_t scalar_bits; };
+inline GroupSizes group_sizes(Group g) {
+  switch (g) {
+    case Group::Bn254G1: return {64, 255};
+    case Group::Bn254G2: return {128, 255};
+    case Group::Bls12G1: return {96, 256};
+    default: return {192, 256};
+  }
+}
+
 struct BasesEntry {
-  void* d = nullptr;
+  DevBuf d;
   size_t n = 0;
-  bool g2 = false;
-  bool bls = false;      // BLS12-381 points: G1 (Fp381 Montgomery, 96 B affine), the KZG trusted setup; with g2 set, G2
-                         // (Fp2 over Fp381, 192 B affine), followed by the prepared Miller-loop lines of points 0 and 1
+  Group group = Group::Bn254G1;
   bool g2_gen0 = false;  // BLS12-381 G2: point 0 is the generator (so point 1 is [tau]2 of a KZG setup)
   uint32_t table_c = 0;  // != 0: d holds W = ceil(255/c) windows of n points: 2^(c*w) * P_i at w*n + i
   // a 4096-point BLS12-381 G1 monomial setup used for EIP-7594 cell proofs (kzg_cells.cu): its FK20 table, 64 x 128 native
-  // affine points, built on the handle's first such call and freed with it; consumers on other streams wait on fk20_ready
-  void* fk20 = nullptr;
-  cudaEvent_t fk20_ready = nullptr;
+  // affine points, built on the handle's first such call and freed with it
+  OnceTable fk20;
 };
 
 }  // namespace b200zk
@@ -71,31 +105,21 @@ struct b200zk_ctx {
   uint32_t zinv_log_n = 0xffffffffu;
   // cudaFuncSetAttribute (opt-in to > 48 KiB dynamic shared memory) is per DEVICE: remembered per context, not per process
   bool attr_sort = false, attr_acc = false, attr_ntt512 = false, attr_ntt256 = false, attr_kzg = false, attr_kzg_cells = false;
-  // EIP-4844 proofs (bls381.cu): the blob domain's 4096 roots of unity in bit-reversed order, then 1/4096 (Fr381
-  // Montgomery), built once per context; consumers on other streams wait on kzg_roots_ready.  ws_kzg: blobs, z, quotients,
-  // partial sums and encoded results of one call
-  b200zk::DevBuf kzg_roots, ws_kzg;
-  cudaEvent_t kzg_roots_ready = nullptr;
-  // EIP-7594 cells (kzg_cells.cu): w^i for the 8192nd root w, i < 8192, then 1/4096 (Fr381 Montgomery), built once per
-  // context; consumers on other streams wait on kzg_cells_tw_ready
-  b200zk::DevBuf kzg_cells_tw;
-  cudaEvent_t kzg_cells_tw_ready = nullptr;
+  // tables built once per context on first use (once_table):
+  //   kzg_roots (bls381.cu): the EIP-4844 blob domain's 4096 roots of unity in bit-reversed order, then 1/4096 (Fr381 Montgomery)
+  //   kzg_cells_tw (kzg_cells.cu): w^i for the 8192nd root w, i < 8192, then 1/4096 (Fr381 Montgomery)
+  //   secp_gtab (secp256k1.cu): d G for d = 1 .. 4095 as affine secp256k1 points (256 KB)
+  //   p256_gtab (secp256r1.cu): the same table for the P-256 generator (affine, Montgomery form, 256 KB)
+  b200zk::OnceTable kzg_roots, kzg_cells_tw, secp_gtab, p256_gtab;
+  b200zk::DevBuf ws_kzg;      // EIP-4844 / EIP-7594 proofs and cells: blobs, z, quotients, partial sums and encoded results of one call
   b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
                               // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu) and
                               // P256VERIFY (secp256r1.cu) batches
-  // ECRECOVER (secp256k1.cu): d G for d = 1 .. 4095 as affine secp256k1 points (256 KB), built once per context on first use;
-  // consumers on other streams wait on secp_gtab_ready
-  b200zk::DevBuf secp_gtab;
-  cudaEvent_t secp_gtab_ready = nullptr;
-  // P256VERIFY (secp256r1.cu): the same table for the P-256 generator (affine, Montgomery form, 256 KB), waited on through
-  // p256_gtab_ready
-  b200zk::DevBuf p256_gtab;
-  cudaEvent_t p256_gtab_ready = nullptr;
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
   cudaEvent_t ev[8] = {};
-  // grow-only workspaces
+  // grow-only workspaces (every DevBuf, OnceTable and BasesEntry frees itself when the context is deleted)
   b200zk::DevBuf ws_hist, ws_offsets, ws_cursor, ws_blocksums, ws_idx, ws_buckets, ws_chunkS, ws_chunkV, ws_result,
       ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segoff, ws_segbucket, ws_digits, ws_q0, ws_q1, ws_prefix, ws_info, ws_pairoff0, ws_pairoff1;
   // 2^28-th primitive root of unity of Fr the NTT derives its domain generators from (canonical limbs).
@@ -180,6 +204,64 @@ struct Carve {
     return p;
   }
 };
+
+// runs layout(Carve&) once to size the call's buffers, grows ws to fit, then runs it again over ws.p
+template <class Layout> int carve(b200zk_ctx* ctx, DevBuf& ws, Layout&& layout) {
+  Carve c;
+  layout(c);
+  B2_TRY(ensure(ctx, ws, c.off + 256));
+  c = Carve{(uint8_t*)ws.p, 0};
+  layout(c);
+  return B200ZK_OK;
+}
+
+// The table t (bytes long) on stream st: the first call allocates it, enqueues enqueue_build(void* table) (an int status)
+// and records t.ready behind it; later calls wait on t.ready.  A failed build leaves t unbuilt, so the next call builds it
+// again.  Without an event the build is synchronised here instead.
+template <class Build>
+int once_table(b200zk_ctx* ctx, OnceTable& t, size_t bytes, cudaStream_t st, Build&& enqueue_build, const void** out) {
+  if (!t.built) {
+    B2_TRY(ensure(ctx, t.buf, bytes));
+    B2_TRY(enqueue_build(t.buf.p));
+    if (!t.ready && cudaEventCreateWithFlags(&t.ready, cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); t.ready = nullptr; }
+    if (t.ready) B2_CUDA(ctx, cudaEventRecord(t.ready, st));
+    else B2_CUDA(ctx, cudaStreamSynchronize(st));
+    t.built = true;
+  } else if (t.ready) {
+    B2_CUDA(ctx, cudaStreamWaitEvent(st, t.ready, 0));
+  }
+  *out = t.buf.p;
+  return B200ZK_OK;
+}
+
+// the resident bases behind handle (of group g), or nullptr after failing with msg
+inline BasesEntry* find_bases(b200zk_ctx* ctx, uint64_t handle, const char* msg) {
+  auto it = ctx->bases.find(handle);
+  if (it != ctx->bases.end()) return &it->second;
+  fail(ctx, B200ZK_ERR_INVALID_ARG, msg);
+  return nullptr;
+}
+inline BasesEntry* find_bases(b200zk_ctx* ctx, uint64_t handle, Group g, const char* msg) {
+  BasesEntry* e = find_bases(ctx, handle, msg);
+  if (!e || e->group == g) return e;
+  fail(ctx, B200ZK_ERR_INVALID_ARG, msg);
+  return nullptr;
+}
+
+// takes ownership of a filled entry under a new handle
+inline int register_bases(b200zk_ctx* ctx, BasesEntry&& e, uint64_t* handle) {
+  *handle = ctx->next_handle++;
+  ctx->bases.emplace(*handle, std::move(e));
+  return B200ZK_OK;
+}
+
+// pair_offsets of `count` >= 1 checks: first entry 0, never decreasing
+inline int check_offsets(b200zk_ctx* ctx, const uint32_t* offsets, size_t count, const char* what) {
+  if (offsets[0] != 0) return fail(ctx, B200ZK_ERR_INVALID_ARG, (std::string(what) + ": pair_offsets[0] must be 0").c_str());
+  for (size_t i = 0; i < count; ++i)
+    if (offsets[i + 1] < offsets[i]) return fail(ctx, B200ZK_ERR_INVALID_ARG, (std::string(what) + ": pair_offsets must be non-decreasing").c_str());
+  return B200ZK_OK;
+}
 
 // every kernel launch in the library goes through this macro so gpu_launches is a count, not a guess
 #define B2_LAUNCH(ctx, kernel, grid, block, smem, st, ...)                                   \
@@ -305,7 +387,7 @@ void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_
 void hash_to_bls_field(const uint8_t digest[32], uint8_t out_be[32]);
 int kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st);
 // the setup handle of a KZG call: a BLS12-381 G1 handle of exactly 4096 points, else status 4 naming `what`
-int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const BasesEntry** e);
+int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, BasesEntry** e);
 // one 4096-point MSM per blob over the setup (scalars n x 4096 x 32 bytes): XYZZ partial sums 192 B apart, each encoded into
 // its own 128-byte slot of enc (the 48-byte compressed point first)
 int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_t n, uint32_t flags, uint8_t* partials, uint8_t* enc, cudaStream_t st);
@@ -316,5 +398,19 @@ int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_
 int kzg_cells_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, uint8_t* d_cells, cudaStream_t st);
 int kzg_cell_scalars_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, const uint8_t* d_r_be, void* d_weights, void* d_partial,
                          void* d_s_proof, void* d_s_lin, void* d_s_setup, cudaStream_t st);
+
+// every element of n_blobs big-endian blobs, and of the n_extra z values right behind them, < r; else status 2 naming
+// `what` and the first offending blob and element (or z)
+inline int check_blobs(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n_blobs, size_t n_extra, cudaStream_t st, const char* what) {
+  constexpr size_t kElems = 4096;  // FIELD_ELEMENTS_PER_BLOB
+  const size_t elems = n_blobs * kElems;
+  size_t bad = elems + n_extra;
+  B2_TRY(bls_scalars_check(ctx, d_blobs, elems + n_extra, true, st, &bad));
+  if (bad >= elems + n_extra) return B200ZK_OK;
+  char msg[160];
+  if (bad < elems) snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kElems, bad % kElems);
+  else snprintf(msg, sizeof msg, "%s: z of blob %zu is >= the BLS12-381 group order", what, bad - elems);
+  return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+}
 
 }  // namespace b200zk

@@ -36,10 +36,9 @@ int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const 
   size_t wit_end = 0;  // witness entries the columns reach
   for (int k = 0; k < 5; ++k) {
     if (!pk->handle[k]) { if (k == 1) continue; return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_commit: only the B_g1 column may be absent"); }
-    auto it = ctx->bases.find(pk->handle[k]);
-    if (it == ctx->bases.end() || it->second.bls || it->second.g2 != (k == 2)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_commit: unknown handle or wrong group for a column");
-    if (pk->count[k] > it->second.n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_commit: a column count exceeds its resident bases");
-    col[k] = &it->second;
+    col[k] = find_bases(ctx, pk->handle[k], k == 2 ? Group::Bn254G2 : Group::Bn254G1, "groth16_commit: unknown handle or wrong group for a column");
+    if (!col[k]) return B200ZK_ERR_INVALID_ARG;
+    if (pk->count[k] > col[k]->n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_commit: a column count exceeds its resident bases");
     if (k < 4 && pk->offset[k] + pk->count[k] > wit_end) wit_end = pk->offset[k] + pk->count[k];
   }
   if (pk->offset[4] + pk->count[4] > n) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_commit: the H column reaches past the quotient's 2^log_n coefficients");
@@ -83,14 +82,14 @@ int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const 
     for (int j = k + 1; j < 4 && !donor; ++j)
       donor = col[j] && cnt >= 2 && pk->offset[j] == pk->offset[k] && pk->count[j] == cnt && col[j]->table_c == col[k]->table_c && (!col[k]->table_c || col[j]->n == col[k]->n);
     const int mode = share ? 2 : (donor ? 1 : 0);
-    int rc = (k == 2) ? msm_run_g2(ctx, col[k]->d, sc, cnt, wflags, st, out + kPartialOff[k], col[k]->table_c, col[k]->n, nullptr, mode)
-                      : msm_run_g1(ctx, col[k]->d, sc, cnt, wflags, st, out + kPartialOff[k], col[k]->table_c, col[k]->n, nullptr, mode);
+    int rc = (k == 2) ? msm_run_g2(ctx, col[k]->d.p, sc, cnt, wflags, st, out + kPartialOff[k], col[k]->table_c, col[k]->n, nullptr, mode)
+                      : msm_run_g1(ctx, col[k]->d.p, sc, cnt, wflags, st, out + kPartialOff[k], col[k]->table_c, col[k]->n, nullptr, mode);
     if (rc > B200ZK_OK_INFINITY) return rc;
     if (!share) prev = k;
   }
   {
     const uint8_t* hc = (const uint8_t*)d_a + pk->offset[4] * 32;
-    int rc = msm_run_g1(ctx, col[4]->d, hc, pk->count[4], B200ZK_SCALARS_MONT, st, out + kPartialOff[4], col[4]->table_c, col[4]->n, nullptr, 0);
+    int rc = msm_run_g1(ctx, col[4]->d.p, hc, pk->count[4], B200ZK_SCALARS_MONT, st, out + kPartialOff[4], col[4]->table_c, col[4]->n, nullptr, 0);
     if (rc > B200ZK_OK_INFINITY) return rc;
   }
   return B200ZK_OK;
@@ -109,14 +108,17 @@ static bool fr_canonical(const uint8_t* x) {
 // the key terms of a b200zk_groth16_zk: plain (not precomputed) BN254 bases of the right group and point count
 static int zk_terms(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void** g1, const void** g2) {
   if (!zk) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: null argument");
-  auto it1 = ctx->bases.find(zk->g1_terms), it2 = ctx->bases.find(zk->g2_terms);
-  if (it1 == ctx->bases.end() || it1->second.bls || it1->second.g2 || it1->second.table_c || it1->second.n != 3)
-    return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: g1_terms must be a plain G1 handle of 3 points (alpha, beta, delta)");
-  if (it2 == ctx->bases.end() || it2->second.bls || !it2->second.g2 || it2->second.table_c || it2->second.n != 2)
-    return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: g2_terms must be a plain G2 handle of 2 points (beta, delta)");
+  static const char* kG1 = "groth16 zk: g1_terms must be a plain G1 handle of 3 points (alpha, beta, delta)";
+  static const char* kG2 = "groth16 zk: g2_terms must be a plain G2 handle of 2 points (beta, delta)";
+  const BasesEntry* e1 = find_bases(ctx, zk->g1_terms, Group::Bn254G1, kG1);
+  if (!e1) return B200ZK_ERR_INVALID_ARG;
+  if (e1->table_c || e1->n != 3) return fail(ctx, B200ZK_ERR_INVALID_ARG, kG1);
+  const BasesEntry* e2 = find_bases(ctx, zk->g2_terms, Group::Bn254G2, kG2);
+  if (!e2) return B200ZK_ERR_INVALID_ARG;
+  if (e2->table_c || e2->n != 2) return fail(ctx, B200ZK_ERR_INVALID_ARG, kG2);
   if (!fr_canonical(zk->r) || !fr_canonical(zk->s)) return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, "groth16 zk: r or s is not below the group order");
-  *g1 = it1->second.d;
-  *g2 = it2->second.d;
+  *g1 = e1->d.p;
+  *g2 = e2->d.p;
   return B200ZK_OK;
 }
 

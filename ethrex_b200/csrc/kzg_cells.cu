@@ -348,16 +348,12 @@ __global__ void __launch_bounds__(kDft / 2, 1) kzg_fk20_proofs(const void* __res
   bls_g1_compress(proofs + 48 * (base + kCellN + t), xyzz_to_affine(load_xyzz<Fp381>(s_pts, kCellN + t)));
 }
 
-// the twiddle table, built on first use; later calls on any stream wait on its event
+// the twiddle table, built on first use
 int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
-  if (!ctx->kzg_cells_tw.p) {
-    B2_TRY(ensure(ctx, ctx->kzg_cells_tw, (kExtN + 1) * 32));
-    B2_LAUNCH(ctx, kzg_cells_tw_build, (kExtN + 256) / 256, 256, 0, st, ctx->kzg_cells_tw.p);
-    if (cudaEventCreateWithFlags(&ctx->kzg_cells_tw_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(ctx->kzg_cells_tw_ready, st));
-    else { cudaGetLastError(); ctx->kzg_cells_tw_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
-  } else if (ctx->kzg_cells_tw_ready) {
-    B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->kzg_cells_tw_ready, 0));
-  }
+  B2_TRY(once_table(ctx, ctx->kzg_cells_tw, (kExtN + 1) * 32, st, [&](void* t) -> int {
+    B2_LAUNCH(ctx, kzg_cells_tw_build, (kExtN + 256) / 256, 256, 0, st, t);
+    return B200ZK_OK;
+  }, tw));
   if (!ctx->attr_kzg_cells) {
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_extend, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
@@ -365,22 +361,15 @@ int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_fk20_columns, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColSmem));
     ctx->attr_kzg_cells = true;
   }
-  *tw = ctx->kzg_cells_tw.p;
   return B200ZK_OK;
 }
 
-// the FK20 table of a monomial setup, built on the handle's first cell-proof call; later calls on any stream wait on its event
+// the FK20 table of a monomial setup, built on the handle's first cell-proof call
 int fk20_table(b200zk_ctx* ctx, BasesEntry& e, const void* tw, cudaStream_t st, const void** table) {
-  if (!e.fk20) {
-    B2_CUDA(ctx, cudaMalloc(&e.fk20, (size_t)kCellN * kDft * 96));
-    B2_LAUNCH(ctx, kzg_fk20_table, kCellN, kDft / 2, 0, st, (const void*)e.d, tw, e.fk20);
-    if (cudaEventCreateWithFlags(&e.fk20_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(e.fk20_ready, st));
-    else { cudaGetLastError(); e.fk20_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
-  } else if (e.fk20_ready) {
-    B2_CUDA(ctx, cudaStreamWaitEvent(st, e.fk20_ready, 0));
-  }
-  *table = e.fk20;
-  return B200ZK_OK;
+  return once_table(ctx, e.fk20, (size_t)kCellN * kDft * 96, st, [&](void* t) -> int {
+    B2_LAUNCH(ctx, kzg_fk20_table, kCellN, kDft / 2, 0, st, (const void*)e.d.p, tw, t);
+    return B200ZK_OK;
+  }, table);
 }
 
 }  // namespace
@@ -417,19 +406,11 @@ int b200zk_kzg_compute_cells(b200zk_ctx* ctx, const uint8_t* blobs, size_t n_blo
   if (!n_blobs) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
   uint8_t *d_blobs, *d_cells;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_kzg, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_kzg.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_kzg, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(n_blobs * kN * 32); d_cells = c.take<uint8_t>(n_blobs * kExtN * 32);
-  }
+  }));
   B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, n_blobs * kN * 32, cudaMemcpyHostToDevice, st));
-  size_t bad = 0;
-  B2_TRY(bls_scalars_check(ctx, d_blobs, n_blobs * kN, true, st, &bad));
-  if (bad < n_blobs * kN) {
-    char msg[160];
-    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kN, bad % kN);
-    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
-  }
+  B2_TRY(check_blobs(ctx, d_blobs, n_blobs, 0, st, what));
   B2_TRY(kzg_cells_run(ctx, d_blobs, n_blobs, d_cells, st));
   B2_CUDA(ctx, cudaMemcpyAsync(cells, d_cells, n_blobs * kExtN * 32, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
@@ -442,33 +423,25 @@ int b200zk_kzg_blob_to_commitment_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_l
   if (!ctx || (n_blobs && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_blob_to_commitment_and_cell_proofs: null argument");
   NvtxRange nvtx("b200zk:kzg_blob_to_commitment_and_cell_proofs");
   DeviceGuard guard(ctx);
-  const BasesEntry *lag = nullptr, *mono = nullptr;
+  BasesEntry *lag = nullptr, *mono = nullptr;
   B2_TRY(kzg_setup(ctx, g1_lagrange, "kzg_blob_to_commitment_and_cell_proofs (g1_lagrange)", &lag));
   B2_TRY(kzg_setup(ctx, g1_monomial, "kzg_blob_to_commitment_and_cell_proofs (g1_monomial)", &mono));
   if (!n_blobs) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
   uint8_t *d_blobs, *d_hat, *d_u, *d_partials, *d_enc, *d_proofs;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_kzg, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_kzg.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_kzg, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(n_blobs * kN * 32);
     d_hat = c.take<uint8_t>(n_blobs * kDft * kCellN * 32);
     d_u = c.take<uint8_t>(n_blobs * kDft * 192);
     d_partials = c.take<uint8_t>(n_blobs * 192);
     d_enc = c.take<uint8_t>(n_blobs * 128);
     d_proofs = c.take<uint8_t>(n_blobs * kCells * 48);
-  }
+  }));
   B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, n_blobs * kN * 32, cudaMemcpyHostToDevice, st));
-  size_t bad = 0;
-  B2_TRY(bls_scalars_check(ctx, d_blobs, n_blobs * kN, true, st, &bad));
-  if (bad < n_blobs * kN) {
-    char msg[160];
-    snprintf(msg, sizeof msg, "%s: blob %zu, element %zu is >= the BLS12-381 group order", what, bad / kN, bad % kN);
-    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
-  }
+  B2_TRY(check_blobs(ctx, d_blobs, n_blobs, 0, st, what));
   const void *tw = nullptr, *table = nullptr;
   B2_TRY(cells_tw(ctx, st, &tw));
-  B2_TRY(fk20_table(ctx, ctx->bases[g1_monomial], tw, st, &table));
+  B2_TRY(fk20_table(ctx, *mono, tw, st, &table));
   B2_LAUNCH(ctx, kzg_fk20_columns, (unsigned)n_blobs, kThreads, kColSmem, st, (const uint8_t*)d_blobs, tw, (void*)d_hat);
   const size_t n_msm = n_blobs * kDft;
   B2_LAUNCH(ctx, kzg_fk20_msm, (unsigned)((n_msm + kMsmWarps - 1) / kMsmWarps), 32 * kMsmWarps, 0, st, table, (const void*)d_hat, n_msm, (void*)d_u);

@@ -278,22 +278,22 @@ int bn254_g1_mul_batch(b200zk_ctx* ctx, const uint8_t* points, const uint8_t* sc
 
 int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint32_t* pair_offsets, size_t count, uint8_t* result, uint8_t* status) {
   if (!count) return B200ZK_OK;
-  if (pair_offsets[0] != 0) return fail(ctx, B200ZK_ERR_INVALID_ARG, "pairing_check_batch: pair_offsets[0] must be 0");
-  for (size_t i = 0; i < count; ++i)
-    if (pair_offsets[i + 1] < pair_offsets[i]) return fail(ctx, B200ZK_ERR_INVALID_ARG, "pairing_check_batch: pair_offsets must be non-decreasing");
+  B2_TRY(check_offsets(ctx, pair_offsets, count, "pairing_check_batch"));
   const size_t n_pairs = pair_offsets[count];
   cudaStream_t st = ctx->stream;
-  // workspace: [pairs 192 B][Fq12 384 B][pair status 1 B] per pair, then [offsets][result][status] per check
-  const size_t off_f = (n_pairs * 192 + 15) & ~(size_t)15, off_ps = off_f + n_pairs * sizeof(Fq12);
-  const size_t off_offs = (off_ps + n_pairs + 15) & ~(size_t)15, off_res = off_offs + (count + 1) * 4, off_st = off_res + count;
-  B2_TRY(ensure(ctx, ctx->ws_points, off_st + count));
-  uint8_t* base = (uint8_t*)ctx->ws_points.p;
-  if (n_pairs) B2_CUDA(ctx, cudaMemcpyAsync(base, pairs, n_pairs * 192, cudaMemcpyHostToDevice, st));
-  B2_CUDA(ctx, cudaMemcpyAsync(base + off_offs, pair_offsets, (count + 1) * 4, cudaMemcpyHostToDevice, st));
-  if (n_pairs) B2_LAUNCH(ctx, pairing_miller, (unsigned)((n_pairs + 31) / 32), 32, 0, st, base, n_pairs, (Fq12*)(base + off_f), base + off_ps);
-  B2_LAUNCH(ctx, pairing_final, (unsigned)((count + 31) / 32), 32, 0, st, (const Fq12*)(base + off_f), base + off_ps, (const uint32_t*)(base + off_offs), count, base + off_res, base + off_st);
-  B2_CUDA(ctx, cudaMemcpyAsync(result, base + off_res, count, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(ctx, cudaMemcpyAsync(status, base + off_st, count, cudaMemcpyDeviceToHost, st));
+  uint8_t *in, *pst, *res, *sts;
+  Fq12* f;
+  uint32_t* offs;
+  B2_TRY(carve(ctx, ctx->ws_points, [&](Carve& c) {
+    in = c.take<uint8_t>(192 * n_pairs); f = c.take<Fq12>(n_pairs); pst = c.take<uint8_t>(n_pairs);
+    offs = c.take<uint32_t>(count + 1); res = c.take<uint8_t>(count); sts = c.take<uint8_t>(count);
+  }));
+  if (n_pairs) B2_CUDA(ctx, cudaMemcpyAsync(in, pairs, n_pairs * 192, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(offs, pair_offsets, (count + 1) * 4, cudaMemcpyHostToDevice, st));
+  if (n_pairs) B2_LAUNCH(ctx, pairing_miller, (unsigned)((n_pairs + 31) / 32), 32, 0, st, in, n_pairs, f, pst);
+  B2_LAUNCH(ctx, pairing_final, (unsigned)((count + 31) / 32), 32, 0, st, (const Fq12*)f, pst, (const uint32_t*)offs, count, res, sts);
+  B2_CUDA(ctx, cudaMemcpyAsync(result, res, count, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(status, sts, count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   return B200ZK_OK;
 }

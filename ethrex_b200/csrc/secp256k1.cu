@@ -32,18 +32,12 @@ __global__ void __launch_bounds__(kRecoverThreads) secp256k1_ecrecover_kernel(co
   dst[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
-// the G table, built on first use; later calls on any stream wait on its event
-int secp_gtab(b200zk_ctx* ctx, cudaStream_t st, const Affine<SecpFp>** table) {
-  if (!ctx->secp_gtab.p) {
-    B2_TRY(ensure(ctx, ctx->secp_gtab, kSecpGTable * sizeof(Affine<SecpFp>)));
-    B2_LAUNCH(ctx, secp256k1_gtab_build, (kSecpGTable + 255) / 256, 256, 0, st, (Affine<SecpFp>*)ctx->secp_gtab.p);
-    if (cudaEventCreateWithFlags(&ctx->secp_gtab_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(ctx->secp_gtab_ready, st));
-    else { cudaGetLastError(); ctx->secp_gtab_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
-  } else if (ctx->secp_gtab_ready) {
-    B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->secp_gtab_ready, 0));
-  }
-  *table = (const Affine<SecpFp>*)ctx->secp_gtab.p;
-  return B200ZK_OK;
+// the G table, built on first use
+int secp_gtab(b200zk_ctx* ctx, cudaStream_t st, const void** table) {
+  return once_table(ctx, ctx->secp_gtab, kSecpGTable * sizeof(Affine<SecpFp>), st, [&](void* t) -> int {
+    B2_LAUNCH(ctx, secp256k1_gtab_build, (kSecpGTable + 255) / 256, 256, 0, st, (Affine<SecpFp>*)t);
+    return B200ZK_OK;
+  }, table);
 }
 
 }  // namespace
@@ -62,18 +56,16 @@ int b200zk_secp256k1_ecrecover_batch(b200zk_ctx* ctx, const uint8_t* sigs, const
   DeviceGuard guard(ctx);
   if (!count) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
-  const Affine<SecpFp>* gtab;
+  const void* gtab;
   B2_TRY(secp_gtab(ctx, st, &gtab));
   uint8_t *dsig, *dmsg, *dout, *dst;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     dsig = c.take<uint8_t>(65 * count); dmsg = c.take<uint8_t>(32 * count); dout = c.take<uint8_t>(32 * count); dst = c.take<uint8_t>(count);
-  }
+  }));
   B2_CUDA(ctx, cudaMemcpyAsync(dsig, sigs, 65 * count, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(dmsg, msgs, 32 * count, cudaMemcpyHostToDevice, st));
   B2_LAUNCH(ctx, secp256k1_ecrecover_kernel, (unsigned)((count + kRecoverThreads - 1) / kRecoverThreads), kRecoverThreads, 0, st,
-            (const uint8_t*)dsig, (const uint8_t*)dmsg, count, flags, gtab, dout, dst);
+            (const uint8_t*)dsig, (const uint8_t*)dmsg, count, flags, (const Affine<SecpFp>*)gtab, dout, dst);
   B2_CUDA(ctx, cudaMemcpyAsync(out, dout, 32 * count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(status, dst, count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));

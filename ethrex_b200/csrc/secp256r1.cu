@@ -25,18 +25,12 @@ __global__ void __launch_bounds__(kVerifyThreads) secp256r1_verify_kernel(const 
   result[i] = p256_verify(inputs + 160 * i, gtab) ? 1 : 0;
 }
 
-// the G table, built on first use; later calls on any stream wait on its event
-int p256_gtab(b200zk_ctx* ctx, cudaStream_t st, const Affine<P256Fp>** table) {
-  if (!ctx->p256_gtab.p) {
-    B2_TRY(ensure(ctx, ctx->p256_gtab, kSecpGTable * sizeof(Affine<P256Fp>)));
-    B2_LAUNCH(ctx, secp256r1_gtab_build, (kSecpGTable + 255) / 256, 256, 0, st, (Affine<P256Fp>*)ctx->p256_gtab.p);
-    if (cudaEventCreateWithFlags(&ctx->p256_gtab_ready, cudaEventDisableTiming) == cudaSuccess) B2_CUDA(ctx, cudaEventRecord(ctx->p256_gtab_ready, st));
-    else { cudaGetLastError(); ctx->p256_gtab_ready = nullptr; B2_CUDA(ctx, cudaStreamSynchronize(st)); }
-  } else if (ctx->p256_gtab_ready) {
-    B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->p256_gtab_ready, 0));
-  }
-  *table = (const Affine<P256Fp>*)ctx->p256_gtab.p;
-  return B200ZK_OK;
+// the G table, built on first use
+int p256_gtab(b200zk_ctx* ctx, cudaStream_t st, const void** table) {
+  return once_table(ctx, ctx->p256_gtab, kSecpGTable * sizeof(Affine<P256Fp>), st, [&](void* t) -> int {
+    B2_LAUNCH(ctx, secp256r1_gtab_build, (kSecpGTable + 255) / 256, 256, 0, st, (Affine<P256Fp>*)t);
+    return B200ZK_OK;
+  }, table);
 }
 
 }  // namespace
@@ -53,17 +47,13 @@ int b200zk_secp256r1_verify_batch(b200zk_ctx* ctx, const uint8_t* inputs, size_t
   DeviceGuard guard(ctx);
   if (!count) return B200ZK_OK;
   cudaStream_t st = ctx->stream;
-  const Affine<P256Fp>* gtab;
+  const void* gtab;
   B2_TRY(p256_gtab(ctx, st, &gtab));
   uint8_t *din, *dres;
-  Carve c;
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass) { B2_TRY(ensure(ctx, ctx->ws_pairing, c.off + 256)); c = Carve{(uint8_t*)ctx->ws_pairing.p, 0}; }
-    din = c.take<uint8_t>(160 * count); dres = c.take<uint8_t>(count);
-  }
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) { din = c.take<uint8_t>(160 * count); dres = c.take<uint8_t>(count); }));
   B2_CUDA(ctx, cudaMemcpyAsync(din, inputs, 160 * count, cudaMemcpyHostToDevice, st));
   B2_LAUNCH(ctx, secp256r1_verify_kernel, (unsigned)((count + kVerifyThreads - 1) / kVerifyThreads), kVerifyThreads, 0, st,
-            (const uint8_t*)din, count, gtab, dres);
+            (const uint8_t*)din, count, (const Affine<P256Fp>*)gtab, dres);
   B2_CUDA(ctx, cudaMemcpyAsync(result, dres, count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   return B200ZK_OK;
