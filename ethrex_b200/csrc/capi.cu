@@ -192,10 +192,9 @@ int b200zk_init(int device, b200zk_ctx** out) {
   {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);  // hi = numerically lowest = greatest priority
-    if (cudaStreamCreateWithPriority(&ctx->stream_sort, cudaStreamNonBlocking, hi) != cudaSuccess) { cudaGetLastError(); b200zk_destroy(ctx); return B200ZK_ERR_CUDA; }
+    if (cudaStreamCreateWithPriority(&ctx->stream_upload, cudaStreamNonBlocking, hi) != cudaSuccess) { cudaGetLastError(); b200zk_destroy(ctx); return B200ZK_ERR_CUDA; }
     cudaEventCreateWithFlags(&ctx->ev_in, cudaEventDisableTiming);
     for (auto& e : ctx->ev_up) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    for (auto& sl : ctx->slot) { cudaEventCreateWithFlags(&sl.sorted, cudaEventDisableTiming); cudaEventCreateWithFlags(&sl.released, cudaEventDisableTiming); }
   }
   *out = ctx;
   return B200ZK_OK;
@@ -209,13 +208,9 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   cudaDeviceSynchronize();
   // the resident bases, the once-built tables and every workspace DevBuf free themselves (here and in `delete ctx`)
   ctx->bases.clear();
-  for (auto& sl : ctx->slot) {
-    if (sl.sorted) cudaEventDestroy(sl.sorted);
-    if (sl.released) cudaEventDestroy(sl.released);
-  }
   if (ctx->ev_in) cudaEventDestroy(ctx->ev_in);
   for (auto& e : ctx->ev_up) if (e) cudaEventDestroy(e);
-  if (ctx->stream_sort) cudaStreamDestroy(ctx->stream_sort);
+  if (ctx->stream_upload) cudaStreamDestroy(ctx->stream_upload);
   for (auto& kv : ctx->twiddles) { cudaFree(kv.second.d); if (kv.second.ready) cudaEventDestroy(kv.second.ready); }
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);

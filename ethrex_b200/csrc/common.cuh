@@ -53,9 +53,11 @@ struct TwiddleSet {   // per (log_n, direction): see ntt.cu
   cudaEvent_t ready = nullptr;  // recorded behind the build kernel: consumers on OTHER streams wait on it
 };
 
-struct SortSlot {  // one of the two sort workspaces of the chunk-pipelined MSM
+// the MSM's digit sort (msm.cu sort_digits) and its run offsets: hist / offsets / idx are the sort, run_off numbers the
+// accumulation's runs, tsum is scan scratch; digits and cursor serve the one-pass sort only, key / ctab / cnt2 the
+// two-level sort only
+struct SortWorkspace {
   DevBuf hist, offsets, cursor, run_off, tsum, digits, idx, key, ctab, cnt2;
-  cudaEvent_t sorted = nullptr, released = nullptr;
 };
 
 // Bls12G1: Fp381 Montgomery, 96 B affine, the KZG trusted setup; Bls12G2: Fp2 over Fp381, 192 B affine, followed by the
@@ -93,13 +95,12 @@ struct b200zk_ctx {
   std::string last_error;
   uint64_t launches = 0;
   uint32_t msm_window = 0;
-  uint32_t msm_chunks = 0;   // chunk count of the pipelined MSM schedule; 0 = automatic
-  cudaStream_t stream_sort = nullptr;  // high-priority stream the sort of chunk k+1 runs on while chunk k accumulates
+  uint32_t msm_chunks = 0;   // chunk count of the MSM schedule; 0 = automatic
+  cudaStream_t stream_upload = nullptr;  // copy stream: host scalars of a chunked MSM upload on it, one chunk ahead of the kernels
   cudaEvent_t ev_in = nullptr;
-  cudaEvent_t ev_up[64] = {};  // upload k of the chunk-pipelined MSM has landed (recorded on stream_sort, waited on by the caller's stream)
-  b200zk::SortSlot slot[2];
+  cudaEvent_t ev_up[64] = {};  // upload k of a chunked MSM has landed (recorded on stream_upload, waited on by the caller's stream)
+  b200zk::SortWorkspace sort;
   b200zk::DevBuf ws_totals, ws_bitpart;
-  b200zk::DevBuf ws_key, ws_ctab, ws_cnt2;  // two-level sort: 16-bit fine keys of the coarse-partitioned entries; per-(bin, CTA) counts / bases
   b200zk::DevBuf ws_g16[4];   // b200zk_groth16_commit: staged A/B/C evaluations (host inputs) and the 768-byte partial block
   b200zk::DevBuf ws_zinv;     // 1/(5^n - 1) of the last quotient domain, canonical limbs (cached per log_n)
   uint32_t zinv_log_n = 0xffffffffu;
@@ -120,8 +121,8 @@ struct b200zk_ctx {
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
   cudaEvent_t ev[8] = {};
   // grow-only workspaces (every DevBuf, OnceTable and BasesEntry frees itself when the context is deleted)
-  b200zk::DevBuf ws_hist, ws_offsets, ws_cursor, ws_blocksums, ws_idx, ws_buckets, ws_chunkS, ws_chunkV, ws_result,
-      ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segoff, ws_segbucket, ws_digits, ws_q0, ws_q1, ws_prefix, ws_info, ws_pairoff0, ws_pairoff1;
+  b200zk::DevBuf ws_buckets, ws_chunkS, ws_chunkV, ws_result, ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segbucket, ws_q0, ws_q1,
+      ws_prefix, ws_info, ws_pairoff0, ws_pairoff1;
   // 2^28-th primitive root of unity of Fr the NTT derives its domain generators from (canonical limbs).
   // Default = ark-poly / gnark-crypto 5^((r-1)/2^28); halo2curves uses 7^((r-1)/2^28) (b200zk_set_ntt_root).
   uint32_t ntt_root[8] = {0x725b19f0u, 0x9bd61b6eu, 0x41112ed4u, 0x402d111eu, 0x8ef62abcu, 0x00e0a7ebu, 0xa58a7e85u, 0x2a3c09f0u};

@@ -77,7 +77,7 @@ int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const 
     const uint8_t* sc = d_wit + pk->offset[k] * 32;
     bool share = prev >= 0 && cnt >= 2 && pk->offset[prev] == pk->offset[k] && pk->count[prev] == cnt && col[prev]->table_c == col[k]->table_c &&
                  (!col[k]->table_c || col[prev]->n == col[k]->n);
-    // is this column followed by one that can reuse its sort?  (then it must run the one-shot schedule and keep it)
+    // is this column followed by one that can reuse its sort?  (then it must run as one chunk and keep it)
     bool donor = false;
     for (int j = k + 1; j < 4 && !donor; ++j)
       donor = col[j] && cnt >= 2 && pk->offset[j] == pk->offset[k] && pk->count[j] == cnt && col[j]->table_c == col[k]->table_c && (!col[k]->table_c || col[j]->n == col[k]->n);

@@ -3,33 +3,32 @@
 // Replaces ark_ec::VariableBaseMSM::msm (ark-ec 0.5.0, /root/reference/Cargo.lock:978) as reached by the
 // Groth16 wrap behind /root/reference/crates/prover/src/backend/sp1.rs:97-134 and risc0.rs:24-29,71-82
 // (SURVEY.md section 8a rows a6/a7).  Same digit rule as ark's `make_digits` (signed radix-2^c digits, carry
-// when the window value >= 2^(c-1), 2^(c-1) buckets per window), but the schedule is GPU shaped:
+// when the window value >= 2^(c-1), 2^(c-1) buckets per window), but the schedule is GPU shaped (msm_run):
 //
-//   1. msm_hist      one thread per scalar: recode into W signed digits, store them window-major, histogram
-//                    (window,bucket) with warp-aggregated global atomics (the W*2^(c-1) counters live in L2);
-//   2. scan_*        exclusive prefix sums -> bucket offsets and segment offsets (3 small kernels each);
-//   3. msm_scatter   walk the digits window by window and drop each point index, with the digit's sign in
-//                    bit 31, into its bucket's slice of the sorted index array (one window's slice is L2 sized);
-//   4. msm_accumulate  THE hot kernel: one thread per fixed SLICE of 256 sorted entries (perfectly balanced):
+//   1. digit sort    recode every scalar into W signed digits and sort the (window,bucket) entries: each becomes a
+//                    point index with the digit's sign in bit 31, bucket-major.  The two-level sort (msm_sort_*: tile-
+//                    local counting sorts in shared memory) from 2^16 points up; below that the one-pass sort (msm_hist
+//                    histogram, scan, msm_scatter);
+//   2. scan_*        exclusive prefix sums -> the runs' offsets (3 small kernels, exclusive_scan);
+//   3. msm_accumulate  THE hot kernel: one thread per fixed SLICE of <= 256 sorted entries (perfectly balanced):
 //                    gathers 64/128-byte affine bases with 128-bit loads, one ahead of the addition in
 //                    flight, folds them into an XYZZ accumulator (8M+2S per point) and closes a run at every
-//                    bucket boundary; partial_tree then sums the runs of buckets that have more than one;
-//   5. bucket_chunk / bucket_tree  sum_b (b+1)*B_b per window: running sums over chunks of 32 buckets, then a
-//                    log-depth pairwise tree carrying (sum, weighted sum) -- no serial 2^(c-1) loop anywhere;
-//   6. msm_horner    sum_w 2^(c*w) * S_w in one thread (W*c doublings), leaving one XYZZ partial sum.
+//                    bucket boundary; partial_tree then sums the runs of buckets that have many;
+//   4. bucket_merge / bucket_chunk / bucket_bitsums or bucket_tree  sum_b (b+1)*B_b per window: bucket totals, running
+//                    sums over chunks of 16 buckets, then a log-depth combination -- no serial 2^(c-1) loop anywhere;
+//   5. msm_horner    sum_w 2^(c*w) * S_w in one thread (W*c doublings), leaving one XYZZ partial sum.
 //
+// Large MSMs over host scalars run steps 1-3 once per chunk of points while the next chunk's scalars upload.
 // The affine normalisation / byte encoding (msm_encode) is a separate single-thread kernel so that the
 // multi-GPU path can all-gather the 128/256-byte XYZZ partials first (SURVEY.md section 8e).
 #include "common.cuh"
 #include "tma.cuh"
-#include <cstdlib>
 
 namespace b200zk {
 
 static constexpr int kMaxWindows = 64;
 static constexpr uint32_t kMaxPipelineChunks = 64;  // = events in b200zk_ctx::ev_up
-static constexpr int kChunk = 16;  // buckets per running-sum chunk (B200ZK_CHUNK=8|32|64 selects others)
-static constexpr int kG2MinBlocks = 1;  // register cap of msm_accumulate<Fq2> (see the launch site)
+static constexpr int kChunk = 16;  // buckets per running-sum chunk
 
 struct MsmPlan {
   uint32_t c, W, B;       // window bits, windows, buckets per window (2^(c-1))
@@ -37,7 +36,6 @@ struct MsmPlan {
   uint32_t merged;        // 1: bases carry precomputed 2^(c*w) multiples, all windows share ONE bucket set
   uint32_t Wr;            // bucket sets to reduce: W, or 1 when merged
   uint32_t table_stride;  // merged: bases of window w start at w * table_stride
-  uint32_t adaptive;      // 1: warp aggregation of the sort's atomics only when the warp shows skew (see warp_group)
 };
 
 // window for a precomputed table (all windows share the buckets, so c can be larger: fewer windows)
@@ -66,15 +64,9 @@ static MsmPlan make_plan(size_t n, uint32_t forced_c, uint32_t scalar_bits = 255
   p.c = c;
   p.W = (scalar_bits + c - 1) / c;
   p.B = 1u << (c - 1);
-  static int chunk_knob = -1;  // experiment knob B200ZK_CHUNK=8|16|32|64: buckets per running-sum chunk
-  if (chunk_knob < 0) { const char* e = getenv("B200ZK_CHUNK"); chunk_knob = e ? atoi(e) : 0; if (chunk_knob & (chunk_knob - 1)) chunk_knob = 0; }
-  const uint32_t want_chunk = chunk_knob > 0 ? (uint32_t)chunk_knob : (uint32_t)kChunk;
-  p.chunk = p.B < want_chunk ? p.B : want_chunk;
+  p.chunk = p.B < (uint32_t)kChunk ? p.B : (uint32_t)kChunk;
   p.T = p.B / p.chunk;
   p.merged = 0; p.Wr = p.W; p.table_stride = 0;
-  static int adaptive = -1;
-  if (adaptive < 0) { const char* e = getenv("B200ZK_SORT_MATCH"); adaptive = (e && *e == '1') ? 0 : 1; }  // =1: always MATCH (experiment knob)
-  p.adaptive = (uint32_t)adaptive;
   return p;
 }
 
@@ -131,21 +123,19 @@ static constexpr uint32_t kNoDigit = 0xffffffffu;
 
 // One atomic per distinct key per warp: hot buckets (top window, scalars 0/1/small) would otherwise serialise
 // 32 atomics on one L2 address.  Returns the warp-wide count of `key` and this lane's rank within its group.
-// MATCH costs about as many address-divergence-unit cycles as the divergent atomic it saves, so it only runs when the warp shows skew: `adaptive` first counts the
+// MATCH costs about as many address-divergence-unit cycles as the divergent atomic it saves, so it only runs when the warp shows skew: first count the
 // lanes that carry the first active lane's key (one SHFL + one VOTE); fewer than kSkewLanes of them and every lane
 // simply is its own group.  Uniform digits (the prover's case) take the cheap path, a hot bucket the exact one.
 static constexpr uint32_t kSkewLanes = 3;
-B2_D uint32_t warp_group(uint32_t key, bool active, uint32_t* rank, uint32_t* group_mask, bool adaptive) {
-  if (adaptive) {
-    const uint32_t full = __activemask();
-    const uint32_t act = __ballot_sync(full, active);
-    const uint32_t k0 = __shfl_sync(full, key, act ? __ffs(act) - 1 : 0);
-    const uint32_t m0 = __ballot_sync(full, active && key == k0);
-    if (__popc(m0) < kSkewLanes) {
-      *rank = 0;
-      *group_mask = 1u << (threadIdx.x & 31);
-      return 1;
-    }
+B2_D uint32_t warp_group(uint32_t key, bool active, uint32_t* rank, uint32_t* group_mask) {
+  const uint32_t full = __activemask();
+  const uint32_t act = __ballot_sync(full, active);
+  const uint32_t k0 = __shfl_sync(full, key, act ? __ffs(act) - 1 : 0);
+  const uint32_t m0 = __ballot_sync(full, active && key == k0);
+  if (__popc(m0) < kSkewLanes) {
+    *rank = 0;
+    *group_mask = 1u << (threadIdx.x & 31);
+    return 1;
   }
   uint32_t mask = __match_any_sync(__activemask(), active ? key : kNoDigit);
   uint32_t lane = threadIdx.x & 31;
@@ -188,7 +178,7 @@ __global__ void __launch_bounds__(kHistTile) msm_hist(const void* scalars, size_
       uint32_t code = mag ? ((mag - 1) | neg) : kNoDigit;
       if (live) digits[(size_t)w * n + i] = code;
       uint32_t rank, gm;
-      uint32_t cnt = warp_group(mag - 1, live && mag != 0, &rank, &gm, pl.adaptive != 0);
+      uint32_t cnt = warp_group(mag - 1, live && mag != 0, &rank, &gm);
       if (live && mag && rank == 0) atomicAdd(&hist[(pl.merged ? 0 : (size_t)w * pl.B) + (mag - 1)], cnt);
     }
     __syncthreads();  // everyone is done with tile[buf] before it is refilled two iterations later
@@ -221,7 +211,7 @@ __global__ void __launch_bounds__(256) msm_scatter(const uint32_t* __restrict__ 
     for (int u = 0; u < kScatterIlp; ++u) {
       base[u] = 0; rank[u] = 0; mask[u] = 0;
       if (live[u]) {
-        uint32_t cnt = warp_group(g[u], active[u], &rank[u], &mask[u], pl.adaptive != 0);
+        uint32_t cnt = warp_group(g[u], active[u], &rank[u], &mask[u]);
         if (active[u] && rank[u] == 0) base[u] = atomicAdd(&cursor[g[u]], cnt);
       }
     }
@@ -673,8 +663,8 @@ B2_D uint32_t bucket_of(const uint32_t* __restrict__ offsets, uint32_t G, uint32
 
 // DIRECT: `points` is already the sorted, sign-applied entry array (output of pair_sum); else entries are
 // idx[e] = base index | sign << 31 into the bases / window table.
-template <class F, bool DIRECT, int MINB = 1>
-__global__ void __launch_bounds__(128, MINB) msm_accumulate(const void* __restrict__ points, const uint32_t* __restrict__ idx,
+template <class F, bool DIRECT>
+__global__ void __launch_bounds__(128, 1) msm_accumulate(const void* __restrict__ points, const uint32_t* __restrict__ idx,
                                                       const uint32_t* __restrict__ offsets, const uint32_t* __restrict__ run_off,
                                                       uint32_t G, uint32_t kSegLen, void* __restrict__ partials, uint32_t* __restrict__ run_bucket) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -813,9 +803,11 @@ B2_D void pair_add_mixed(const PairLane& L, XYZZHalf& acc, const Fq& x2, const F
   acc.zzz = L.mul(acc.zzz, pzzz, PPP, pPPP);
 }
 
-// one thread PAIR per slice of kSegLen sorted entries; blockDim.x threads = blockDim.x / 2 slices
-template <int MINB>
-__global__ void __launch_bounds__(128, MINB) msm_accumulate_g2_pair(const void* __restrict__ points, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ offsets,
+// One thread PAIR per slice of kSegLen sorted entries; blockDim.x threads = blockDim.x / 2 slices.  Compiled for
+// kG2PairBlocks CTAs per SM: 154 registers, no spills.  At 4 CTAs per SM (128 registers, spills) a G2 MSM at 2^24 on an
+// H100 SXM at a 400 W power limit took 138.6-143.8 ms against 134.8 ms at 3 (median step, two alternating runs each).
+static constexpr unsigned kG2PairBlocks = 3;
+__global__ void __launch_bounds__(128, kG2PairBlocks) msm_accumulate_g2_pair(const void* __restrict__ points, const uint32_t* __restrict__ idx, const uint32_t* __restrict__ offsets,
                                                                 const uint32_t* __restrict__ run_off, uint32_t G, uint32_t kSegLen, void* __restrict__ partials,
                                                                 uint32_t* __restrict__ run_bucket) {
   const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1386,56 +1378,60 @@ static inline void phase_mark(b200zk_ctx* ctx, int k, cudaStream_t st) {
   if (ctx->profiling) cudaEventRecord(ctx->ev[k], st);
 }
 
-// ---- accumulation launch: G1 one thread per slice; G2 one lane PAIR per slice (msm_accumulate_g2_pair) unless the knob says otherwise
-static int g2_pair_knob() {
-  // experiment knob B200ZK_G2_PAIR=0: the one-thread-per-slice G2 kernel; 3 | 4: CTAs per SM the lane-pair kernel is
-  // compiled for (154 registers, no spills | 128 registers, spills).  Default 3: a G2 MSM at 2^24 on an H100 SXM at a
-  // 400 W power limit takes 134.8 | 138.6-143.8 ms (median step, two alternating runs each)
-  static int k = -1;
-  if (k < 0) { const char* e = getenv("B200ZK_G2_PAIR"); k = (e && (*e == '0' || *e == '3' || *e == '4')) ? (*e - '0') : 3; }
-  return k;
-}
+// threads of one accumulation wave: G1 one thread per slice, G2 one lane PAIR per slice (msm_accumulate_g2_pair)
 template <class F> static size_t resident_slices(const b200zk_ctx* ctx) {
-  if (IsFq2<F>::value) { const int k = g2_pair_knob(); return (size_t)ctx->sm_count * (k ? 64u * (unsigned)k : 256u); }
+  if (IsFq2<F>::value) return (size_t)ctx->sm_count * 64u * kG2PairBlocks;
   return (size_t)ctx->sm_count * (sizeof(F) > 32 ? 256u : 512u);
 }
 template <class F>
 static int launch_accumulate(b200zk_ctx* ctx, cudaStream_t st, const void* pts, const uint32_t* idx, const uint32_t* offsets, const uint32_t* run_off, uint32_t G, uint32_t L,
                              size_t slices, void* partials, uint32_t* run_bucket) {
-  const unsigned agrid = (unsigned)((slices + 127) / 128);
-  if constexpr (IsFq2<F>::value) {
-    const int k = g2_pair_knob();
-    const unsigned pgrid = (unsigned)((2 * slices + 127) / 128);
-    if (k == 3) B2_LAUNCH(ctx, msm_accumulate_g2_pair<3>, pgrid, 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
-    else if (k == 4) B2_LAUNCH(ctx, msm_accumulate_g2_pair<4>, pgrid, 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
-    else B2_LAUNCH(ctx, (msm_accumulate<F, false, 1>), agrid, 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
-  } else {
-    B2_LAUNCH(ctx, (msm_accumulate<F, false>), agrid, 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
-  }
+  if constexpr (IsFq2<F>::value)
+    B2_LAUNCH(ctx, msm_accumulate_g2_pair, (unsigned)((2 * slices + 127) / 128), 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
+  else
+    B2_LAUNCH(ctx, (msm_accumulate<F, false>), (unsigned)((slices + 127) / 128), 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
   return B200ZK_OK;
 }
 
-// two-level sort of the (window,bucket) entries of n scalars: hist[G], offsets[G+1] and idx[M] come out exactly as the
-// legacy msm_hist / scan / msm_scatter sequence leaves them.  ent1: W*n 8-byte scratch (value | fine key), ctab: 2*(C*NC+1) u32.
-static int legacy_sort_knob() {
-  static int knob = -1;  // experiment knob B200ZK_SORT=legacy: the r1 sort (one global atomic per entry and phase)
-  if (knob < 0) { const char* e = getenv("B200ZK_SORT"); knob = (e && !strcmp(e, "legacy")) ? 1 : 0; }
-  return knob;
+// exclusive scan of G values (scan_value: counts, or run flags when seg > 0) into out[0..G]; cursor, if given, receives
+// out[0..G) as well.  tsum: one word per kScanTile values.
+static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t shift, uint32_t* tsum,
+                          uint32_t* out, uint32_t* cursor = nullptr) {
+  const size_t tiles = (G + kScanTile - 1) / kScanTile;
+  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, shift, tsum);
+  B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
+  B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, shift, (const uint32_t*)tsum, out, cursor);
+  return B200ZK_OK;
 }
-// growth ratio of the host-scalar pipeline's chunk sizes (B200ZK_CHUNK_RATIO, read per call: 1 = equal chunks)
-static double chunk_ratio_knob(double dflt) {
-  const char* e = getenv("B200ZK_CHUNK_RATIO");
-  double r = (e && *e) ? atof(e) : dflt;
-  return (r >= 1.0 && r <= 64.0) ? r : dflt;
-}
+
 // scratch sizes of the two-level sort for up to M_max entries
 static size_t sort_ctab_bytes(int sm_count) { return (2 * ((size_t)kSortMaxBins * (size_t)sm_count + 1) + kSortMaxBins + 1) * 4; }
 static size_t sort_cnt2_bytes(size_t M_max) { return (M_max / kFineSeg + kSortMaxBins + 1) * (size_t)kSortMaxFine * 4; }
-static int run_two_level_sort(b200zk_ctx* ctx, const void* d_scalars, size_t n, uint32_t flags, const MsmPlan& pl, const SortPlan& sp, uint32_t* hist, uint32_t* offsets,
-                              uint32_t* tsum, uint2* ent1, uint32_t* ctab, uint32_t* cnt2, uint32_t* idx, cudaStream_t st, bool mark) {
-  const size_t Gc = (size_t)sp.C * sp.NC, tilesC = (Gc + kScanTile - 1) / kScanTile;
-  const size_t G = sp.G, tilesG = (G + kScanTile - 1) / kScanTile;
-  uint32_t *cnt = ctab, *base = ctab + Gc + 1, *item_start = base + Gc + 1;
+
+// Digit sort of n scalars into ctx->sort: hist[G] = entries per (window,bucket), offsets[G+1] = their exclusive scan,
+// idx[M] = the entries in bucket order.  The two-level sort wherever make_sort_plan accepts the size and plan (it leaves
+// hist, offsets and idx exactly as the one-pass sort does), the one-pass msm_hist / scan / msm_scatter everywhere else.
+// msm_run has sized the workspace for the sort that runs.
+static int sort_digits(b200zk_ctx* ctx, const void* d_scalars, size_t n, uint32_t flags, const MsmPlan& pl, cudaStream_t st) {
+  SortWorkspace& s = ctx->sort;
+  const size_t G = (size_t)pl.Wr * pl.B;
+  uint32_t *hist = (uint32_t*)s.hist.p, *offsets = (uint32_t*)s.offsets.p, *tsum = (uint32_t*)s.tsum.p, *idx = (uint32_t*)s.idx.p;
+  SortPlan sp;
+  if (!make_sort_plan(n, pl, ctx->sm_count, &sp)) {
+    B2_CUDA(ctx, cudaMemsetAsync(hist, 0, G * 4, st));
+    const unsigned sgrid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8);
+    B2_LAUNCH(ctx, msm_hist, sgrid, 256, 0, st, d_scalars, n, flags, pl, hist, (uint32_t*)s.digits.p);
+    phase_mark(ctx, 1, st);
+    B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, 0, tsum, offsets, (uint32_t*)s.cursor.p));
+    phase_mark(ctx, 2, st);
+    const unsigned wgrid = (unsigned)std::min<size_t>((n * (size_t)pl.W + 255) / 256, (size_t)ctx->sm_count * 32);
+    B2_LAUNCH(ctx, msm_scatter, wgrid, 256, 0, st, (const uint32_t*)s.digits.p, n, pl, (uint32_t*)s.cursor.p, idx);
+    return B200ZK_OK;
+  }
+  // two-level: ent1 = W*n 8-byte scratch (value | fine key); ctab = cnt[C*NC+1], base[C*NC+1], item_start
+  const size_t Gc = (size_t)sp.C * sp.NC;
+  uint32_t *cnt = (uint32_t*)s.ctab.p, *base = cnt + Gc + 1, *item_start = base + Gc + 1, *cnt2 = (uint32_t*)s.cnt2.p;
+  uint2* ent1 = (uint2*)s.key.p;
   if (!ctx->attr_sort) {
     B2_CUDA(ctx, cudaFuncSetAttribute(msm_sort_coarse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SortCoarseSmem)));
     B2_CUDA(ctx, cudaFuncSetAttribute(msm_sort_fine_place, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SortFineSmem)));
@@ -1443,11 +1439,9 @@ static int run_two_level_sort(b200zk_ctx* ctx, const void* d_scalars, size_t n, 
   }
   B2_CUDA(ctx, cudaMemsetAsync(cnt, 0, (Gc + 1) * 4, st));
   B2_LAUNCH(ctx, msm_sort_count, sp.NC * kSortCountSub, kHistTile, 0, st, d_scalars, n, flags, pl, sp, cnt);
-  if (mark) phase_mark(ctx, 1, st);
-  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tilesC, kScanThreads, 0, st, (const uint32_t*)cnt, (const uint32_t*)nullptr, Gc, 0u, 0u, tsum);
-  B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tilesC);
-  B2_LAUNCH(ctx, scan_apply, (unsigned)tilesC, kScanThreads, 0, st, (const uint32_t*)cnt, (const uint32_t*)nullptr, Gc, 0u, 0u, (const uint32_t*)tsum, base, (uint32_t*)nullptr);
-  if (mark) phase_mark(ctx, 2, st);
+  phase_mark(ctx, 1, st);
+  B2_TRY(exclusive_scan(ctx, st, cnt, nullptr, Gc, 0, 0, tsum, base));
+  phase_mark(ctx, 2, st);
   B2_LAUNCH(ctx, msm_sort_coarse, sp.NC, kSortTile, sizeof(SortCoarseSmem), st, d_scalars, n, flags, pl, sp, (const uint32_t*)base, ent1);
   // fine pass over segments of kFineSeg entries: at most M / kFineSeg + C items (the grid is this bound; surplus CTAs exit)
   const unsigned max_items = (unsigned)((n * (size_t)pl.W) / kFineSeg + sp.C + 1);
@@ -1455,310 +1449,30 @@ static int run_two_level_sort(b200zk_ctx* ctx, const void* d_scalars, size_t n, 
   B2_LAUNCH(ctx, msm_sort_items, 1, 1024, 0, st, (const uint32_t*)base, sp, item_start);
   B2_LAUNCH(ctx, msm_sort_fine_count, max_items, 1024, 0, st, (const uint2*)ent1, sp, (const uint32_t*)base, (const uint32_t*)item_start, cnt2);
   B2_LAUNCH(ctx, msm_sort_fine_prefix, (unsigned)(((size_t)sp.C * F + 255) / 256), 256, 0, st, sp, (const uint32_t*)item_start, cnt2, hist);
-  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tilesG, kScanThreads, 0, st, (const uint32_t*)hist, (const uint32_t*)nullptr, G, 0u, 0u, tsum);
-  B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tilesG);
-  B2_LAUNCH(ctx, scan_apply, (unsigned)tilesG, kScanThreads, 0, st, (const uint32_t*)hist, (const uint32_t*)nullptr, G, 0u, 0u, (const uint32_t*)tsum, offsets, (uint32_t*)nullptr);
+  B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, 0, tsum, offsets));
   B2_LAUNCH(ctx, msm_sort_fine_place, max_items, 1024, sizeof(SortFineSmem), st, (const uint2*)ent1, sp, (const uint32_t*)base, (const uint32_t*)item_start, (const uint32_t*)cnt2,
             (const uint32_t*)offsets, idx);
   return B200ZK_OK;
 }
 
-// ---- chunk-pipelined schedule --------------------------------------------------------------------------------
-// Host scalars arrive over PCIe (512 MiB at 2^24, a sizeable fraction of the MSM's time).  The points are cut into K chunks;
-// chunk k's scalars are uploaded on a second stream while earlier chunks are being sorted and accumulated, so that only
-// the FIRST chunk's upload is exposed.  r1 also ran the sort of chunk k+1 concurrently with the accumulation of chunk k
-// (second stream, a shared-memory reservation to keep room on the SMs); with the r2 two-level sort -- whose CTAs want a
-// whole SM -- all kernels run on ONE stream in the order sort(0), accumulate(0), sort(1), ...: every kernel has the
-// machine to itself and the copy engine works underneath, one chunk ahead.  Each chunk's bucket totals are folded into a dense totals array, which is reduced once at the end.
+// Folds the runs of every bucket with more than kDirectRuns of them into its first run.  Worst case every one of
+// `entries` lands in one bucket: ceil(entries / L) + 1 runs to fold.
 template <class F>
-static int msm_run_pipelined(b200zk_ctx* ctx, const void* d_points, const void* d_scalars, const void* h_scalars, size_t n, uint32_t flags,
-                             cudaStream_t st, void* d_partial, const MsmPlan& pl, uint32_t K) {
-  const size_t G = (size_t)pl.Wr * pl.B;
-  const size_t tiles = (G + kScanTile - 1) / kScanTile;
-  const size_t xy = 4 * FieldBytes<F>::value, pt = 2 * FieldBytes<F>::value;
-  // Chunk k covers points [bnd[k], bnd[k+1]).  With HOST scalars the sizes grow geometrically (ratio r): only the first
-  // chunk's upload is exposed, and chunk k+1 uploads while chunk k computes -- the kernels are ~3.7x slower per point than
-  // the PCIe copy, so a chunk may be ~3x its predecessor and still arrive in time.  Fewer, larger chunks also pay the
-  // per-chunk costs (sort launches, wave tails, bucket_merge over all G buckets) fewer times.  Resident scalars: equal chunks.
-  size_t bnd[kMaxPipelineChunks + 1];
-  uint32_t chunks = 0;
-  {
-    // G1 3 chunks x4, G2 2 chunks x12 (tools/e2e_sweep.py sweeps them): the ratio tracks compute time / copy time
-    const double r = h_scalars ? chunk_ratio_knob(IsFq2<F>::value ? 12.0 : 4.0) : 1.0;
-    double tot = 0, w = 1;
-    for (uint32_t k = 0; k < K; ++k) { tot += w; w *= r; }
-    double cum = 0; w = 1;
-    bnd[0] = 0;
-    for (uint32_t k = 0; k < K; ++k) {
-      cum += w; w *= r;
-      size_t hi = (k == K - 1) ? n : std::min(n, (((size_t)((double)n * (cum / tot))) + 1023) & ~(size_t)1023);
-      if (hi > bnd[chunks]) bnd[++chunks] = hi;  // empty chunks (tiny n) vanish
-    }
-  }
-  size_t chunk = 0;  // the largest chunk sizes the workspaces
-  for (uint32_t k = 0; k < chunks; ++k) chunk = std::max(chunk, bnd[k + 1] - bnd[k]);
-  const size_t Mk_max = chunk * pl.W;
-  const size_t resident = resident_slices<F>(ctx);
-  uint32_t Lk[kMaxPipelineChunks];  // slice length per chunk: each fills whole waves of resident threads
-  size_t S_max = 0;
-  for (uint32_t k = 0; k < chunks; ++k) {
-    const size_t Mk = (bnd[k + 1] - bnd[k]) * pl.W;
-    Lk[k] = pick_slice_len(Mk, resident);
-    S_max = std::max(S_max, Mk / Lk[k] + 1 + G);
-  }
-  SortPlan sp0;
-  const bool two_level = !legacy_sort_knob() && make_sort_plan(chunk, pl, ctx->sm_count, &sp0);
-  const size_t Gc = (size_t)kSortMaxBins * (size_t)ctx->sm_count;  // upper bound of C * NC for any chunk
-  for (int sl = 0; sl < 2; ++sl) {
-    SortSlot& s = ctx->slot[sl];
-    B2_TRY(ensure(ctx, s.hist, G * 4)); B2_TRY(ensure(ctx, s.offsets, (G + 1) * 4)); B2_TRY(ensure(ctx, s.cursor, G * 4));
-    B2_TRY(ensure(ctx, s.run_off, (G + 1) * 4));
-    B2_TRY(ensure(ctx, s.tsum, std::max(tiles, (Gc + kScanTile - 1) / kScanTile) * 4));
-    B2_TRY(ensure(ctx, s.digits, Mk_max * 4)); B2_TRY(ensure(ctx, s.idx, Mk_max * 4));
-    if (two_level) { B2_TRY(ensure(ctx, s.key, Mk_max * 8)); B2_TRY(ensure(ctx, s.ctab, sort_ctab_bytes(ctx->sm_count))); B2_TRY(ensure(ctx, s.cnt2, sort_cnt2_bytes(Mk_max))); }
-  }
-  B2_TRY(ensure(ctx, ctx->ws_buckets, S_max * xy));
-  B2_TRY(ensure(ctx, ctx->ws_segbucket, S_max * 4));
-  B2_TRY(ensure(ctx, ctx->ws_totals, G * xy));
-  B2_TRY(ensure(ctx, ctx->ws_chunkS, (size_t)pl.Wr * pl.T * xy));
-  B2_TRY(ensure(ctx, ctx->ws_chunkV, (size_t)pl.Wr * pl.T * xy));
-  if (h_scalars) B2_TRY(ensure(ctx, ctx->ws_scalars, n * 32 + 32));
-  const uint8_t* dsc = (const uint8_t*)(h_scalars ? ctx->ws_scalars.p : d_scalars);
-  cudaStream_t cs = ctx->stream_sort;  // the copy stream: uploads only
-  // uploads: all issued up front on the copy stream (they serialise on the one H2D engine in chunk order); the staging
-  // buffer may still be read by the previous call's kernels on `st`, so the copy stream first waits for `st`
-  if (h_scalars) {
-    B2_CUDA(ctx, cudaEventRecord(ctx->ev_in, st));
-    B2_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->ev_in, 0));
-    if (chunks > kMaxPipelineChunks) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm: too many pipeline chunks");
-    for (uint32_t k = 0; k < chunks; ++k) {
-      const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
-      B2_CUDA(ctx, cudaMemcpyAsync((void*)(dsc + lo * 32), (const uint8_t*)h_scalars + lo * 32, nk * 32, cudaMemcpyHostToDevice, cs));
-      B2_CUDA(ctx, cudaEventRecord(ctx->ev_up[k], cs));
-    }
-  }
-  auto sort_chunk = [&](uint32_t k) -> int {
-    const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
-    const uint32_t L = Lk[k];
-    SortSlot& s = ctx->slot[k & 1];
-    uint32_t *hist = (uint32_t*)s.hist.p, *offsets = (uint32_t*)s.offsets.p, *cursor = (uint32_t*)s.cursor.p, *run_off = (uint32_t*)s.run_off.p,
-             *tsum = (uint32_t*)s.tsum.p, *digits = (uint32_t*)s.digits.p, *idx = (uint32_t*)s.idx.p;
-    if (h_scalars) B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_up[k], 0));
-    SortPlan sp;
-    const bool tl = two_level && make_sort_plan(nk, pl, ctx->sm_count, &sp);
-    if (tl) {
-      B2_TRY(run_two_level_sort(ctx, (const void*)(dsc + lo * 32), nk, flags, pl, sp, hist, offsets, tsum, (uint2*)s.key.p, (uint32_t*)s.ctab.p, (uint32_t*)s.cnt2.p, idx, st, false));
-    } else {
-      B2_CUDA(ctx, cudaMemsetAsync(hist, 0, G * 4, st));
-      const unsigned sgrid = (unsigned)std::min<size_t>((nk + 255) / 256, (size_t)ctx->sm_count * 8);
-      B2_LAUNCH(ctx, msm_hist, sgrid, 256, 0, st, (const void*)(dsc + lo * 32), nk, flags, pl, hist, digits);
-      B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, 0u, tsum);
-      B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-      B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, 0u, tsum, offsets, cursor);
-      const unsigned wgrid = (unsigned)std::min<size_t>((nk * (size_t)pl.W + 255) / 256, (size_t)ctx->sm_count * 32);
-      B2_LAUNCH(ctx, msm_scatter, wgrid, 256, 0, st, (const uint32_t*)digits, nk, pl, cursor, idx);
-    }
-    B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)offsets, G, L, 0u, tsum);
-    B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-    B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)offsets, G, L, 0u, tsum, run_off, (uint32_t*)nullptr);
-    return B200ZK_OK;
-  };
-  for (uint32_t k = 0; k < chunks; ++k) {
-    const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
-    const uint32_t L = Lk[k];
-    const size_t slices = (nk * pl.W + L - 1) / L;
-    // sort(k) waits for upload k only: with the kernels serialised there is nothing to gain from sorting ahead, and
-    // sort(k+1) before accumulate(k) would stall the stream on upload k+1
-    B2_TRY(sort_chunk(k));
-    SortSlot& s = ctx->slot[k & 1];
-    const void* pts = (const uint8_t*)d_points + lo * pt;
-    B2_TRY(launch_accumulate<F>(ctx, st, pts, (const uint32_t*)s.idx.p, (const uint32_t*)s.offsets.p, (const uint32_t*)s.run_off.p, (uint32_t)G, L, slices, ctx->ws_buckets.p,
-                                (uint32_t*)ctx->ws_segbucket.p));
-    {
-      size_t worst_entries = (pl.merged ? nk * (size_t)pl.W : nk) + 1;
-      size_t worst = (worst_entries + L - 1) / L + 1;
-      for (size_t stride = 1; stride < worst; stride *= kTreeRadix)
-        B2_LAUNCH(ctx, partial_tree<F>, (unsigned)((S_max + 127) / 128), 128, 0, st, (const uint32_t*)s.run_off.p, (const uint32_t*)ctx->ws_segbucket.p, (uint32_t)G, (uint32_t)stride, ctx->ws_buckets.p);
-    }
-    B2_LAUNCH(ctx, bucket_merge<F>, (unsigned)((G + 127) / 128), 128, 0, st, (const void*)ctx->ws_buckets.p, (const uint32_t*)s.run_off.p, (uint32_t)G, k == 0 ? 1 : 0, ctx->ws_totals.p);
-  }
-  const size_t nchunks = (size_t)pl.Wr * pl.T;
-  B2_LAUNCH(ctx, bucket_chunk<F>, (unsigned)((nchunks + 127) / 128), 128, 0, st, (const void*)ctx->ws_totals.p, (const uint32_t*)nullptr, pl, ctx->ws_chunkS.p, ctx->ws_chunkV.p);
-  uint32_t chunk_log2 = 0;
-  while ((1u << chunk_log2) < pl.chunk) ++chunk_log2;
-  if (pl.T >= 64) {
-    uint32_t nbits = 0;
-    while ((1u << nbits) < pl.T) ++nbits;
-    B2_TRY(ensure(ctx, ctx->ws_bitpart, (size_t)pl.Wr * (nbits + 1) * kBitParts * xy));
-    B2_LAUNCH(ctx, bucket_bitsums<F>, dim3(nbits + 1, pl.Wr, kBitParts), kBitThreads, 0, st, pl, nbits, (const void*)ctx->ws_chunkS.p, (const void*)ctx->ws_chunkV.p, ctx->ws_bitpart.p);
-    B2_LAUNCH(ctx, bucket_bitfinal<F>, pl.Wr, 32, 0, st, pl, nbits, chunk_log2, (const void*)ctx->ws_bitpart.p, ctx->ws_chunkV.p);
-  } else {
-    for (uint32_t half = 1, lvl = 0; half < pl.T; half <<= 1, ++lvl) {
-      size_t pairs = (size_t)pl.Wr * (pl.T / (2 * half));
-      B2_LAUNCH(ctx, bucket_tree<F>, (unsigned)((pairs + 127) / 128), 128, 0, st, pl, half, lvl + chunk_log2, ctx->ws_chunkS.p, ctx->ws_chunkV.p);
-    }
-  }
-  B2_LAUNCH(ctx, msm_horner<F>, 1, 32, 0, st, pl, ctx->ws_chunkV.p, d_partial);
+static int fold_runs(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* run_off, const uint32_t* run_bucket, uint32_t G, size_t entries, uint32_t L, size_t S_max, void* partials) {
+  const size_t worst = (entries + 1 + L - 1) / L + 1;
+  for (size_t stride = 1; stride < worst; stride *= kTreeRadix)
+    B2_LAUNCH(ctx, partial_tree<F>, (unsigned)((S_max + 127) / 128), 128, 0, st, run_off, run_bucket, G, (uint32_t)stride, partials);
   return B200ZK_OK;
 }
 
+// Bucket reduction and Horner: d_partial = sum_w 2^(c*w) sum_b (b+1) * B[w][b], from the dense totals in ws_totals
+// (run_off == nullptr) or from the runs in ws_buckets that run_off numbers.
 template <class F>
-static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars, size_t n, uint32_t flags, cudaStream_t st, void* d_partial,
-                   uint32_t table_c, size_t table_stride, const void* h_scalars, int sort_mode) {
-  NvtxRange nvtx_msm(IsFq2<F>::value ? "b200zk:g2_msm" : (sizeof(F) > 32 ? "b200zk:bls12_381_g1_msm" : "b200zk:g1_msm"));
-  // sort_mode (b200zk_msm_multi_resident_device): 0 = ordinary call; 1 = one-shot schedule, the digit sort stays in
-  // the workspaces; 2 = the sort of the previous call (same scalars, same plan) is reused: only the point-dependent
-  // half of the MSM runs (run scan, accumulation, bucket reduction)
-  if (n == 0) {
-    B2_LAUNCH(ctx, write_identity<F>, 1, 32, 0, st, d_partial);
-    return B200ZK_OK;
-  }
-  if (n >= ((size_t)1 << 31)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: n must be < 2^31");
-  // 128-bit loads and the bulk copies of the scalar tiles need 16-byte aligned device buffers
-  if (((uintptr_t)d_points & 15) || ((uintptr_t)d_scalars & 15)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm: device buffers must be 16-byte aligned");
-  MsmPlan pl = make_plan(n, table_c ? table_c : ctx->msm_window, ScalarBits<F>::value);
-  if (table_c) {
-    pl.merged = 1; pl.Wr = 1; pl.table_stride = (uint32_t)table_stride;
-    if ((unsigned long long)table_stride * pl.W >= (1ull << 31)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: precomputed table too large for 31-bit indices");
-  }
-  if ((unsigned long long)n * pl.W >= (1ull << 32)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: n * windows must be < 2^32 (shard the MSM)");
-  {
-    // large inputs: chunk-pipelined schedule (unless phases are being profiled or pair rounds are forced)
-    // with scalars already in HBM one shot: the accumulation fills the SMs, so a next chunk's sort would barely overlap;
-    // with HOST scalars the chunks hide most of the 512 MiB upload at 2^24
-    // chunks of the host-scalar pipeline: few and geometrically growing (msm_run_pipelined)
-    static int k_knob = -1;  // experiment knob B200ZK_E2E_CHUNKS: default chunk count of the host-scalar pipeline
-    if (k_knob < 0) { const char* e = getenv("B200ZK_E2E_CHUNKS"); k_knob = (e && *e) ? atoi(e) : 0; if (k_knob < 0 || k_knob > 64) k_knob = 0; }
-    uint32_t K = ctx->msm_chunks ? ctx->msm_chunks : ((h_scalars && n >= ((size_t)1 << 22)) ? (k_knob ? (uint32_t)k_knob : (IsFq2<F>::value ? 2u : 3u)) : 1u);
-    if (K > 64) K = 64;
-    if (sort_mode == 0 && (K > 1 || h_scalars) && !ctx->profiling && ctx->msm_pair_rounds <= 0 && n >= 4096)
-      return msm_run_pipelined<F>(ctx, d_points, d_scalars, h_scalars, n, flags, st, d_partial, pl, K);
-  }
-  if (h_scalars) {  // unpipelined path takes device scalars: stage them first
-    B2_TRY(ensure(ctx, ctx->ws_scalars, n * 32 + 32));
-    B2_CUDA(ctx, cudaMemcpyAsync(ctx->ws_scalars.p, h_scalars, n * 32, cudaMemcpyHostToDevice, st));
-    d_scalars = ctx->ws_scalars.p;
-  }
-  const size_t G = (size_t)pl.Wr * pl.B;
-  const size_t tiles = (G + kScanTile - 1) / kScanTile;
+static int reduce_buckets(b200zk_ctx* ctx, cudaStream_t st, const MsmPlan& pl, const uint32_t* run_off, void* d_partial) {
   const size_t xy = 4 * FieldBytes<F>::value;
-  static int dense_knob = -1;  // experiment knob, see the bucket reduction below
-  if (dense_knob < 0) { const char* e = getenv("B200ZK_DENSE_TOTALS"); dense_knob = (e && *e == '0') ? 0 : 1; }
-  const bool dense_totals = dense_knob && G >= ((size_t)1 << 14);
-  if (dense_totals) B2_TRY(ensure(ctx, ctx->ws_totals, G * xy));
-  B2_TRY(ensure(ctx, ctx->ws_hist, G * 4));
-  B2_TRY(ensure(ctx, ctx->ws_offsets, (G + 1) * 4));
-  B2_TRY(ensure(ctx, ctx->ws_cursor, G * 4));
-  B2_TRY(ensure(ctx, ctx->ws_blocksums, tiles * 4));
-  B2_TRY(ensure(ctx, ctx->ws_idx, n * (size_t)pl.W * 4));
-  B2_TRY(ensure(ctx, ctx->ws_digits, n * (size_t)pl.W * 4));
-  const size_t M_max = n * (size_t)pl.W;
-  // pair-summing rounds.  A round is bound by its ~330 B of scattered memory traffic per pair, not by its 6.7
-  // products, and costs more than the XYZZ addition it removes, so the automatic setting is OFF; the path stays available (b200zk_set_msm_pair_rounds)
-  // for parts with a different compute:bandwidth balance and is covered by the parity tests.
-  uint32_t rounds = 0;
-  if (ctx->msm_pair_rounds >= 0) rounds = (uint32_t)ctx->msm_pair_rounds;
-  if (rounds > 4) rounds = 4;
-  if (rounds && M_max >= ((size_t)1 << 31)) rounds = 0;
-  if (sort_mode) rounds = 0;
-  const uint32_t kSegLen = pick_slice_len(M_max >> rounds, resident_slices<F>(ctx));
-  const size_t S_max = (M_max >> rounds) / kSegLen + 1 + G;  // upper bound on the number of runs
-  const size_t slices = ((M_max >> rounds) + G + kSegLen - 1) / kSegLen;
-  if (rounds) {
-    const size_t pt = 2 * FieldBytes<F>::value;
-    B2_TRY(ensure(ctx, ctx->ws_q1, (M_max / 2 + G + 1) * pt));
-    if (rounds > 1) B2_TRY(ensure(ctx, ctx->ws_q0, (M_max / 4 + G + 1) * pt));
-    B2_TRY(ensure(ctx, ctx->ws_prefix, (M_max / 2 + G + 1) * FieldBytes<F>::value));
-    B2_TRY(ensure(ctx, ctx->ws_info, (M_max / 2 + G + 1) * 4));
-    B2_TRY(ensure(ctx, ctx->ws_pairoff0, (G + 1) * 4));
-    B2_TRY(ensure(ctx, ctx->ws_pairoff1, (G + 1) * 4));
-  }
-  B2_TRY(ensure(ctx, ctx->ws_buckets, S_max * xy));     // segment partials (bucket totals after partial_tree)
-  B2_TRY(ensure(ctx, ctx->ws_segoff, (G + 1) * 4));
-  B2_TRY(ensure(ctx, ctx->ws_segbucket, S_max * 4));
-  B2_TRY(ensure(ctx, ctx->ws_chunkS, (size_t)pl.Wr * pl.T * xy));
-  B2_TRY(ensure(ctx, ctx->ws_chunkV, (size_t)pl.Wr * pl.T * xy));
-  uint32_t* hist = (uint32_t*)ctx->ws_hist.p;
-  uint32_t* offsets = (uint32_t*)ctx->ws_offsets.p;
-  uint32_t* cursor = (uint32_t*)ctx->ws_cursor.p;
-  uint32_t* tsum = (uint32_t*)ctx->ws_blocksums.p;
-  uint32_t* idx = (uint32_t*)ctx->ws_idx.p;
-
-  SortPlan sp;
-  const bool two_level = !legacy_sort_knob() && make_sort_plan(n, pl, ctx->sm_count, &sp);
-  if (two_level) {
-    B2_TRY(ensure(ctx, ctx->ws_key, M_max * 8));
-    B2_TRY(ensure(ctx, ctx->ws_ctab, sort_ctab_bytes(ctx->sm_count)));
-    B2_TRY(ensure(ctx, ctx->ws_cnt2, sort_cnt2_bytes(M_max)));
-    B2_TRY(ensure(ctx, ctx->ws_blocksums, (std::max(tiles, ((size_t)sp.C * sp.NC + kScanTile - 1) / kScanTile)) * 4));
-    tsum = (uint32_t*)ctx->ws_blocksums.p;
-  }
-  phase_mark(ctx, 0, st);
-  nvtxRangePushA("b200zk:msm_sort");
-  if (sort_mode != 2 && two_level) {
-    B2_TRY(run_two_level_sort(ctx, d_scalars, n, flags, pl, sp, hist, offsets, tsum, (uint2*)ctx->ws_key.p, (uint32_t*)ctx->ws_ctab.p, (uint32_t*)ctx->ws_cnt2.p, idx, st, true));
-  } else if (sort_mode != 2) {
-    B2_CUDA(ctx, cudaMemsetAsync(hist, 0, G * 4, st));
-    const unsigned sgrid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8);
-    uint32_t* digits = (uint32_t*)ctx->ws_digits.p;
-    B2_LAUNCH(ctx, msm_hist, sgrid, 256, 0, st, d_scalars, n, flags, pl, hist, digits);
-    phase_mark(ctx, 1, st);
-    B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, 0u, tsum);
-    B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-    B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, 0u, tsum, offsets, cursor);
-    phase_mark(ctx, 2, st);
-    const unsigned wgrid = (unsigned)std::min<size_t>((n * (size_t)pl.W + 255) / 256, (size_t)ctx->sm_count * 32);
-    B2_LAUNCH(ctx, msm_scatter, wgrid, 256, 0, st, (const uint32_t*)digits, n, pl, cursor, idx);
-  } else {
-    phase_mark(ctx, 1, st);
-    phase_mark(ctx, 2, st);
-  }
-  nvtxRangePop();
-  phase_mark(ctx, 3, st);
-  NvtxRange nvtx_acc("b200zk:msm_accumulate+reduce");
-  // batched-affine pair-summing rounds: each halves the entries the XYZZ accumulation has to fold
-  const uint32_t* cur_off = offsets;
-  const void* cur_pts = d_points;
-  for (uint32_t r = 1; r <= rounds; ++r) {
-    uint32_t* off_r = (uint32_t*)(r & 1 ? ctx->ws_pairoff1.p : ctx->ws_pairoff0.p);
-    B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, r, tsum);
-    B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-    B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, hist, (const uint32_t*)nullptr, G, 0u, r, tsum, off_r, (uint32_t*)nullptr);
-    const size_t out_max = (M_max >> r) + G;
-    void* q = (r & 1) ? ctx->ws_q1.p : ctx->ws_q0.p;
-    const unsigned pgrid = (unsigned)((out_max / kPairBatch + 1 + 127) / 128);
-    if (r == 1) B2_LAUNCH(ctx, (pair_sum<F, true>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)idx, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
-    else B2_LAUNCH(ctx, (pair_sum<F, false>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)idx, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
-    cur_off = off_r;
-    cur_pts = q;
-  }
-  uint32_t* seg_off = (uint32_t*)ctx->ws_segoff.p;
-  uint32_t* seg_bucket = (uint32_t*)ctx->ws_segbucket.p;
-  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, hist, cur_off, G, kSegLen, 0u, tsum);
-  B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-  B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, hist, cur_off, G, kSegLen, 0u, tsum, seg_off, (uint32_t*)nullptr);
-  if (rounds) B2_LAUNCH(ctx, (msm_accumulate<F, true>), (unsigned)((slices + 127) / 128), 128, 0, st, cur_pts, (const uint32_t*)idx, cur_off, (const uint32_t*)seg_off, (uint32_t)G, kSegLen, ctx->ws_buckets.p, seg_bucket);
-  else {
-    B2_TRY(launch_accumulate<F>(ctx, st, cur_pts, (const uint32_t*)idx, cur_off, (const uint32_t*)seg_off, (uint32_t)G, kSegLen, slices, ctx->ws_buckets.p, seg_bucket));
-  }
-  {
-    // worst case every point of a window lands in one bucket: ceil(entries / kSegLen) + 1 runs to fold
-    size_t worst_entries = ((pl.merged ? n * (size_t)pl.W : n) >> rounds) + 1;
-    size_t worst = (worst_entries + kSegLen - 1) / kSegLen + 1;
-    for (size_t stride = 1; stride < worst; stride *= kTreeRadix)
-      B2_LAUNCH(ctx, partial_tree<F>, (unsigned)((S_max + 127) / 128), 128, 0, st, seg_off, seg_bucket, (uint32_t)G, (uint32_t)stride, ctx->ws_buckets.p);
-  }
-  phase_mark(ctx, 4, st);
   const size_t chunks = (size_t)pl.Wr * pl.T;
-  // Bucket totals first, one thread per bucket (full occupancy, every lane busy), then the running sums over dense totals:
-  // bucket_chunk's threads are few (G / chunk) and serial, so every run addition moved out of them shortens the
-  // latency-bound tail (B200ZK_DENSE_TOTALS=0: the fused form, bucket_chunk summing the runs itself).
-  if (dense_totals) {
-    B2_LAUNCH(ctx, bucket_merge<F>, (unsigned)((G + 127) / 128), 128, 0, st, (const void*)ctx->ws_buckets.p, (const uint32_t*)seg_off, (uint32_t)G, 1, ctx->ws_totals.p);
-    B2_LAUNCH(ctx, bucket_chunk<F>, (unsigned)((chunks + 127) / 128), 128, 0, st, (const void*)ctx->ws_totals.p, (const uint32_t*)nullptr, pl, ctx->ws_chunkS.p, ctx->ws_chunkV.p);
-  } else {
-    B2_LAUNCH(ctx, bucket_chunk<F>, (unsigned)((chunks + 127) / 128), 128, 0, st, ctx->ws_buckets.p, seg_off, pl, ctx->ws_chunkS.p, ctx->ws_chunkV.p);
-  }
+  const void* totals = run_off ? ctx->ws_buckets.p : ctx->ws_totals.p;
+  B2_LAUNCH(ctx, bucket_chunk<F>, (unsigned)((chunks + 127) / 128), 128, 0, st, totals, run_off, pl, ctx->ws_chunkS.p, ctx->ws_chunkV.p);
   uint32_t chunk_log2 = 0;
   while ((1u << chunk_log2) < pl.chunk) ++chunk_log2;
   if (pl.T >= 64) {
@@ -1777,6 +1491,184 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
   B2_LAUNCH(ctx, msm_horner<F>, 1, 32, 0, st, pl, ctx->ws_chunkV.p, d_partial);
   phase_mark(ctx, 6, st);
   return B200ZK_OK;
+}
+
+// One schedule for every MSM: the points are cut into K >= 1 chunks, and each chunk is sorted, scanned, accumulated and
+// its bucket totals folded before the next; one bucket reduction and Horner close the call.
+// Host scalars arrive over PCIe (512 MiB at 2^24, a sizeable fraction of the MSM's time).  On the chunked path chunk k's
+// scalars upload on the copy stream (ctx->stream_upload) while earlier chunks compute, so that only the FIRST chunk's
+// upload is exposed.  Every kernel runs on the caller's stream in the order sort(0), accumulate(0), sort(1), ...: the
+// two-level sort's CTAs want whole SMs, so each kernel has the machine to itself and the copy engine works underneath,
+// one chunk ahead.  Profiled calls, pair-summing rounds, shared sorts (sort_mode 1 / 2) and tiny inputs run one chunk and
+// stage host scalars on the caller's stream.
+template <class F>
+static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars, size_t n, uint32_t flags, cudaStream_t st, void* d_partial,
+                   uint32_t table_c, size_t table_stride, const void* h_scalars, int sort_mode) {
+  NvtxRange nvtx_msm(IsFq2<F>::value ? "b200zk:g2_msm" : (sizeof(F) > 32 ? "b200zk:bls12_381_g1_msm" : "b200zk:g1_msm"));
+  // sort_mode (b200zk_msm_multi_resident_device, groth16_commit): 0 = ordinary call; 1 = one chunk, the digit sort stays in
+  // ctx->sort; 2 = the sort of the previous call (same scalars, same plan) is reused: only the point-dependent
+  // half of the MSM runs (run scan, accumulation, bucket reduction)
+  if (n == 0) {
+    B2_LAUNCH(ctx, write_identity<F>, 1, 32, 0, st, d_partial);
+    return B200ZK_OK;
+  }
+  if (n >= ((size_t)1 << 31)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: n must be < 2^31");
+  // 128-bit loads and the bulk copies of the scalar tiles need 16-byte aligned device buffers
+  if (((uintptr_t)d_points & 15) || ((uintptr_t)d_scalars & 15)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "msm: device buffers must be 16-byte aligned");
+  MsmPlan pl = make_plan(n, table_c ? table_c : ctx->msm_window, ScalarBits<F>::value);
+  if (table_c) {
+    pl.merged = 1; pl.Wr = 1; pl.table_stride = (uint32_t)table_stride;
+    if ((unsigned long long)table_stride * pl.W >= (1ull << 31)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: precomputed table too large for 31-bit indices");
+  }
+  if ((unsigned long long)n * pl.W >= (1ull << 32)) return fail(ctx, B200ZK_ERR_UNSUPPORTED, "msm: n * windows must be < 2^32 (shard the MSM)");
+  // with scalars already in HBM one chunk: the accumulation fills the SMs, so there is nothing to overlap; host scalars
+  // from 2^22 points up: G1 3 chunks, G2 2 (b200zk_set_msm_chunks overrides the count)
+  uint32_t K = ctx->msm_chunks ? ctx->msm_chunks : ((h_scalars && n >= ((size_t)1 << 22)) ? (IsFq2<F>::value ? 2u : 3u) : 1u);
+  if (K > kMaxPipelineChunks) K = kMaxPipelineChunks;
+  const bool chunked = sort_mode == 0 && (K > 1 || h_scalars) && !ctx->profiling && ctx->msm_pair_rounds <= 0 && n >= 4096;
+  if (!chunked) K = 1;
+  const size_t G = (size_t)pl.Wr * pl.B;
+  const size_t xy = 4 * FieldBytes<F>::value, pt = 2 * FieldBytes<F>::value;
+  // Chunk k covers points [bnd[k], bnd[k+1]).  With HOST scalars the sizes grow geometrically (ratio r): only the first
+  // chunk's upload is exposed, and chunk k+1 uploads while chunk k computes -- the kernels are ~3.7x slower per point than
+  // the PCIe copy, so a chunk may be ~3x its predecessor and still arrive in time.  Fewer, larger chunks also pay the
+  // per-chunk costs (sort launches, wave tails, bucket_merge over all G buckets) fewer times.  Resident scalars: equal chunks.
+  size_t bnd[kMaxPipelineChunks + 1];
+  uint32_t chunks = 0;
+  {
+    // G1 ratio 4, G2 ratio 12: the ratio tracks compute time / copy time
+    const double r = h_scalars ? (IsFq2<F>::value ? 12.0 : 4.0) : 1.0;
+    double tot = 0, w = 1;
+    for (uint32_t k = 0; k < K; ++k) { tot += w; w *= r; }
+    double cum = 0; w = 1;
+    bnd[0] = 0;
+    for (uint32_t k = 0; k < K; ++k) {
+      cum += w; w *= r;
+      size_t hi = (k == K - 1) ? n : std::min(n, (((size_t)((double)n * (cum / tot))) + 1023) & ~(size_t)1023);
+      if (hi > bnd[chunks]) bnd[++chunks] = hi;  // empty chunks (tiny n) vanish
+    }
+  }
+  // pair-summing rounds (one chunk only).  A round is bound by its ~330 B of scattered memory traffic per pair, not by its 6.7
+  // products, and costs more than the XYZZ addition it removes, so the automatic setting is OFF; the path stays available (b200zk_set_msm_pair_rounds)
+  // for parts with a different compute:bandwidth balance and is covered by the parity tests.
+  const size_t M_max = n * (size_t)pl.W;
+  uint32_t rounds = 0;
+  if (ctx->msm_pair_rounds >= 0) rounds = (uint32_t)ctx->msm_pair_rounds;
+  if (rounds > 4) rounds = 4;
+  if (rounds && M_max >= ((size_t)1 << 31)) rounds = 0;
+  if (sort_mode) rounds = 0;
+  // per chunk: slice length (each chunk fills whole waves of resident threads); over all chunks: the largest run count and
+  // the largest entry count of either sort
+  const size_t resident = resident_slices<F>(ctx);
+  uint32_t Lk[kMaxPipelineChunks];
+  size_t S_max = 0, M_two = 0, M_one = 0;
+  for (uint32_t k = 0; k < chunks; ++k) {
+    const size_t nk = bnd[k + 1] - bnd[k], Mk = nk * pl.W;
+    Lk[k] = pick_slice_len(Mk >> rounds, resident);
+    S_max = std::max(S_max, (Mk >> rounds) / Lk[k] + 1 + G);
+    SortPlan sp;
+    size_t& M_sort = make_sort_plan(nk, pl, ctx->sm_count, &sp) ? M_two : M_one;
+    M_sort = std::max(M_sort, Mk);
+  }
+  // Bucket totals first, one thread per bucket (full occupancy, every lane busy), then the running sums over dense totals:
+  // bucket_chunk's threads are few (G / chunk) and serial, so every run addition moved out of them shortens the
+  // latency-bound tail.  Dense totals also carry the chunked path's buckets from chunk to chunk.  Below 2^14 buckets a
+  // one-chunk call lets bucket_chunk sum the runs itself.
+  const bool dense_totals = chunked || G >= ((size_t)1 << 14);
+  {
+    SortWorkspace& s = ctx->sort;
+    const size_t tiles = std::max((G + kScanTile - 1) / kScanTile, ((size_t)kSortMaxBins * ctx->sm_count + kScanTile - 1) / kScanTile);
+    B2_TRY(ensure(ctx, s.hist, G * 4));
+    B2_TRY(ensure(ctx, s.offsets, (G + 1) * 4));
+    B2_TRY(ensure(ctx, s.run_off, (G + 1) * 4));
+    B2_TRY(ensure(ctx, s.tsum, tiles * 4));
+    B2_TRY(ensure(ctx, s.idx, std::max(M_two, M_one) * 4));
+    if (M_one) { B2_TRY(ensure(ctx, s.cursor, G * 4)); B2_TRY(ensure(ctx, s.digits, M_one * 4)); }
+    if (M_two) { B2_TRY(ensure(ctx, s.key, M_two * 8)); B2_TRY(ensure(ctx, s.ctab, sort_ctab_bytes(ctx->sm_count))); B2_TRY(ensure(ctx, s.cnt2, sort_cnt2_bytes(M_two))); }
+  }
+  if (rounds) {
+    B2_TRY(ensure(ctx, ctx->ws_q1, (M_max / 2 + G + 1) * pt));
+    if (rounds > 1) B2_TRY(ensure(ctx, ctx->ws_q0, (M_max / 4 + G + 1) * pt));
+    B2_TRY(ensure(ctx, ctx->ws_prefix, (M_max / 2 + G + 1) * FieldBytes<F>::value));
+    B2_TRY(ensure(ctx, ctx->ws_info, (M_max / 2 + G + 1) * 4));
+    B2_TRY(ensure(ctx, ctx->ws_pairoff0, (G + 1) * 4));
+    B2_TRY(ensure(ctx, ctx->ws_pairoff1, (G + 1) * 4));
+  }
+  B2_TRY(ensure(ctx, ctx->ws_buckets, S_max * xy));  // run partials (bucket totals after partial_tree)
+  B2_TRY(ensure(ctx, ctx->ws_segbucket, S_max * 4));
+  if (dense_totals) B2_TRY(ensure(ctx, ctx->ws_totals, G * xy));
+  B2_TRY(ensure(ctx, ctx->ws_chunkS, (size_t)pl.Wr * pl.T * xy));
+  B2_TRY(ensure(ctx, ctx->ws_chunkV, (size_t)pl.Wr * pl.T * xy));
+  const uint8_t* dsc = (const uint8_t*)d_scalars;
+  if (h_scalars) {
+    B2_TRY(ensure(ctx, ctx->ws_scalars, n * 32 + 32));
+    dsc = (const uint8_t*)ctx->ws_scalars.p;
+    if (!chunked) {
+      B2_CUDA(ctx, cudaMemcpyAsync(ctx->ws_scalars.p, h_scalars, n * 32, cudaMemcpyHostToDevice, st));
+    } else {
+      // all uploads issued up front on the copy stream (they serialise on the one H2D engine in chunk order); the staging
+      // buffer may still be read by the previous call's kernels on `st`, so the copy stream first waits for `st`
+      cudaStream_t cs = ctx->stream_upload;
+      B2_CUDA(ctx, cudaEventRecord(ctx->ev_in, st));
+      B2_CUDA(ctx, cudaStreamWaitEvent(cs, ctx->ev_in, 0));
+      for (uint32_t k = 0; k < chunks; ++k) {
+        const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
+        B2_CUDA(ctx, cudaMemcpyAsync((void*)(dsc + lo * 32), (const uint8_t*)h_scalars + lo * 32, nk * 32, cudaMemcpyHostToDevice, cs));
+        B2_CUDA(ctx, cudaEventRecord(ctx->ev_up[k], cs));
+      }
+    }
+  }
+  SortWorkspace& s = ctx->sort;
+  uint32_t *hist = (uint32_t*)s.hist.p, *offsets = (uint32_t*)s.offsets.p, *tsum = (uint32_t*)s.tsum.p, *run_off = (uint32_t*)s.run_off.p;
+  uint32_t* run_bucket = (uint32_t*)ctx->ws_segbucket.p;
+  for (uint32_t k = 0; k < chunks; ++k) {
+    const size_t lo = bnd[k], nk = bnd[k + 1] - lo;
+    const uint32_t L = Lk[k];
+    // sort(k) waits for upload k only: with the kernels serialised there is nothing to gain from sorting ahead, and
+    // sort(k+1) before accumulate(k) would stall the stream on upload k+1
+    if (chunked && h_scalars) B2_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_up[k], 0));
+    phase_mark(ctx, 0, st);
+    nvtxRangePushA("b200zk:msm_sort");
+    if (sort_mode == 2) {
+      // hist, offsets and idx are the sort the immediately preceding msm_run on this context left in ctx->sort: its
+      // callers (groth16_commit's column loop, msm_multi_resident_device) guarantee that call was mode 1 or 2 over the same
+      // scalars and the same plan, and mode 1 runs one chunk, so the whole sort is in the workspace
+      phase_mark(ctx, 1, st);
+      phase_mark(ctx, 2, st);
+    } else {
+      B2_TRY(sort_digits(ctx, dsc + lo * 32, nk, flags, pl, st));
+    }
+    nvtxRangePop();
+    phase_mark(ctx, 3, st);
+    NvtxRange nvtx_acc("b200zk:msm_accumulate+reduce");
+    // batched-affine pair-summing rounds: each halves the entries the XYZZ accumulation has to fold
+    const uint32_t* cur_off = offsets;
+    const void* cur_pts = (const uint8_t*)d_points + lo * pt;
+    for (uint32_t r = 1; r <= rounds; ++r) {
+      uint32_t* off_r = (uint32_t*)(r & 1 ? ctx->ws_pairoff1.p : ctx->ws_pairoff0.p);
+      B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, r, tsum, off_r));
+      const size_t out_max = (M_max >> r) + G;
+      void* q = (r & 1) ? ctx->ws_q1.p : ctx->ws_q0.p;
+      const unsigned pgrid = (unsigned)((out_max / kPairBatch + 1 + 127) / 128);
+      if (r == 1) B2_LAUNCH(ctx, (pair_sum<F, true>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
+      else B2_LAUNCH(ctx, (pair_sum<F, false>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
+      cur_off = off_r;
+      cur_pts = q;
+    }
+    B2_TRY(exclusive_scan(ctx, st, hist, cur_off, G, L, 0, tsum, run_off));
+    const size_t Mk = (nk * pl.W) >> rounds;
+    if (rounds) {
+      // a bucket of h entries leaves ceil(h / 2^rounds): up to G more than Mk
+      const size_t slices = (Mk + G + L - 1) / L;
+      B2_LAUNCH(ctx, (msm_accumulate<F, true>), (unsigned)((slices + 127) / 128), 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)run_off, (uint32_t)G, L, ctx->ws_buckets.p, run_bucket);
+    } else {
+      B2_TRY(launch_accumulate<F>(ctx, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)run_off, (uint32_t)G, L, (Mk + L - 1) / L, ctx->ws_buckets.p, run_bucket));
+    }
+    B2_TRY(fold_runs<F>(ctx, st, run_off, run_bucket, (uint32_t)G, (pl.merged ? nk * (size_t)pl.W : nk) >> rounds, L, S_max, ctx->ws_buckets.p));
+    phase_mark(ctx, 4, st);
+    if (dense_totals) B2_LAUNCH(ctx, bucket_merge<F>, (unsigned)((G + 127) / 128), 128, 0, st, (const void*)ctx->ws_buckets.p, (const uint32_t*)run_off, (uint32_t)G, k == 0 ? 1 : 0, ctx->ws_totals.p);
+  }
+  return reduce_buckets<F>(ctx, st, pl, dense_totals ? nullptr : run_off, d_partial);
 }
 
 template <class F>

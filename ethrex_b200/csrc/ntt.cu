@@ -398,24 +398,11 @@ struct Plan { int P; uint32_t s[4]; uint32_t t[4]; };
 
 static Plan make_ntt_plan(uint32_t k) {
   Plan p{};
-  const char* env = getenv("B200ZK_NTT_PLAN");  // e.g. "8,8,8" : experiment knob
-  if (env && *env) {
-    uint32_t sum = 0; int P = 0; const char* c = env;
-    while (*c && P < 4) { p.s[P] = (uint32_t)strtoul(c, (char**)&c, 10); sum += p.s[P]; ++P; if (*c == ',') ++c; }
-    bool ok = sum == k;
-    for (int i = 0; i < P; ++i) ok = ok && p.s[i] >= 1 && p.s[i] <= (uint32_t)kMaxStage;
-    if (ok) p.P = P;
-  }
-  if (!p.P) {
-    if (k <= (uint32_t)kMaxStage) { p.P = 1; p.s[0] = k; }
-    // 64 KiB tiles keep several CTAs per SM to cover barrier and copy latency, so stages are capped at 10-11
-    else if (k <= 20) { p.P = 2; p.s[0] = (k + 1) / 2; p.s[1] = k - p.s[0]; }
-    else { p.P = 3; p.s[0] = (k + 2) / 3; p.s[1] = (k - p.s[0] + 1) / 2; p.s[2] = k - p.s[0] - p.s[1]; }
-  }
-  uint32_t tile_log = 11;  // 2048 elements = 64 KiB per CTA by default
-  const char* te = getenv("B200ZK_NTT_TILE_LOG");
-  if (te && *te) tile_log = (uint32_t)strtoul(te, nullptr, 10);
-  if (tile_log > (uint32_t)kMaxStage) tile_log = kMaxStage;
+  if (k <= (uint32_t)kMaxStage) { p.P = 1; p.s[0] = k; }
+  // 64 KiB tiles keep several CTAs per SM to cover barrier and copy latency, so stages are capped at 10-11
+  else if (k <= 20) { p.P = 2; p.s[0] = (k + 1) / 2; p.s[1] = k - p.s[0]; }
+  else { p.P = 3; p.s[0] = (k + 2) / 3; p.s[1] = (k - p.s[0] + 1) / 2; p.s[2] = k - p.s[0] - p.s[1]; }
+  const uint32_t tile_log = 11;  // 2048 elements = 64 KiB per CTA
   for (int i = 0; i < p.P; ++i) {
     uint32_t tl = tile_log < p.s[i] ? p.s[i] : tile_log;
     p.t[i] = tl - p.s[i];
@@ -435,16 +422,9 @@ static int launch_pass(b200zk_ctx* ctx, const PassArgs& a, cudaStream_t st) {
     B2_LAUNCH(ctx, (ntt_pass<512, 1>), grid, 512, smem, st, a);
   } else {
     // 64 KiB tiles: three CTAs fit an SM's shared memory; MINB = 3 caps registers at 85 so that they also fit
-    // its register file (experiment knob B200ZK_NTT_MINB=2 keeps the uncapped 100-register build)
-    static int minb = 0;  // the knob only (an environment variable is process-wide by nature)
-    if (!minb) { const char* e = getenv("B200ZK_NTT_MINB"); minb = (e && *e == '2') ? 2 : 3; }
-    if (!ctx->attr_ntt256) {
-      B2_CUDA(ctx, cudaFuncSetAttribute((ntt_pass<256, 2>), cudaFuncAttributeMaxDynamicSharedMemorySize, 1 << 16));
-      B2_CUDA(ctx, cudaFuncSetAttribute((ntt_pass<256, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize, 1 << 16));
-      ctx->attr_ntt256 = true;
-    }
-    if (minb == 2) B2_LAUNCH(ctx, (ntt_pass<256, 2>), grid, 256, smem, st, a);
-    else B2_LAUNCH(ctx, (ntt_pass<256, 3>), grid, 256, smem, st, a);
+    // its register file
+    if (!ctx->attr_ntt256) { B2_CUDA(ctx, cudaFuncSetAttribute((ntt_pass<256, 3>), cudaFuncAttributeMaxDynamicSharedMemorySize, 1 << 16)); ctx->attr_ntt256 = true; }
+    B2_LAUNCH(ctx, (ntt_pass<256, 3>), grid, 256, smem, st, a);
   }
   return B200ZK_OK;
 }

@@ -1,5 +1,5 @@
 """The MSM schedules that the other parity files do not reach: BLS12-381 (msm_run<Fp381>, 256 scalar bits) through the
-two-level sort, dense bucket totals, pair-sum rounds, the chunk-pipelined schedule, window tables and forced windows; the
+two-level sort, dense bucket totals, pair-sum rounds, the chunked schedule, window tables and forced windows; the
 BN254 partial-sum entry points over resident bases; the profiled schedule; and the refusal of B200ZK_SCALARS_RAW by every
 BN254 MSM entry point.
 
@@ -32,7 +32,7 @@ class Plan:
     G: int            # buckets to reduce: W * 2^(c-1), or 2^(c-1) on a window table
     merged: bool      # window table: all windows share one bucket set
     two_level: bool   # two-level digit sort instead of the legacy hist / scan / scatter one
-    dense: bool       # one-shot schedule: dense bucket totals instead of the fused bucket_chunk
+    dense: bool       # one-chunk call: dense bucket totals instead of the fused bucket_chunk (a chunked call always has them)
     bitsums: bool     # bucket reduction by bit-sums (T >= 64) instead of the pairwise tree
 
     @property
@@ -47,8 +47,8 @@ def table_window(n_bases: int) -> int:
 
 
 def msm_plan(n: int, forced_c: int = 0, scalar_bits: int = 255, table_c: int = 0) -> Plan:
-    """make_plan (msm.cu:56-79), make_sort_plan (msm.cu:270-287) and the reduction choices of msm_run (dense totals
-    msm.cu:1514, bit-sums msm.cu:1631).  scalar_bits: 255 for BN254, 256 for BLS12-381 (ScalarBits<F>)."""
+    """make_plan (msm.cu:54-71), make_sort_plan (msm.cu:260-277) and the reduction choices of msm_run (dense totals
+    msm.cu:1577, bit-sums msm.cu:1478).  scalar_bits: 255 for BN254, 256 for BLS12-381 (ScalarBits<F>)."""
     lg = (n - 1).bit_length()
     forced = table_c or forced_c       # a window table fixes c; set_msm_window does not apply to it
     c = forced if forced else (lg - 4 if lg > 8 else 4)
@@ -66,8 +66,10 @@ def msm_plan(n: int, forced_c: int = 0, scalar_bits: int = 255, table_c: int = 0
 
 
 def pipelined(n: int, chunks: int = 0, host_scalars: bool = False, profiling: bool = False, pair_rounds: int = -1, g2: bool = False) -> bool:
-    """msm_run's choice of the chunk-pipelined schedule (msm.cu:1499-1502).  BLS12-381 calls stage their scalars
-    themselves and reach msm_run with device scalars (host_scalars=False)."""
+    """msm_run's one rule for more than one chunk, or host scalars uploaded on the copy stream (msm.cu:1526-1529): a
+    plain call (sort_mode 0) with K > 1 chunks or host scalars, not profiled, without pair-sum rounds, from 4096 points.
+    Otherwise the call runs one chunk and stages host scalars on the caller's stream.  BLS12-381 calls stage their
+    scalars themselves and reach msm_run with device scalars (host_scalars=False)."""
     K = chunks or ((2 if g2 else 3) if host_scalars and n >= (1 << 22) else 1)
     return (K > 1 or host_scalars) and not profiling and pair_rounds <= 0 and n >= 4096
 

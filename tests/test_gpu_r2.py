@@ -395,32 +395,47 @@ def test_two_level_sort_on_skewed_scalars(ctx, table):
             ctx.bases_free(h)
 
 
-def test_host_scalar_pipeline_with_growing_chunks(ctx, monkeypatch):
-    """b200zk_g1_msm_resident with HOST scalars cuts the points into chunks whose sizes grow geometrically (only the first
-    chunk's upload is exposed; B200ZK_CHUNK_RATIO, default 3; set_msm_chunks = how many).  Every (count, ratio) -- equal
-    chunks, steep growth, more chunks than 1024-point units at the small size -- must return the one-shot bytes, with the
-    two-level sort (chunks >= 2^16 points) and with the legacy one (small chunks), on plain bases and on a window table."""
+def test_host_scalar_pipeline_with_growing_chunks(ctx):
+    """set_msm_chunks = how many chunks an MSM's points are cut into.  Over device scalars the chunks are equal (ratio 1);
+    over HOST scalars their sizes grow geometrically so that only the first chunk's upload is exposed (ratio 4 for G1,
+    12 for G2).  Every count must return the one-chunk bytes, with the two-level sort (chunks >= 2^16 points) and with the
+    one-pass one (small chunks; the tiny case, where most chunks are empty and vanish), on plain bases and on a window
+    table."""
+    import torch
     k, d = chain_kd()
-    n = (1 << 18) + 777
+    n, m = (1 << 18) + 777, 5000
     pts = orc.g1_chain(n, k, d)
     s = np.ascontiguousarray(orc.rand_fr(pyref.SEED_SCALARS, 0, n))
     s[: n // 3] = s[3]                       # a heavy bucket per window inside the first chunks
-    exp = orc.g1_msm(pts, s)
+    exp, exp_m = orc.g1_msm(pts, s), orc.g1_msm(pts[:m], s[:m])
+    ds = to_dev(s)
     dp = to_dev(pts)
     h = ctx.g1_bases_from_device(dp, n)
     ht = ctx.g1_bases_from_device(dp, n)
     ctx.bases_precompute(ht, 0)
+    dp2 = dev_empty(16 * n)
+    ctx.g2_chain_device(dp2, 0, n, k, d)
+    h2 = ctx.g2_bases_from_device(dp2, n)
+    h2t = ctx.g2_bases_from_device(dp2, n)
+    ctx.bases_precompute(h2t, 0)
+    del dp2
+    torch.cuda.empty_cache()
+    exp2, exp2_m = expected_chain_msm_g2(s, k, d), expected_chain_msm_g2(s[:m], k, d)
     try:
-        assert ctx.g1_msm_resident_device(ht, to_dev(s), n) == exp
+        assert ctx.g1_msm_resident_device(ht, ds, n) == exp
         for chunks in (2, 3, 5):
             ctx.set_msm_chunks(chunks)
-            for ratio in ("1", "2.5", "3", "8"):
-                monkeypatch.setenv("B200ZK_CHUNK_RATIO", ratio)
-                assert ctx.g1_msm_resident(ht, s, n) == exp, (chunks, ratio, "table")
-                assert ctx.g1_msm_resident(h, s, n) == exp, (chunks, ratio, "plain")
-                m = 5000                      # tiny: most chunks are empty and vanish
-                assert ctx.g1_msm_resident(h, s[:m], m) == orc.g1_msm(pts[:m], s[:m]), (chunks, ratio, "tiny")
+            for handle, kind in ((ht, "table"), (h, "plain")):
+                assert ctx.g1_msm_resident_device(handle, ds, n) == exp, (chunks, kind, "ratio 1")
+                assert ctx.g1_msm_resident(handle, s, n) == exp, (chunks, kind, "ratio 4")
+            assert ctx.g1_msm_resident_device(h, ds, m) == exp_m, (chunks, "tiny", "ratio 1")
+            assert ctx.g1_msm_resident(h, s[:m], m) == exp_m, (chunks, "tiny", "ratio 4")
+        for chunks in (2, 3):
+            ctx.set_msm_chunks(chunks)
+            for handle, kind in ((h2t, "table"), (h2, "plain")):
+                assert ctx.g2_msm_resident(handle, s, n) == exp2, (chunks, kind, "ratio 12")
+            assert ctx.g2_msm_resident(h2, s[:m], m) == exp2_m, (chunks, "tiny", "ratio 12")
     finally:
         ctx.set_msm_chunks(0)
-        ctx.bases_free(h)
-        ctx.bases_free(ht)
+        for handle in (h, ht, h2, h2t):
+            ctx.bases_free(handle)

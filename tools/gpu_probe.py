@@ -1,4 +1,4 @@
-"""Exploration probe (not the bench): times the field core, NTT plans and MSM windows on one GPU and
+"""Exploration probe (not the bench): times the field core, the NTT and MSM windows on one GPU and
 writes JSON lines to gpurun_out/probe.jsonl.  Usage: python tools/gpu_probe.py [section ...]"""
 import json
 import os
@@ -62,18 +62,11 @@ def main():
             n = 1 << log_n
             d = dev(4 * n)
             ctx.fr_random_device(d, n, 3, 0, eb.SCALARS_MONT)
-            plans = ["", "12,12", "8,8,8"] if log_n == 24 else ["", "10,10", "7,7,6"]
-            for plan in plans:
-                for tile in ("11", "12"):
-                    os.environ["B200ZK_NTT_PLAN"] = plan
-                    os.environ["B200ZK_NTT_TILE_LOG"] = tile
-                    try:
-                        med, best = timed(lambda: ctx.fr_ntt_device(d, log_n, 0), iters=5)
-                        emit(section="ntt", log_n=log_n, plan=plan or "auto", tile_log=tile, ms=med, best_ms=best, gelem_per_s=n / best / 1e6)
-                    except Exception as e:  # noqa: BLE001
-                        emit(section="ntt", log_n=log_n, plan=plan, tile_log=tile, error=str(e))
-            os.environ.pop("B200ZK_NTT_PLAN", None)
-            os.environ.pop("B200ZK_NTT_TILE_LOG", None)
+            try:
+                med, best = timed(lambda: ctx.fr_ntt_device(d, log_n, 0), iters=5)
+                emit(section="ntt", log_n=log_n, ms=med, best_ms=best, gelem_per_s=n / best / 1e6)
+            except Exception as e:  # noqa: BLE001
+                emit(section="ntt", log_n=log_n, error=str(e))
     if "msm" in sections:
         import pyref
         k, dd = pyref.chain_scalar(pyref.SEED_POINTS)

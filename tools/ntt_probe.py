@@ -16,4 +16,4 @@ for log_n in (20, 22, 24):
     ctx.fr_random_device(d, n, 3, 0, eb.SCALARS_MONT)
     for flags, name in ((0, "fwd"), (eb.NTT_INVERSE, "inv"), (eb.NTT_COSET, "coset"), (eb.NTT_COSET | eb.NTT_INVERSE, "coset_inv")):
         ms = timed(lambda: ctx.fr_ntt_device(d, log_n, flags))
-        print(json.dumps({"log_n": log_n, "mode": name, "minb": os.environ.get("B200ZK_NTT_MINB", "3"), "ms": round(ms, 4), "gelem_s": round(n / ms / 1e6, 3)}), flush=True)
+        print(json.dumps({"log_n": log_n, "mode": name, "ms": round(ms, 4), "gelem_s": round(n / ms / 1e6, 3)}), flush=True)
