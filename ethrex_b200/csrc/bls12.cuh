@@ -1,8 +1,8 @@
 // bls12.cuh -- BLS12-381 pieces shared by bls381.cu (commitments, proofs), bls_pairing.cu (the pairing, KZG verification)
 // and bls_ops.cu (EIP-2537 addition and MSM): big-endian byte loaders and stores, the 48-byte compressed G1 decoding, the
 // EIP-2537 64-byte field element, Fp2 = Fp[u]/(u^2 + 1) over Fp381 with Fq2's interface, so curve.cuh's XYZZ formulas (and
-// xyzz_scalar_mul) instantiate over the twist unchanged, the r P = O subgroup checks, and the workspace carver of the
-// pairing-family calls.  The build has no -rdc: each translation unit keeps its own device copy of the __noinline__
+// xyzz_scalar_mul and in_subgroup) instantiate over the twist unchanged, and the workspace carver of the pairing-family
+// calls.  The build has no -rdc: each translation unit keeps its own device copy of the __noinline__
 // functions, and `inline` lets the host linker merge their host-side stubs.
 #pragma once
 #include "common.cuh"
@@ -118,20 +118,6 @@ struct Fp2_381 {
 template <> struct CurveB<Fp2_381> {
   static B2_D Fp2_381 b() { Fp381 four = Fp381::zero(); four.v[0] = 4; four = Fp381::to_mont(four); return {four, four}; }  // 4 (1 + u)
 };
-
-// ---- subgroup checks: r P = O (no endomorphism shortcuts) -------------------------------------------------------------
-__device__ __noinline__ inline bool g1_in_subgroup(const Affine<Fp381>& p) {
-  uint32_t k[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
-  return xyzz_scalar_mul<Fp381>(k, p).is_inf();
-}
-__device__ __noinline__ inline bool g2_in_subgroup(const Affine<Fp2_381>& q) {
-  uint32_t k[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) k[j] = bls_r_limb(j);
-  return xyzz_scalar_mul<Fp2_381>(k, q).is_inf();
-}
 
 // EIP-2537 field element: 16 zero bytes, then 48 bytes big-endian below p
 B2_D bool load_fp64(const uint8_t* src, Fp381* out) {

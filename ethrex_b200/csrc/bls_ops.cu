@@ -45,11 +45,6 @@ B2_D void store_fe64(uint8_t* out, const F2& a) { store_fe64(out, a.c0); store_f
 // the precompile's output: padded EIP-2537 coordinates, the identity (0, 0) as all-zero bytes
 template <class F> B2_D void store_point64(uint8_t* out, const Affine<F>& p) { store_fe64(out, p.x); store_fe64(out + fe_bytes<F>(), p.y); }
 
-template <class F> B2_D bool in_subgroup(const Affine<F>& p) {
-  if constexpr (sizeof(F) == sizeof(Fp381)) return g1_in_subgroup(p);
-  else return g2_in_subgroup(p);
-}
-
 // ---- kernels ----------------------------------------------------------------------------------------------------------
 // one thread per item: out[i] = a[i] + b[i].  Both points are range-checked (status 2) before either curve check (status 3)
 template <class F>
@@ -81,14 +76,14 @@ __global__ void __launch_bounds__(64) bls_msm_terms(const uint8_t* __restrict__ 
   XYZZ<F> t = XYZZ<F>::identity();
   uint32_t s = 0;
   if (!load_point64(src, &p)) s = B200ZK_ERR_NOT_IN_FIELD;
-  else if (!affine_on_curve(p) || (!p.is_inf() && !in_subgroup(p))) s = B200ZK_ERR_NOT_ON_CURVE;
+  else if (!affine_on_curve(p) || (!p.is_inf() && !in_subgroup<bls_r_limb>(p))) s = B200ZK_ERR_NOT_ON_CURVE;
   else if (!p.is_inf()) t = xyzz_scalar_mul<F>(load_be32(src + point_bytes<F>()).v, p);  // raw 256 bits, not reduced
   terms[i] = t;
   pst[i] = (uint8_t)s;
 }
 
 // one CTA per call: pairs [offsets[c], offsets[c + 1]).  A range error anywhere in the call outranks a curve error (the
-// precedence of bls_pairing_final); a failed call writes zero bytes
+// precedence of pairing_check); a failed call writes zero bytes
 template <class F>
 __global__ void __launch_bounds__(kFoldThreads) bls_msm_fold(const XYZZ<F>* terms, const uint8_t* pst, const uint32_t* offsets, uint8_t* out, uint8_t* status) {
   __shared__ XYZZ<F> part[kFoldThreads];

@@ -4,8 +4,8 @@
 //   verify_blob_kzg_proof_batch        BlobsBundle::verify_kzg_proofs -> kzg::verify_kzg_proof_batch (blobs_bundle.rs:155-173,
 //                                      kzg.rs:168-192); verify_blob_kzg_proof (provider.rs:509-544) is its batch of one
 //
-// Tower: Fp2 = Fp[u]/(u^2 + 1) (bls12.cuh), Fp6 = Fp2[v]/(v^3 - (1 + u)), Fp12 = Fp6[w]/(w^2 - v).  The twist is M-type:
-// E': y^2 = x^3 + 4(1 + u).
+// Tower: Fp2 = Fp[u]/(u^2 + 1) (bls12.cuh), Fp6 = Fp2[v]/(v^3 - (1 + u)), Fp12 = Fp6[w]/(w^2 - v) (tower.cuh).  The
+// twist is M-type: E': y^2 = x^3 + 4(1 + u).
 // Miller loop: optimal ate over |x| = 0xd201000000010000 (64 bits: 63 doublings, 5 additions).  The line coefficients of a
 // G2 point depend on that point only, so a prepare pass (one thread per G2 point) writes its 68 triples in homogeneous
 // projective coordinates -- no inversion anywhere -- and the Miller kernel (one thread per pair) only evaluates them at P:
@@ -16,6 +16,7 @@
 // a check asks whether a product of pairings is one, and since gcd(3, r) = 1, z^3 = 1 exactly when z = 1 for z in the
 // order-r group mu_r.  tests/test_bls12_pairing_host.py recomputes every constant of this file and checks the identity.
 #include "bls12.cuh"
+#include "tower.cuh"
 #include "sha256.h"
 #include <cstring>
 #include <vector>
@@ -62,10 +63,8 @@ const uint8_t kG2GenCompressed[96] = {
 
 constexpr uint64_t kX = 0xd201000000010000ull;  // |x|; x = -|x|
 constexpr int kLines = 68;                      // line triples per G2 point: 63 doublings + 5 additions
-constexpr uint8_t kTrivial = 0x80;              // pair status bit: a side is the identity, the pair contributes 1
 
-struct Fp6b { F2 c0, c1, c2; };
-struct Fp12b { Fp6b c0, c1; };
+typedef Fp12<F2> F12;
 struct BlsLine { F2 c0, c1, c2; };  // l = c0 + (c1 xP) v + (c2 yP) v w  (mul_by_014 positions)
 
 B2_D Fp381 fp_const(const uint32_t* canonical) {
@@ -75,91 +74,38 @@ B2_D Fp381 fp_const(const uint32_t* canonical) {
   return Fp381::to_mont(a);
 }
 
-// ---- Fp6 ------------------------------------------------------------------------------------------------------------
-B2_D Fp6b f6_zero() { return {F2::zero(), F2::zero(), F2::zero()}; }
-B2_D Fp6b f6_one() { return {F2::one(), F2::zero(), F2::zero()}; }
-B2_D Fp6b f6_add(const Fp6b& a, const Fp6b& b) { return {F2::add(a.c0, b.c0), F2::add(a.c1, b.c1), F2::add(a.c2, b.c2)}; }
-B2_D Fp6b f6_sub(const Fp6b& a, const Fp6b& b) { return {F2::sub(a.c0, b.c0), F2::sub(a.c1, b.c1), F2::sub(a.c2, b.c2)}; }
-B2_D Fp6b f6_neg(const Fp6b& a) { return {F2::neg(a.c0), F2::neg(a.c1), F2::neg(a.c2)}; }
-B2_D Fp6b f6_mul_v(const Fp6b& a) { return {F2::mul_xi(a.c2), a.c0, a.c1}; }
-__device__ __noinline__ Fp6b f6_mul(const Fp6b& a, const Fp6b& b) {  // Karatsuba over Fp2: six products
-  const F2 t0 = F2::mul(a.c0, b.c0), t1 = F2::mul(a.c1, b.c1), t2 = F2::mul(a.c2, b.c2);
-  Fp6b r;
-  r.c0 = F2::add(t0, F2::mul_xi(F2::sub(F2::sub(F2::mul(F2::add(a.c1, a.c2), F2::add(b.c1, b.c2)), t1), t2)));
-  r.c1 = F2::add(F2::sub(F2::sub(F2::mul(F2::add(a.c0, a.c1), F2::add(b.c0, b.c1)), t0), t1), F2::mul_xi(t2));
-  r.c2 = F2::add(F2::sub(F2::sub(F2::mul(F2::add(a.c0, a.c2), F2::add(b.c0, b.c2)), t0), t2), t1);
-  return r;
-}
-// a (b0 + b1 v): the line's sparse shape
-__device__ __noinline__ Fp6b f6_mul_01(const Fp6b& a, const F2& b0, const F2& b1) {
-  return {F2::add(F2::mul(a.c0, b0), F2::mul_xi(F2::mul(a.c2, b1))), F2::add(F2::mul(a.c0, b1), F2::mul(a.c1, b0)),
-          F2::add(F2::mul(a.c1, b1), F2::mul(a.c2, b0))};
-}
-B2_D Fp6b f6_mul_1(const Fp6b& a, const F2& b1) { return {F2::mul_xi(F2::mul(a.c2, b1)), F2::mul(a.c0, b1), F2::mul(a.c1, b1)}; }
-__device__ __noinline__ Fp6b f6_inv(const Fp6b& a) {
-  const F2 A = F2::sub(F2::sqr(a.c0), F2::mul_xi(F2::mul(a.c1, a.c2)));
-  const F2 B = F2::sub(F2::mul_xi(F2::sqr(a.c2)), F2::mul(a.c0, a.c1));
-  const F2 C = F2::sub(F2::sqr(a.c1), F2::mul(a.c0, a.c2));
-  const F2 Fi = F2::inv(F2::add(F2::mul(a.c0, A), F2::mul_xi(F2::add(F2::mul(a.c2, B), F2::mul(a.c1, C)))));
-  return {F2::mul(A, Fi), F2::mul(B, Fi), F2::mul(C, Fi)};
-}
-
-// ---- Fp12 -----------------------------------------------------------------------------------------------------------
-B2_D Fp12b f12_one() { return {f6_one(), f6_zero()}; }
-__device__ __noinline__ Fp12b f12_mul(const Fp12b& a, const Fp12b& b) {
-  const Fp6b t0 = f6_mul(a.c0, b.c0), t1 = f6_mul(a.c1, b.c1);
-  return {f6_add(t0, f6_mul_v(t1)), f6_sub(f6_sub(f6_mul(f6_add(a.c0, a.c1), f6_add(b.c0, b.c1)), t0), t1)};
-}
-__device__ __noinline__ Fp12b f12_sqr(const Fp12b& a) {  // complex squaring: two Fp6 products
-  const Fp6b ab = f6_mul(a.c0, a.c1);
-  const Fp6b c0 = f6_sub(f6_sub(f6_mul(f6_add(a.c0, a.c1), f6_add(a.c0, f6_mul_v(a.c1))), ab), f6_mul_v(ab));
-  return {c0, f6_add(ab, ab)};
-}
-// f (c0 + c1 v + c4 v w): aa = f.c0 (c0 + c1 v), bb = f.c1 (c4 v), then Karatsuba over Fp6
-__device__ __noinline__ Fp12b f12_mul_014(const Fp12b& f, const F2& c0, const F2& c1, const F2& c4) {
-  const Fp6b aa = f6_mul_01(f.c0, c0, c1), bb = f6_mul_1(f.c1, c4);
-  const Fp6b t = f6_mul_01(f6_add(f.c0, f.c1), c0, F2::add(c1, c4));
-  return {f6_add(aa, f6_mul_v(bb)), f6_sub(f6_sub(t, aa), bb)};
-}
-B2_D Fp12b f12_conj(const Fp12b& a) { return {a.c0, f6_neg(a.c1)}; }
-__device__ __noinline__ Fp12b f12_inv(const Fp12b& a) {
-  const Fp6b t = f6_inv(f6_sub(f6_mul(a.c0, a.c0), f6_mul_v(f6_mul(a.c1, a.c1))));
-  return {f6_mul(a.c0, t), f6_neg(f6_mul(a.c1, t))};
-}
-B2_D bool f12_is_one(const Fp12b& a) {
-  return a.c0.c0 == F2::one() && a.c0.c1.is_zero() && a.c0.c2.is_zero() && a.c1.c0.is_zero() && a.c1.c1.is_zero() && a.c1.c2.is_zero();
-}
+// ---- Frobenius maps -------------------------------------------------------------------------------------------------
 // (sum_k a_k w^k)^p = sum_k conj(a_k) xi^(k (p-1)/6) w^k; the coefficient of w^k is c0.c_(k/2) for even k, c1.c_(k/2) for odd
 B2_D F2 frob1_coeff(int k) { return {fp_const(kFrob1[k][0]), fp_const(kFrob1[k][1])}; }
-__device__ __noinline__ Fp12b f12_frob(const Fp12b& a) {
+__device__ __noinline__ F12 f12_frob(const F12& a) {
   return {{F2::mul(F2::conj(a.c0.c0), frob1_coeff(0)), F2::mul(F2::conj(a.c0.c1), frob1_coeff(2)), F2::mul(F2::conj(a.c0.c2), frob1_coeff(4))},
           {F2::mul(F2::conj(a.c1.c0), frob1_coeff(1)), F2::mul(F2::conj(a.c1.c1), frob1_coeff(3)), F2::mul(F2::conj(a.c1.c2), frob1_coeff(5))}};
 }
-__device__ __noinline__ Fp12b f12_frob2(const Fp12b& a) {  // Fp2 is fixed by the p^2 power: only the w^k factors move
+__device__ __noinline__ F12 f12_frob2(const F12& a) {  // Fp2 is fixed by the p^2 power: only the w^k factors move
   return {{a.c0.c0, F2::scale(a.c0.c1, fp_const(kFrob2[2])), F2::scale(a.c0.c2, fp_const(kFrob2[4]))},
           {F2::scale(a.c1.c0, fp_const(kFrob2[1])), F2::scale(a.c1.c1, fp_const(kFrob2[3])), F2::scale(a.c1.c2, fp_const(kFrob2[5]))}};
 }
 
 // f^x for f in the cyclotomic subgroup (there f^-1 = conj f): square-and-multiply over |x|, then conjugate
-__device__ __noinline__ Fp12b f12_exp_x(const Fp12b& f) {
-  Fp12b acc = f;
+__device__ __noinline__ F12 f12_exp_x(const F12& f) {
+  F12 acc = f;
 #pragma unroll 1
   for (int i = 62; i >= 0; --i) {
-    acc = f12_sqr(acc);
-    if ((kX >> i) & 1) acc = f12_mul(acc, f);
+    acc = F12::sqr(acc);
+    if ((kX >> i) & 1) acc = F12::mul(acc, f);
   }
-  return f12_conj(acc);
+  return F12::conj(acc);
 }
 
 // f^(3 (p^12 - 1)/r): see the header for why the cube answers "is the pairing product one" exactly
-__device__ __noinline__ Fp12b final_exponentiate(const Fp12b& f0) {
-  Fp12b f = f12_mul(f12_conj(f0), f12_inv(f0));  // f^(p^6 - 1)
-  f = f12_mul(f12_frob2(f), f);                   // ^(p^2 + 1): f is now in the cyclotomic subgroup
-  Fp12b t = f12_mul(f12_exp_x(f), f12_conj(f));   // f^(x - 1)
-  t = f12_mul(f12_exp_x(t), f12_conj(t));         // f^((x - 1)^2)
-  t = f12_mul(f12_exp_x(t), f12_frob(t));         // ^(x + p)
-  t = f12_mul(f12_mul(f12_exp_x(f12_exp_x(t)), f12_frob2(t)), f12_conj(t));  // ^(x^2 + p^2 - 1)
-  return f12_mul(t, f12_mul(f12_sqr(f), f));      // * f^3
+__device__ __noinline__ F12 final_exponentiate(const F12& f0) {
+  F12 f = F12::mul(F12::conj(f0), F12::inv(f0));  // f^(p^6 - 1)
+  f = F12::mul(f12_frob2(f), f);                   // ^(p^2 + 1): f is now in the cyclotomic subgroup
+  F12 t = F12::mul(f12_exp_x(f), F12::conj(f));    // f^(x - 1)
+  t = F12::mul(f12_exp_x(t), F12::conj(t));        // f^((x - 1)^2)
+  t = F12::mul(f12_exp_x(t), f12_frob(t));         // ^(x + p)
+  t = F12::mul(F12::mul(f12_exp_x(f12_exp_x(t)), f12_frob2(t)), F12::conj(t));  // ^(x^2 + p^2 - 1)
+  return F12::mul(t, F12::mul(F12::sqr(f), f));   // * f^3
 }
 
 // ---- G2 line coefficients, homogeneous projective T = (X : Y : Z), M-type twist ---------------------------------------
@@ -205,20 +151,20 @@ __device__ __noinline__ void g2_prepare(const Affine<F2>& q, BlsLine* out) {
 }
 
 // f_{|x|,Q}(P) over prepared lines, conjugated for x < 0
-__device__ __noinline__ Fp12b miller_prepared(const BlsLine* L, const Affine<Fp381>& p) {
-  Fp12b f = f12_one();
+__device__ __noinline__ F12 miller_prepared(const BlsLine* L, const Affine<Fp381>& p) {
+  F12 f = F12::one();
   int k = 0;
 #pragma unroll 1
   for (int i = 62; i >= 0; --i) {
-    f = f12_sqr(f);
+    f = F12::sqr(f);
     BlsLine l = L[k++];
-    f = f12_mul_014(f, l.c0, F2::scale(l.c1, p.x), F2::scale(l.c2, p.y));
+    f = F12::mul_014(f, l.c0, F2::scale(l.c1, p.x), F2::scale(l.c2, p.y));
     if ((kX >> i) & 1) {
       l = L[k++];
-      f = f12_mul_014(f, l.c0, F2::scale(l.c1, p.x), F2::scale(l.c2, p.y));
+      f = F12::mul_014(f, l.c0, F2::scale(l.c1, p.x), F2::scale(l.c2, p.y));
     }
   }
-  return f12_conj(f);
+  return F12::conj(f);
 }
 
 // ---- kernels ----------------------------------------------------------------------------------------------------------
@@ -240,7 +186,7 @@ __global__ void __launch_bounds__(64) bls_pair_decode(const uint8_t* __restrict_
     p = {Fp381::to_mont(c[0]), Fp381::to_mont(c[1])};
     q = {{Fp381::to_mont(c[2]), Fp381::to_mont(c[3])}, {Fp381::to_mont(c[4]), Fp381::to_mont(c[5])}};
     if (!affine_on_curve(p) || !affine_on_curve(q)) s = B200ZK_ERR_NOT_ON_CURVE;
-    else if ((!p.is_inf() && !g1_in_subgroup(p)) || (!q.is_inf() && !g2_in_subgroup(q))) s = B200ZK_ERR_NOT_ON_CURVE;
+    else if ((!p.is_inf() && !in_subgroup<bls_r_limb>(p)) || (!q.is_inf() && !in_subgroup<bls_r_limb>(q))) s = B200ZK_ERR_NOT_ON_CURVE;
   }
   if (!s && (p.is_inf() || q.is_inf())) s = kTrivial;
   P[i] = p;
@@ -272,7 +218,7 @@ __global__ void __launch_bounds__(64) bls_g2_decode(const uint8_t* __restrict__ 
       const bool larger = Fp381::less(half, y1) || (y1.is_zero() && Fp381::less(half, y0));
       if (larger != sign_flag) y = F2::neg(y);
       pt = {x, y};
-      if (!g2_in_subgroup(pt)) bad_point = true;
+      if (!in_subgroup<bls_r_limb>(pt)) bad_point = true;
     }
   }
   if (bad_field) atomicMin(status, (unsigned long long)i);
@@ -290,34 +236,12 @@ __global__ void __launch_bounds__(64) bls_g2_prepare(const Affine<F2>* Q, const 
 }
 
 // one thread per pair: the Miller value over prepared lines (pair i uses line set i, or i % period when period != 0)
-__global__ void __launch_bounds__(32) bls_miller(const Affine<Fp381>* P, const BlsLine* lines, uint32_t period, const uint8_t* pst, size_t n, Fp12b* f) {
+__global__ void __launch_bounds__(32) bls_miller(const Affine<Fp381>* P, const BlsLine* lines, uint32_t period, const uint8_t* pst, size_t n, F12* f) {
   const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  Fp12b r = f12_one();
+  F12 r = F12::one();
   if (!pst[i]) r = miller_prepared(lines + kLines * (period ? i % period : i), P[i]);
   f[i] = r;
-}
-
-// one thread per check: the product of its Miller values, one final exponentiation.  A range error anywhere in the check
-// outranks a curve error (every point is range-checked before any curve check)
-__global__ void __launch_bounds__(32) bls_pairing_final(const Fp12b* f, const uint8_t* pst, const uint32_t* offsets, size_t count, uint8_t* result, uint8_t* status) {
-  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  const uint32_t lo = offsets[i], hi = offsets[i + 1];
-  uint32_t s = 0;
-  for (uint32_t k = lo; k < hi; ++k) {
-    const uint32_t ps = pst[k] & ~kTrivial;
-    if (ps == B200ZK_ERR_NOT_IN_FIELD) s = ps;
-    else if (ps && !s) s = ps;
-  }
-  uint32_t ok = 0;
-  if (!s) {
-    Fp12b acc = f12_one();
-    for (uint32_t k = lo; k < hi; ++k) acc = f12_mul(acc, f[k]);
-    ok = f12_is_one(final_exponentiate(acc)) ? 1u : 0u;
-  }
-  result[i] = (uint8_t)ok;
-  status[i] = (uint8_t)s;
 }
 
 // c-kzg validate_kzg_g1 on 48-byte compressed points: decompression (status 2 / 3) and r P = O (status 3); identity valid
@@ -326,7 +250,7 @@ __global__ void __launch_bounds__(64) bls_g1_decode_subgroup(const uint8_t* __re
   if (i >= n) return;
   Affine<Fp381> p;
   uint32_t s = bls_g1_decompress(in + 48 * i, &p);
-  if (!s && !p.is_inf() && !g1_in_subgroup(p)) s = B200ZK_ERR_NOT_ON_CURVE;
+  if (!s && !p.is_inf() && !in_subgroup<bls_r_limb>(p)) s = B200ZK_ERR_NOT_ON_CURVE;
   if (s) p = {Fp381::zero(), Fp381::zero()};
   out[i] = p;
   st[i] = (uint8_t)s;
@@ -427,9 +351,9 @@ int kzg_g2_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, const Bases
 
 // Miller values of n_pairs pairs (line set i, or i % period), then `count` checks over d_offsets
 int pairing_run(b200zk_ctx* ctx, const Affine<Fp381>* P, const BlsLine* lines, uint32_t period, const uint8_t* pst, size_t n_pairs,
-                const uint32_t* offsets, size_t count, Fp12b* f, uint8_t* result, uint8_t* status, cudaStream_t st) {
+                const uint32_t* offsets, size_t count, F12* f, uint8_t* result, uint8_t* status, cudaStream_t st) {
   if (n_pairs) B2_LAUNCH(ctx, bls_miller, (unsigned)((n_pairs + 31) / 32), 32, 0, st, P, lines, period, pst, n_pairs, f);
-  B2_LAUNCH(ctx, bls_pairing_final, (unsigned)((count + 31) / 32), 32, 0, st, (const Fp12b*)f, pst, offsets, count, result, status);
+  B2_LAUNCH(ctx, (pairing_check<F12, final_exponentiate>), (unsigned)((count + 31) / 32), 32, 0, st, (const F12*)f, pst, offsets, count, result, status);
   return B200ZK_OK;
 }
 
@@ -491,11 +415,11 @@ int b200zk_bls12_381_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, 
   Affine<Fp381>* P;
   Affine<F2>* Q;
   BlsLine* lines;
-  Fp12b* f;
+  F12* f;
   uint32_t* offs;
   B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     in = c.take<uint8_t>(384 * n); P = c.take<Affine<Fp381>>(n); Q = c.take<Affine<F2>>(n); pst = c.take<uint8_t>(n);
-    lines = c.take<BlsLine>(kLines * n); f = c.take<Fp12b>(n); offs = c.take<uint32_t>(count + 1); res = c.take<uint8_t>(count); sts = c.take<uint8_t>(count);
+    lines = c.take<BlsLine>(kLines * n); f = c.take<F12>(n); offs = c.take<uint32_t>(count + 1); res = c.take<uint8_t>(count); sts = c.take<uint8_t>(count);
   }));
   if (n) B2_CUDA(ctx, cudaMemcpyAsync(in, pairs, 384 * n, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(offs, pair_offsets, (count + 1) * 4, cudaMemcpyHostToDevice, st));
@@ -522,11 +446,11 @@ int b200zk_kzg_verify_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const uint
   cudaStream_t st = ctx->stream;
   uint8_t *in, *zb, *yb, *pt_st, *pst, *res, *sts;
   Affine<Fp381>*pts, *P;
-  Fp12b* f;
+  F12* f;
   uint32_t* offs;
   B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     in = c.take<uint8_t>(96 * n); zb = c.take<uint8_t>(32 * n); yb = c.take<uint8_t>(32 * n); pts = c.take<Affine<Fp381>>(2 * n);
-    pt_st = c.take<uint8_t>(2 * n); P = c.take<Affine<Fp381>>(2 * n); pst = c.take<uint8_t>(2 * n); f = c.take<Fp12b>(2 * n);
+    pt_st = c.take<uint8_t>(2 * n); P = c.take<Affine<Fp381>>(2 * n); pst = c.take<uint8_t>(2 * n); f = c.take<F12>(2 * n);
     offs = c.take<uint32_t>(n + 1); res = c.take<uint8_t>(n); sts = c.take<uint8_t>(n);
   }));
   std::vector<uint32_t> h_offs(n + 1);
@@ -559,12 +483,12 @@ int b200zk_kzg_verify_blob_proof_batch(b200zk_ctx* ctx, uint64_t g2_setup, const
   uint8_t *d_blobs, *zb, *q, *yb, *in, *pt_st, *rho, *pst, *res, *sts;
   Affine<Fp381>*pts, *P;
   XYZZ<Fp381>* terms;
-  Fp12b* f;
+  F12* f;
   uint32_t* offs;
   B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(kBlob * n); zb = c.take<uint8_t>(32 * n); q = c.take<uint8_t>(kBlob * n); yb = c.take<uint8_t>(32 * n);
     in = c.take<uint8_t>(96 * n); pts = c.take<Affine<Fp381>>(2 * n); pt_st = c.take<uint8_t>(2 * n); rho = c.take<uint8_t>(32);
-    terms = c.take<XYZZ<Fp381>>(2 * n); P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<Fp12b>(2);
+    terms = c.take<XYZZ<Fp381>>(2 * n); P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<F12>(2);
     offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
   }));
   char msg[160];
@@ -643,14 +567,14 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   Affine<F2>* q2;
   XYZZ<Fp381>* parts;
   BlsLine* lines;
-  Fp12b* f;
+  F12* f;
   uint32_t* offs;
   B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(kBlob * n); cells = c.take<uint8_t>(kExt * n); in = c.take<uint8_t>(48 * (n + m));
     pts = c.take<Affine<Fp381>>(n + m); pt_st = c.take<uint8_t>(n + m); rbe = c.take<uint8_t>(32);
     weights = c.take<uint4>(2 * 65); partial = c.take<uint4>(2 * 64 * n); s_proof = c.take<uint4>(2 * m); s_lin = c.take<uint4>(2 * (n + m));
     s_setup = c.take<uint4>(2 * kN); parts = c.take<XYZZ<Fp381>>(3); q2 = c.take<Affine<F2>>(2); lines = c.take<BlsLine>(2 * kLines);
-    P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<Fp12b>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
+    P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<F12>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
   }));
   char msg[160];
   // 1. every blob element < r (c-kzg blob_to_polynomial inside compute_cells): an error, not a false

@@ -130,6 +130,15 @@ template <class F> B2_HD XYZZ<F> xyzz_scalar_mul(const uint32_t* k, const Affine
   return acc;
 }
 
+// the subgroup check r P = O (no endomorphism shortcuts), Order(j) = limb j of the group order r (8 little-endian limbs):
+// FrCfg::mod for BN254, bls_r_limb for BLS12-381.  Non-inlined: one copy per translation unit and group.
+template <uint32_t (*Order)(int), class F> __device__ __noinline__ bool in_subgroup(const Affine<F>& p) {
+  uint32_t k[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) k[j] = Order(j);
+  return xyzz_scalar_mul<F>(k, p).is_inf();
+}
+
 // curve constants in Montgomery form
 template <class F> struct CurveB;
 template <> struct CurveB<Fq> {

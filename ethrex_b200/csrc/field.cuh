@@ -526,6 +526,10 @@ struct Fq2 {
     Fq d = Fq::inv(Fq::add(Fq::sqr(a.c0), Fq::sqr(a.c1)));
     return {Fq::mul(a.c0, d), Fq::neg(Fq::mul(a.c1, d))};
   }
+  static B2_D Fq2 mul_xi(const Fq2& a) {  // (a0 + a1 u)(9 + u) = (9 a0 - a1) + (9 a1 + a0) u, xi of the BN254 tower
+    Fq2 t = dbl(dbl(dbl(a)));
+    return {Fq::sub(Fq::add(t.c0, a.c0), a.c1), Fq::add(Fq::add(t.c1, a.c1), a.c0)};
+  }
 };
 
 }  // namespace b200zk

@@ -10,12 +10,14 @@
 // One thread works on one item (a point pair, or one pairing of a check); a batch fills the machine.
 // Pairing: PLAIN ate pairing f_{T,Q}(P), T = t - 1 = 6x^2 (127 bits, no Frobenius correction lines), affine line
 // functions on the D-type twist (x', y') -> (x' w^2, y' w^3), tower Fq2 = Fq[u]/(u^2+1), Fq6 = Fq2[v]/(v^3 - xi),
-// Fq12 = Fq6[w]/(w^2 - v), xi = 9 + u; final exponentiation = conj(f)/f, then one generic power (p^6+1)/r.  A
+// Fq12 = Fq6[w]/(w^2 - v), xi = 9 + u (tower.cuh over Fq2); final exponentiation = conj(f)/f, then one generic power
+// (p^6+1)/r.  A
 // pairing CHECK asks whether the product is one, which every non-degenerate bilinear pairing on these groups
 // answers identically (ark: `Bn254::multi_pairing(..).0 == one`).  oracle/pyref_tower.py is the same algorithm in
 // Python; oracle/pyref.py holds an independent optimal-ate statement.
 #include "common.cuh"
 #include "curve.cuh"
+#include "tower.cuh"
 
 namespace b200zk {
 namespace {
@@ -29,82 +31,35 @@ __constant__ uint32_t kFinalExp[40] = {  // (p^6 + 1) / r, 1268 bits
     0xa5afdd17u, 0x051c6d1au, 0x19667af5u, 0xb37f6019u, 0x5084015bu, 0x150e578cu, 0xc23998e4u, 0xfbdea556u, 0xc52f5b83u, 0x000fd14cu};
 static constexpr int kFinalExpBits = 1268;
 
-struct Fq6 { Fq2 c0, c1, c2; };
-struct Fq12 { Fq6 c0, c1; };
+typedef Fp12<Fq2> Fq12;
+typedef TowerF2<Fq2> M2;  // the non-inlined Fq2 product and inverse
 
-// the tower is latency-bound single-thread code: keep ONE copy of each heavy routine
-__device__ __noinline__ Fq2 f2_mul(const Fq2& a, const Fq2& b) { return Fq2::mul(a, b); }
-__device__ __noinline__ Fq2 f2_inv(const Fq2& a) { return Fq2::inv(a); }
 B2_D Fq2 f2_scale(const Fq2& a, const Fq& k) { return {Fq::mul(a.c0, k), Fq::mul(a.c1, k)}; }
-B2_D Fq2 f2_mul_xi(const Fq2& a) {  // (a0 + a1 u)(9 + u) = (9 a0 - a1) + (9 a1 + a0) u
-  Fq2 t = Fq2::dbl(Fq2::dbl(Fq2::dbl(a)));
-  return {Fq::sub(Fq::add(t.c0, a.c0), a.c1), Fq::add(Fq::add(t.c1, a.c1), a.c0)};
-}
-
-B2_D Fq6 f6_zero() { return {Fq2::zero(), Fq2::zero(), Fq2::zero()}; }
-B2_D Fq6 f6_one() { return {Fq2::one(), Fq2::zero(), Fq2::zero()}; }
-B2_D Fq6 f6_add(const Fq6& a, const Fq6& b) { return {Fq2::add(a.c0, b.c0), Fq2::add(a.c1, b.c1), Fq2::add(a.c2, b.c2)}; }
-B2_D Fq6 f6_sub(const Fq6& a, const Fq6& b) { return {Fq2::sub(a.c0, b.c0), Fq2::sub(a.c1, b.c1), Fq2::sub(a.c2, b.c2)}; }
-B2_D Fq6 f6_neg(const Fq6& a) { return {Fq2::neg(a.c0), Fq2::neg(a.c1), Fq2::neg(a.c2)}; }
-B2_D Fq6 f6_mul_v(const Fq6& a) { return {f2_mul_xi(a.c2), a.c0, a.c1}; }
-__device__ __noinline__ Fq6 f6_mul(const Fq6& a, const Fq6& b) {
-  Fq2 t0 = f2_mul(a.c0, b.c0), t1 = f2_mul(a.c1, b.c1), t2 = f2_mul(a.c2, b.c2);
-  Fq6 r;
-  r.c0 = Fq2::add(t0, f2_mul_xi(Fq2::sub(Fq2::sub(f2_mul(Fq2::add(a.c1, a.c2), Fq2::add(b.c1, b.c2)), t1), t2)));
-  r.c1 = Fq2::add(Fq2::sub(Fq2::sub(f2_mul(Fq2::add(a.c0, a.c1), Fq2::add(b.c0, b.c1)), t0), t1), f2_mul_xi(t2));
-  r.c2 = Fq2::add(Fq2::sub(Fq2::sub(f2_mul(Fq2::add(a.c0, a.c2), Fq2::add(b.c0, b.c2)), t0), t2), t1);
-  return r;
-}
-__device__ __noinline__ Fq6 f6_inv(const Fq6& a) {
-  Fq2 A = Fq2::sub(f2_mul(a.c0, a.c0), f2_mul_xi(f2_mul(a.c1, a.c2)));
-  Fq2 B = Fq2::sub(f2_mul_xi(f2_mul(a.c2, a.c2)), f2_mul(a.c0, a.c1));
-  Fq2 C = Fq2::sub(f2_mul(a.c1, a.c1), f2_mul(a.c0, a.c2));
-  Fq2 F = Fq2::add(f2_mul(a.c0, A), f2_mul_xi(Fq2::add(f2_mul(a.c2, B), f2_mul(a.c1, C))));
-  Fq2 Fi = f2_inv(F);
-  return {f2_mul(A, Fi), f2_mul(B, Fi), f2_mul(C, Fi)};
-}
-
-B2_D Fq12 f12_one() { return {f6_one(), f6_zero()}; }
-__device__ __noinline__ Fq12 f12_mul(const Fq12& a, const Fq12& b) {
-  Fq6 t0 = f6_mul(a.c0, b.c0), t1 = f6_mul(a.c1, b.c1);
-  Fq12 r;
-  r.c1 = f6_sub(f6_sub(f6_mul(f6_add(a.c0, a.c1), f6_add(b.c0, b.c1)), t0), t1);
-  r.c0 = f6_add(t0, f6_mul_v(t1));
-  return r;
-}
-B2_D Fq12 f12_conj(const Fq12& a) { return {a.c0, f6_neg(a.c1)}; }
-__device__ __noinline__ Fq12 f12_inv(const Fq12& a) {
-  Fq6 t = f6_inv(f6_sub(f6_mul(a.c0, a.c0), f6_mul_v(f6_mul(a.c1, a.c1))));
-  return {f6_mul(a.c0, t), f6_neg(f6_mul(a.c1, t))};
-}
-B2_D bool f12_is_one(const Fq12& a) {
-  return a.c0.c0 == Fq2::one() && a.c0.c1.is_zero() && a.c0.c2.is_zero() && a.c1.c0.is_zero() && a.c1.c1.is_zero() && a.c1.c2.is_zero();
-}
 
 // l(P) = yP - (lam xP) w + (lam xT - yT) w^3, w^3 = v w
 B2_D Fq12 line_at(const Fq2& lam, const Fq2& xt, const Fq2& yt, const Affine<Fq>& p) {
   Fq12 l;
   l.c0 = {{p.y, Fq::zero()}, Fq2::zero(), Fq2::zero()};
-  l.c1 = {Fq2::neg(f2_scale(lam, p.x)), Fq2::sub(f2_mul(lam, xt), yt), Fq2::zero()};
+  l.c1 = {Fq2::neg(f2_scale(lam, p.x)), Fq2::sub(M2::mul(lam, xt), yt), Fq2::zero()};
   return l;
 }
 
 // f_{T,Q}(P); neither point is the identity, Q has order r (so no step meets an exceptional case: T < r)
 __device__ __noinline__ Fq12 miller_ate(const Affine<Fq2>& q, const Affine<Fq>& p) {
-  Fq12 f = f12_one();
+  Fq12 f = Fq12::one();
   Fq2 rx = q.x, ry = q.y;
   for (int i = kAteBits - 2; i >= 0; --i) {
-    Fq2 xx = f2_mul(rx, rx);
-    Fq2 lam = f2_mul(Fq2::add(Fq2::dbl(xx), xx), f2_inv(Fq2::dbl(ry)));
-    f = f12_mul(f12_mul(f, f), line_at(lam, rx, ry, p));
-    Fq2 nx = Fq2::sub(Fq2::sub(f2_mul(lam, lam), rx), rx);
-    ry = Fq2::sub(f2_mul(lam, Fq2::sub(rx, nx)), ry);
+    Fq2 xx = M2::mul(rx, rx);
+    Fq2 lam = M2::mul(Fq2::add(Fq2::dbl(xx), xx), M2::inv(Fq2::dbl(ry)));
+    f = Fq12::mul(Fq12::mul(f, f), line_at(lam, rx, ry, p));
+    Fq2 nx = Fq2::sub(Fq2::sub(M2::mul(lam, lam), rx), rx);
+    ry = Fq2::sub(M2::mul(lam, Fq2::sub(rx, nx)), ry);
     rx = nx;
     if ((kAteT[i >> 5] >> (i & 31)) & 1) {
-      lam = f2_mul(Fq2::sub(ry, q.y), f2_inv(Fq2::sub(rx, q.x)));
-      f = f12_mul(f, line_at(lam, rx, ry, p));
-      nx = Fq2::sub(Fq2::sub(f2_mul(lam, lam), rx), q.x);
-      ry = Fq2::sub(f2_mul(lam, Fq2::sub(rx, nx)), ry);
+      lam = M2::mul(Fq2::sub(ry, q.y), M2::inv(Fq2::sub(rx, q.x)));
+      f = Fq12::mul(f, line_at(lam, rx, ry, p));
+      nx = Fq2::sub(Fq2::sub(M2::mul(lam, lam), rx), q.x);
+      ry = Fq2::sub(M2::mul(lam, Fq2::sub(rx, nx)), ry);
       rx = nx;
     }
   }
@@ -112,11 +67,11 @@ __device__ __noinline__ Fq12 miller_ate(const Affine<Fq2>& q, const Affine<Fq>& 
 }
 
 __device__ __noinline__ Fq12 final_exponentiate(const Fq12& f) {
-  Fq12 b = f12_mul(f12_conj(f), f12_inv(f));  // f^(p^6 - 1)
-  Fq12 acc = f12_one();
+  Fq12 b = Fq12::mul(Fq12::conj(f), Fq12::inv(f));  // f^(p^6 - 1)
+  Fq12 acc = Fq12::one();
   for (int i = kFinalExpBits - 1; i >= 0; --i) {
-    acc = f12_mul(acc, acc);
-    if ((kFinalExp[i >> 5] >> (i & 31)) & 1) acc = f12_mul(acc, b);
+    acc = Fq12::mul(acc, acc);
+    if ((kFinalExp[i >> 5] >> (i & 31)) & 1) acc = Fq12::mul(acc, b);
   }
   return acc;
 }
@@ -200,13 +155,6 @@ __global__ void __launch_bounds__(64) g1_mul_batch(const uint8_t* pts, const uin
   status[i] = (uint8_t)s;
 }
 
-__device__ __noinline__ bool g2_in_subgroup(const Affine<Fq2>& q) {  // r * Q == identity
-  uint32_t k[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) k[j] = FrCfg::mod(j);
-  return xyzz_scalar_mul<Fq2>(k, q).is_inf();
-}
-
 // one thread per (G1, G2) pair: decode, validate, Miller loop.  f[pair] = 1 when either point is the identity.
 __global__ void __launch_bounds__(32) pairing_miller(const uint8_t* pairs, size_t n_pairs, Fq12* f, uint8_t* pair_status) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
@@ -215,31 +163,11 @@ __global__ void __launch_bounds__(32) pairing_miller(const uint8_t* pairs, size_
   Affine<Fq2> q;
   uint32_t sp = decode_g1(pairs + 192 * i, &p), sq = decode_g2(pairs + 192 * i + 64, &q);
   uint32_t s = (sp == B200ZK_ERR_NOT_IN_FIELD || sq == B200ZK_ERR_NOT_IN_FIELD) ? (uint32_t)B200ZK_ERR_NOT_IN_FIELD : (sp ? sp : sq);
-  if (!s && !q.is_inf() && !g2_in_subgroup(q)) s = B200ZK_ERR_NOT_ON_CURVE;  // G1 has cofactor 1: on the curve = in the group
-  Fq12 r = f12_one();
+  if (!s && !q.is_inf() && !in_subgroup<FrCfg::mod>(q)) s = B200ZK_ERR_NOT_ON_CURVE;  // G1 has cofactor 1: on the curve = in the group
+  Fq12 r = Fq12::one();
   if (!s && !p.is_inf() && !q.is_inf()) r = miller_ate(q, p);
   f[i] = r;
   pair_status[i] = (uint8_t)s;
-}
-
-// one thread per check: product of its pairs' Miller values, one final exponentiation
-__global__ void __launch_bounds__(32) pairing_final(const Fq12* f, const uint8_t* pair_status, const uint32_t* offsets, size_t count, uint8_t* result, uint8_t* status) {
-  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  uint32_t lo = offsets[i], hi = offsets[i + 1], s = 0;
-  for (uint32_t k = lo; k < hi; ++k) {  // a range error anywhere outranks a curve error (the wrapper checks ranges first)
-    uint32_t ps = pair_status[k];
-    if (ps == B200ZK_ERR_NOT_IN_FIELD) s = ps;
-    else if (ps && !s) s = ps;
-  }
-  uint32_t ok = 0;
-  if (!s) {
-    Fq12 acc = f12_one();
-    for (uint32_t k = lo; k < hi; ++k) acc = f12_mul(acc, f[k]);
-    ok = (hi == lo) ? 1u : (f12_is_one(final_exponentiate(acc)) ? 1u : 0u);
-  }
-  result[i] = (uint8_t)ok;
-  status[i] = (uint8_t)s;
 }
 
 }  // namespace
@@ -291,7 +219,7 @@ int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint3
   if (n_pairs) B2_CUDA(ctx, cudaMemcpyAsync(in, pairs, n_pairs * 192, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemcpyAsync(offs, pair_offsets, (count + 1) * 4, cudaMemcpyHostToDevice, st));
   if (n_pairs) B2_LAUNCH(ctx, pairing_miller, (unsigned)((n_pairs + 31) / 32), 32, 0, st, in, n_pairs, f, pst);
-  B2_LAUNCH(ctx, pairing_final, (unsigned)((count + 31) / 32), 32, 0, st, (const Fq12*)f, pst, (const uint32_t*)offs, count, res, sts);
+  B2_LAUNCH(ctx, (pairing_check<Fq12, final_exponentiate>), (unsigned)((count + 31) / 32), 32, 0, st, (const Fq12*)f, pst, (const uint32_t*)offs, count, res, sts);
   B2_CUDA(ctx, cudaMemcpyAsync(result, res, count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(status, sts, count, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));

@@ -1,5 +1,6 @@
 // field_conformance.cu -- test-only harness: every field and curve primitive of the product headers, one element per
-// thread, so tests/test_gpu_field_conformance.py can compare each of them with Python integers at its limb edges.
+// thread, so tests/test_gpu_field_conformance.py can compare each of them with Python integers at its limb edges; the
+// pairing towers of tower.cuh op by op the same way.
 // Not part of libb200zk.so; ethrex_b200/csrc/Makefile builds it with the product's own nvcc flags, so the code under
 // test is generated exactly as the library's is.
 //
@@ -16,6 +17,7 @@
 #include "bls381.cuh"
 #include "common.cuh"
 #include "bls12.cuh"
+#include "tower.cuh"
 #include "secp256k1.cuh"
 
 using namespace b200zk;
@@ -24,7 +26,8 @@ namespace {
 
 // type ids
 enum : int { T_FQ = 0, T_FR = 1, T_FQ2 = 2, T_FP381 = 3, T_FR381 = 4, T_FP2_381 = 5, T_SECP_FP = 6, T_SECP_FN = 7, T_BYTES = 8,
-             T_BN_G1 = 10, T_BN_G2 = 11, T_BLS_G1 = 12, T_BLS_G2 = 13, T_SECP_G = 14 };
+             T_BN_G1 = 10, T_BN_G2 = 11, T_BLS_G1 = 12, T_BLS_G2 = 13, T_SECP_G = 14,
+             T_BN_FP6 = 15, T_BN_FP12 = 16, T_BLS_FP6 = 17, T_BLS_FP12 = 18 };
 // field op ids
 enum : int { ADD = 0, SUB, NEG, DBL, MUL, SQR, MUL2_ADD, MUL2_SUB, MUL4_ADD, TO_MONT, FROM_MONT, INV, POW, LESS, SQRT, CONJ,
              MUL_XI, SCALE, N_FIELD_OPS };
@@ -32,6 +35,9 @@ enum : int { ADD = 0, SUB, NEG, DBL, MUL, SQR, MUL2_ADD, MUL2_SUB, MUL4_ADD, TO_
 enum : int { LOAD_BE48 = 0, LOAD_BE48_MASKED, STORE_BE48, LOAD_FP64, LOAD_BE32, LOAD_BE256, STORE_BE256, N_BYTE_OPS };
 // curve op ids: XYZZ points are x | y | zz | zzz, affine points x | y, scalars 8 little-endian limbs
 enum : int { C_ADD = 0, C_ADD_MIXED, C_DBL, C_MDBL, C_TO_AFFINE, C_SCALAR_MUL, C_ON_CURVE, N_CURVE_OPS };
+// tower op ids (tower.cuh): the sparse products' F2 operands follow the tower element
+enum : int { X_ZERO = 0, X_ONE, X_ADD, X_SUB, X_NEG, X_MUL_V, X_MUL, X_SQR, X_CONJ, X_INV, X_IS_ONE, X_MUL_01, X_MUL_1, X_MUL_014,
+             N_TOWER_OPS };
 
 template <class T> __device__ T ld(const uint32_t* p) { T t; memcpy(&t, p, sizeof(T)); return t; }
 template <class T> __device__ void st(uint32_t* p, const T& t) { memcpy(p, &t, sizeof(T)); }
@@ -78,6 +84,7 @@ __global__ void fq2_kernel(int op, const uint32_t* in, uint32_t iw, uint32_t* ou
     case SQR: st(out, Fq2::sqr(x(0))); break;
     case MUL2_SUB: st(out, Fq2::mul2_sub(x(0), x(1), x(2), x(3))); break;
     case INV: st(out, Fq2::inv(x(0))); break;
+    case MUL_XI: st(out, Fq2::mul_xi(x(0))); break;
   }
 }
 
@@ -194,6 +201,48 @@ template <class F> __global__ void curve_kernel(int op, const uint32_t* in, uint
   }
 }
 
+// Fp6<F2> and Fp12<F2>; IS_ONE writes 1 / 0
+template <class F2> __global__ void fp6_kernel(int op, const uint32_t* in, uint32_t iw, uint32_t* out, uint32_t ow, uint64_t n) {
+  typedef Fp6<F2> E;
+  const uint64_t i = item();
+  if (i >= n) return;
+  in += i * iw; out += i * ow;
+  constexpr uint32_t W = words<E>();
+  auto x = [&](int k) { return ld<E>(in + k * W); };
+  auto y = [&](int k) { return ld<F2>(in + W + k * words<F2>()); };
+  switch (op) {
+    case X_ZERO: st(out, E::zero()); break;
+    case X_ONE: st(out, E::one()); break;
+    case X_ADD: st(out, E::add(x(0), x(1))); break;
+    case X_SUB: st(out, E::sub(x(0), x(1))); break;
+    case X_NEG: st(out, E::neg(x(0))); break;
+    case X_MUL_V: st(out, E::mul_v(x(0))); break;
+    case X_MUL: st(out, E::mul(x(0), x(1))); break;
+    case X_INV: st(out, E::inv(x(0))); break;
+    case X_MUL_01: st(out, E::mul_01(x(0), y(0), y(1))); break;
+    case X_MUL_1: st(out, E::mul_1(x(0), y(0))); break;
+  }
+}
+
+template <class F2> __global__ void fp12_kernel(int op, const uint32_t* in, uint32_t iw, uint32_t* out, uint32_t ow, uint64_t n) {
+  typedef Fp12<F2> E;
+  const uint64_t i = item();
+  if (i >= n) return;
+  in += i * iw; out += i * ow;
+  constexpr uint32_t W = words<E>();
+  auto x = [&](int k) { return ld<E>(in + k * W); };
+  auto y = [&](int k) { return ld<F2>(in + W + k * words<F2>()); };
+  switch (op) {
+    case X_ONE: st(out, E::one()); break;
+    case X_MUL: st(out, E::mul(x(0), x(1))); break;
+    case X_SQR: st(out, E::sqr(x(0))); break;
+    case X_CONJ: st(out, E::conj(x(0))); break;
+    case X_INV: st(out, E::inv(x(0))); break;
+    case X_IS_ONE: out[0] = E::is_one(x(0)) ? 1u : 0u; break;
+    case X_MUL_014: st(out, E::mul_014(x(0), y(0), y(1), y(2))); break;
+  }
+}
+
 constexpr uint32_t bits(std::initializer_list<int> ops) {
   uint32_t m = 0;
   for (int o : ops) m |= 1u << o;
@@ -205,7 +254,7 @@ uint32_t supported(int type) {
   switch (type) {
     case T_FQ: case T_FR:
       return bits({ADD, SUB, NEG, DBL, MUL, SQR, MUL2_ADD, MUL2_SUB, MUL4_ADD, TO_MONT, FROM_MONT, INV, POW});
-    case T_FQ2: return bits({ADD, SUB, NEG, DBL, MUL, SQR, MUL2_SUB, INV});
+    case T_FQ2: return bits({ADD, SUB, NEG, DBL, MUL, SQR, MUL2_SUB, INV, MUL_XI});
     case T_FP381: return bits({ADD, SUB, NEG, DBL, MUL, SQR, MUL2_SUB, TO_MONT, FROM_MONT, INV, POW, LESS, SQRT});
     case T_FR381: return bits({ADD, SUB, NEG, DBL, MUL, SQR, MUL2_SUB, TO_MONT, FROM_MONT, INV, POW, LESS});
     case T_FP2_381: return bits({ADD, SUB, NEG, DBL, CONJ, MUL, SQR, MUL_XI, SCALE, MUL2_SUB, INV, POW, SQRT});
@@ -213,6 +262,8 @@ uint32_t supported(int type) {
     case T_SECP_FN: return bits({NEG, MUL, TO_MONT, FROM_MONT, INV});
     case T_BYTES: return (1u << N_BYTE_OPS) - 1;
     case T_BN_G1: case T_BN_G2: case T_BLS_G1: case T_BLS_G2: case T_SECP_G: return (1u << N_CURVE_OPS) - 1;
+    case T_BN_FP6: case T_BLS_FP6: return bits({X_ZERO, X_ONE, X_ADD, X_SUB, X_NEG, X_MUL_V, X_MUL, X_INV, X_MUL_01, X_MUL_1});
+    case T_BN_FP12: case T_BLS_FP12: return bits({X_ONE, X_MUL, X_SQR, X_CONJ, X_INV, X_IS_ONE, X_MUL_014});
   }
   return 0;
 }
@@ -241,6 +292,10 @@ extern "C" int b200zk_conformance_run(int type, int op, const uint32_t* in, uint
     case T_BLS_G1: curve_kernel<Fp381><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
     case T_BLS_G2: curve_kernel<Fp2_381><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
     case T_SECP_G: curve_kernel<SecpFp><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
+    case T_BN_FP6: fp6_kernel<Fq2><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
+    case T_BN_FP12: fp12_kernel<Fq2><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
+    case T_BLS_FP6: fp6_kernel<Fp2_381><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
+    case T_BLS_FP12: fp12_kernel<Fp2_381><<<grid, block>>>(op, in, in_words, out, out_words, n); break;
   }
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaDeviceSynchronize();

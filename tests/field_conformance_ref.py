@@ -19,6 +19,7 @@ import secp256k1_ref
 # ---- ids of tests/csrc/field_conformance.cu ---------------------------------------------------------------------------
 T_FQ, T_FR, T_FQ2, T_FP381, T_FR381, T_FP2_381, T_SECP_FP, T_SECP_FN, T_BYTES = range(9)
 T_BN_G1, T_BN_G2, T_BLS_G1, T_BLS_G2, T_SECP_G = range(10, 15)
+T_BN_FP6, T_BN_FP12, T_BLS_FP6, T_BLS_FP12 = range(15, 19)
 OPS = ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_add", "mul2_sub", "mul4_add", "to_mont", "from_mont", "inv", "pow",
        "less", "sqrt", "conj", "mul_xi", "scale"]
 OP = {name: i for i, name in enumerate(OPS)}
@@ -26,6 +27,12 @@ BYTE_OPS = ["load_be48", "load_be48_masked", "store_be48", "load_fp64", "load_be
 BYTE_OP = {name: i for i, name in enumerate(BYTE_OPS)}
 CURVE_OPS = ["add", "add_mixed", "dbl", "mdbl", "to_affine", "scalar_mul", "on_curve"]
 CURVE_OP = {name: i for i, name in enumerate(CURVE_OPS)}
+TOWER_OPS = ["zero", "one", "add", "sub", "neg", "mul_v", "mul", "sqr", "conj", "inv", "is_one", "mul_01", "mul_1", "mul_014"]
+TOWER_OP = {name: i for i, name in enumerate(TOWER_OPS)}
+# the operands of each tower op: "x" a tower element, "f2" an element of the quadratic extension under it
+TOWER_OPERANDS = {"zero": [], "one": [], "add": ["x", "x"], "sub": ["x", "x"], "neg": ["x"], "mul_v": ["x"], "mul": ["x", "x"],
+                  "sqr": ["x"], "conj": ["x"], "inv": ["x"], "is_one": ["x"], "mul_01": ["x", "f2", "f2"], "mul_1": ["x", "f2"],
+                  "mul_014": ["x", "f2", "f2", "f2"]}
 # operands per op; pow's second operand is an exponent, scale's a base-field element
 ARITY = {"add": 2, "sub": 2, "neg": 1, "dbl": 1, "mul": 2, "sqr": 1, "mul2_add": 4, "mul2_sub": 4, "mul4_add": 8, "to_mont": 1,
          "from_mont": 1, "inv": 1, "pow": 2, "less": 2, "sqrt": 1, "conj": 1, "mul_xi": 1, "scale": 2}
@@ -59,10 +66,10 @@ class Prime:
 
 
 class Quad:
-    """base[u] / (u^2 + 1), elements (c0, c1) of raw base limbs."""
+    """base[u] / (u^2 + 1), elements (c0, c1) of raw base limbs; xi is the tower's non-residue, the factor of mul_xi."""
 
-    def __init__(self, name, tid, base):
-        self.name, self.tid, self.base = name, tid, base
+    def __init__(self, name, tid, base, xi):
+        self.name, self.tid, self.base, self.xi = name, tid, base, xi
         self.m, self.limbs, self.words = base.m, base.limbs, 2 * base.limbs
         self.zero, self.one = (0, 0), (1, 0)
 
@@ -93,10 +100,10 @@ class Quad:
 
 FQ = Prime("fq", T_FQ, pyref.P, 8)
 FR = Prime("fr", T_FR, pyref.R, 8)
-FQ2 = Quad("fq2", T_FQ2, FQ)
+FQ2 = Quad("fq2", T_FQ2, FQ, (9, 1))
 FP381 = Prime("fp381", T_FP381, bls_ref.P, 12)
 FR381 = Prime("fr381", T_FR381, bls_ref.R, 8)
-FP2_381 = Quad("fp2_381", T_FP2_381, FP381)
+FP2_381 = Quad("fp2_381", T_FP2_381, FP381, (1, 1))
 SECP_FP = Prime("secp_fp", T_SECP_FP, secp256k1_ref.P, 8, mont=False)
 SECP_FN = Prime("secp_fn", T_SECP_FN, secp256k1_ref.N, 8)
 PRIMES = [FQ, FR, FP381, FR381, SECP_FP, SECP_FN]
@@ -105,7 +112,7 @@ QUADS = [FQ2, FP2_381]
 # the ops of each type, as the harness implements them
 TYPE_OPS = {
     "fq": ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_add", "mul2_sub", "mul4_add", "to_mont", "from_mont", "inv", "pow"],
-    "fq2": ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_sub", "inv"],
+    "fq2": ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_sub", "inv", "mul_xi"],
     "fp381": ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_sub", "to_mont", "from_mont", "inv", "pow", "less", "sqrt"],
     "fp2_381": ["add", "sub", "neg", "dbl", "conj", "mul", "sqr", "mul_xi", "scale", "mul2_sub", "inv", "pow", "sqrt"],
     "secp_fp": ["add", "sub", "neg", "dbl", "mul", "sqr", "mul2_sub", "inv", "pow", "sqrt"],
@@ -248,7 +255,7 @@ def expect(F, op, xs):
     elif op == "mul4_add": r = F.add(F.add(F.mul(v[0], v[1]), F.mul(v[2], v[3])), F.add(F.mul(v[4], v[5]), F.mul(v[6], v[7])))
     elif op == "inv": r = F.inv(v[0])
     elif op == "conj": r = (v[0][0], F.base.neg(v[0][1]))
-    elif op == "mul_xi": r = F.mul(v[0], (1, 1))
+    elif op == "mul_xi": r = F.mul(v[0], F.xi)
     elif op == "sqrt":
         if isinstance(F, Quad):
             r = fp2_sqrt_candidate(F, v[0])
@@ -260,6 +267,118 @@ def expect(F, op, xs):
     else:
         raise KeyError(op)
     return F.enc(r)
+
+
+# ---- the pairing towers ---------------------------------------------------------------------------------------------
+class Ext:
+    """base[t] / (t^n - nr), elements n-tuples of base elements, products by schoolbook polynomial arithmetic: Fp6 =
+    F2[v] / (v^3 - xi) over a Quad, Fp12 = Fp6[w] / (w^2 - v) over that.  `quad` is the F2 at the bottom."""
+
+    def __init__(self, name, tid, base, n, nr):
+        self.name, self.tid, self.base, self.n, self.nr = name, tid, base, n, nr
+        self.quad = base if isinstance(base, Quad) else base.quad
+        self.m, self.limbs, self.words = base.m, base.limbs, n * base.words
+        self.zero = (base.zero,) * n
+        self.one = (base.one,) + (base.zero,) * (n - 1)
+
+    def add(self, a, b): return tuple(self.base.add(x, y) for x, y in zip(a, b))
+    def sub(self, a, b): return tuple(self.base.sub(x, y) for x, y in zip(a, b))
+    def neg(self, a): return tuple(self.base.neg(x) for x in a)
+    def mul(self, a, b):
+        B, n = self.base, self.n
+        c = [B.zero] * (2 * n - 1)
+        for i in range(n):
+            for j in range(n):
+                c[i + j] = B.add(c[i + j], B.mul(a[i], b[j]))
+        for k in range(2 * n - 2, n - 1, -1):  # t^k = nr t^(k - n)
+            c[k - n] = B.add(c[k - n], B.mul(c[k], self.nr))
+        return tuple(c[:n])
+    def is_zero(self, a): return a == self.zero
+
+    def enc(self, v): return tuple(self.base.enc(x) for x in v)
+    def dec(self, x): return tuple(self.base.dec(c) for c in x)
+    def flat(self, x): return [w for c in x for w in self.base.flat(c)]
+    def unflat(self, xs):
+        k = len(xs) // self.n
+        return tuple(self.base.unflat(xs[i * k:(i + 1) * k]) for i in range(self.n))
+    def canonical(self, x): return all(self.base.canonical(c) for c in x)
+
+
+def _tower(prefix, tid6, tid12, F2):
+    f6 = Ext(prefix + "_fp6", tid6, F2, 3, F2.xi)
+    return f6, Ext(prefix + "_fp12", tid12, f6, 2, (F2.zero, F2.one, F2.zero))  # w^2 = v
+
+
+BN_FP6, BN_FP12 = _tower("bn254", T_BN_FP6, T_BN_FP12, FQ2)
+BLS_FP6, BLS_FP12 = _tower("bls12_381", T_BLS_FP6, T_BLS_FP12, FP2_381)
+TOWERS = [BN_FP6, BN_FP12, BLS_FP6, BLS_FP12]
+TOWER_TYPE_OPS = {6: ["zero", "one", "add", "sub", "neg", "mul_v", "mul", "inv", "mul_01", "mul_1"],
+                  12: ["one", "mul", "sqr", "conj", "inv", "is_one", "mul_014"]}
+
+
+def tower_ops(T):
+    return TOWER_TYPE_OPS[6 if T.n == 3 else 12]
+
+
+def base_coords(T):
+    """the number of base-field coordinates of a tower element"""
+    return T.words // T.limbs
+
+
+def tower_edges(T):
+    """raw tower elements: zero, one, every base coordinate at one edge of edges(), the edges spread over the coordinates,
+    and elements with all but one top-level component zero"""
+    P = T.quad.base
+    es, k = edges(P), base_coords(T)
+    zero = T.unflat([0] * k)
+    out = [zero, T.enc(T.one)]
+    out += [T.unflat([e] * k) for e in es[1:]]
+    out += [T.unflat([es[(i + j) % len(es)] for j in range(k)]) for i in range(len(es))]
+    part = k // T.n
+    for c in range(T.n):  # component c only, its coordinates at the edges
+        for i in range(0, len(es), 4):
+            out.append(T.unflat([es[(i + j) % len(es)] if c * part <= j < (c + 1) * part else 0 for j in range(k)]))
+    return list(dict.fromkeys(out))
+
+
+def random_tower(rng, T, count):
+    """random raw tower elements: uniform and structured coordinates, a fifth of them with one zero component"""
+    P = T.quad.base
+    k, part = base_coords(T), base_coords(T) // T.n
+    cols = [random_raw(rng, P, P.m, count) for _ in range(k)]
+    for c in cols:
+        rng.shuffle(c)
+    out = []
+    for i in range(count):
+        coords = [c[i] for c in cols]
+        if i % 5 == 0:
+            z = rng.randrange(T.n)
+            coords[z * part:(z + 1) * part] = [0] * part
+        out.append(T.unflat(coords))
+    return out
+
+
+def tower_expect(T, op, xs):
+    """the raw result of a tower op on raw operands (an int for is_one); inv has no expected value (see the test)"""
+    if op == "zero": return T.enc(T.zero)
+    if op == "one": return T.enc(T.one)
+    F2 = T.quad
+    v = [T.dec(x) if k == "x" else F2.dec(x) for k, x in zip(TOWER_OPERANDS[op], xs)]
+    if op == "add": r = T.add(v[0], v[1])
+    elif op == "sub": r = T.sub(v[0], v[1])
+    elif op == "neg": r = T.neg(v[0])
+    elif op == "mul": r = T.mul(v[0], v[1])
+    elif op == "sqr": r = T.mul(v[0], v[0])
+    elif op == "mul_v": r = T.mul(v[0], (F2.zero, F2.one, F2.zero))
+    elif op == "conj": r = (v[0][0], T.base.neg(v[0][1]))
+    elif op == "is_one": return int(v[0] == T.one)
+    elif op == "mul_01": r = T.mul(v[0], (v[1], v[2], F2.zero))
+    elif op == "mul_1": r = T.mul(v[0], (F2.zero, v[1], F2.zero))
+    elif op == "mul_014":  # c0 + c1 v + c4 v w
+        r = T.mul(v[0], ((v[1], v[2], F2.zero), (F2.zero, v[3], F2.zero)))
+    else:
+        raise KeyError(op)
+    return T.enc(r)
 
 
 # ---- limbs <-> numpy --------------------------------------------------------------------------------------------------

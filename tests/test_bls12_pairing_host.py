@@ -117,7 +117,7 @@ def test_python_verifier_over_the_known_tau_setup():
     assert not _verify(c, z, y, proof, B.g2_mul(TAU + 1, B.G2))
 
 
-@pytest.mark.parametrize("kernel", ["bls_pair_decode", "bls_g2_decode", "bls_g2_prepare", "bls_miller", "bls_pairing_final",
+@pytest.mark.parametrize("kernel", ["bls_pair_decode", "bls_g2_decode", "bls_g2_prepare", "bls_miller", "pairing_check",
                                     "bls_g1_decode_subgroup", "kzg_verify_combine", "kzg_blob_terms", "kzg_blob_fold"])
 def test_ptxas_lists_the_new_kernels(kernel):
     log = os.path.join(CSRC, "build", "bls_pairing.ptxas.log")

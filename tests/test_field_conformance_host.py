@@ -12,6 +12,7 @@ import pytest
 import bls_pairing_ref
 import field_conformance_ref as ref
 import pyref
+import pyref_tower
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -119,6 +120,38 @@ def test_quad_model_against_references():
     a = (rng.randrange(F.m), rng.randrange(F.m))
     assert F.dec(ref.expect(F, "pow", (F.enc(a), 5))) == bls_pairing_ref.f2_pow(a, 5)
     assert F.dec(ref.expect(F, "mul_xi", (F.enc(a),))) == bls_pairing_ref.f2_mul(a, (1, 1))
+    a = (rng.randrange(ref.FQ2.m), rng.randrange(ref.FQ2.m))
+    assert ref.FQ2.dec(ref.expect(ref.FQ2, "mul_xi", (ref.FQ2.enc(a),))) == pyref_tower.f2_mul_xi(a)
+
+
+def test_tower_model():
+    """the schoolbook towers against the Karatsuba formulas of oracle/pyref_tower.py (BN254) and their defining relations"""
+    rng = random.Random(12)
+    F6, F12 = ref.BN_FP6, ref.BN_FP12
+    r6 = lambda: tuple((rng.randrange(F6.m), rng.randrange(F6.m)) for _ in range(3))
+    for _ in range(20):
+        a, b = r6(), r6()
+        assert F6.mul(a, b) == pyref_tower.f6_mul(a, b)
+        assert F6.mul(a, pyref_tower.f6_inv(a)) == F6.one
+        A, B = (r6(), r6()), (r6(), r6())
+        assert F12.mul(A, B) == pyref_tower.f12_mul(A, B)
+        assert F12.mul(A, pyref_tower.f12_inv(A)) == F12.one
+    for T6, T12 in [(ref.BN_FP6, ref.BN_FP12), (ref.BLS_FP6, ref.BLS_FP12)]:
+        F2 = T6.quad
+        o, z = F2.one, F2.zero
+        v, w = (z, o, z), (T6.zero, T6.one)
+        assert T6.mul(T6.mul(v, v), v) == (F2.xi, z, z)  # v^3 = xi
+        assert T12.mul(w, w) == (v, T6.zero)  # w^2 = v
+        a = tuple((rng.randrange(T6.m), rng.randrange(T6.m)) for _ in range(3))
+        A = (a, T6.neg(a))
+        assert T6.dec(ref.tower_expect(T6, "mul_v", (T6.enc(a),))) == T6.mul(a, v)
+        assert T12.dec(ref.tower_expect(T12, "conj", (T12.enc(A),))) == (a, a)
+        assert ref.tower_expect(T12, "is_one", (T12.enc(T12.one),)) == 1 and ref.tower_expect(T12, "is_one", (T12.enc(A),)) == 0
+    for T in ref.TOWERS:
+        es = ref.tower_edges(T)
+        assert len(set(es)) == len(es) and all(T.canonical(e) for e in es)
+        assert T.enc(T.zero) in es and T.enc(T.one) in es
+        assert ref.unpack_elems(T, ref.pack_elems(T, es)) == es
 
 
 def test_limb_packing_round_trip():
@@ -153,8 +186,9 @@ def test_harness_ids_match_model():
     assert [o.lower() for o in ops[:-1]] == ref.OPS and ops[-1] == "N_FIELD_OPS"
     assert [o.lower() for o in _enum(src, "LOAD_BE48")[:-1]] == ref.BYTE_OPS
     assert [o[2:].lower() for o in _enum(src, "C_ADD")[:-1]] == ref.CURVE_OPS
+    assert [o[2:].lower() for o in _enum(src, "X_ZERO")[:-1]] == ref.TOWER_OPS
     for name in ["T_FQ", "T_FR", "T_FQ2", "T_FP381", "T_FR381", "T_FP2_381", "T_SECP_FP", "T_SECP_FN", "T_BYTES", "T_BN_G1",
-                 "T_BN_G2", "T_BLS_G1", "T_BLS_G2", "T_SECP_G"]:
+                 "T_BN_G2", "T_BLS_G1", "T_BLS_G2", "T_SECP_G", "T_BN_FP6", "T_BN_FP12", "T_BLS_FP6", "T_BLS_FP12"]:
         assert re.search(rf"\b{name} = {getattr(ref, name)}\b", src), name
 
 

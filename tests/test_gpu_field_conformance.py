@@ -5,7 +5,9 @@ library's own nvcc flags); tests/field_conformance_ref.py holds the integer mode
 domain of each op.  Field ops compare bit for bit: binary ops over the full cross product of their edges plus 2^16 random
 pairs, wider ops over edge tuples plus 2^16 random tuples, exponentiations over their edges plus 2^12 random inputs.  Curve formulas compare with affine arithmetic, with the
 accumulators held in non-normalised XYZZ form (lam^2 x, lam^3 y, lam^2, lam^3) so that the exceptional branches compare
-different representations of one point.  A failure names the type, the op and the inputs in hex."""
+different representations of one point.  The pairing towers (Fp6, Fp12 of BN254 and BLS12-381) compare op by op with
+schoolbook products; an inverse is checked as a a^-1 = 1, with inv(0) = 0.  A failure names the type, the op and the inputs
+in hex."""
 import ctypes
 import itertools
 import os
@@ -25,6 +27,8 @@ N_RANDOM = 1 << 16
 # 2^10 over Fp2, where the Python model itself is a square-and-multiply per item
 N_RANDOM_EXP = 1 << 12
 N_RANDOM_SLOW = 1 << 10
+# tower products are dozens of Fp2 products each in the Python model: 2^12 random inputs, 2^10 for the inverses
+N_RANDOM_TOWER = 1 << 12
 
 
 @pytest.fixture(scope="module")
@@ -159,6 +163,52 @@ def test_field_op(harness, F, op):
             av = F.dec(a)
             is_square = av == (0, 0) or pow((av[0] ** 2 + av[1] ** 2) % F.m, (F.m - 1) // 2, F.m) == 1  # its norm is a square
             assert (F.mul(F.dec(r), F.dec(r)) == av) == is_square, f"{F.name} sqrt_candidate {hexs(a)} -> {hexs(r)}"
+
+
+# ---- pairing towers -----------------------------------------------------------------------------------------------------
+def tower_inputs(T, op, rng):
+    """operand tuples: the edges' cross product (binary ops), the edges with edge F2 operands (sparse products), then random
+    tuples; the constructors take one dummy item"""
+    kinds = ref.TOWER_OPERANDS[op]
+    if not kinds:
+        return [()]
+    E, Q = ref.tower_edges(T), ref.quad_edges(T.quad)
+    n_rand = N_RANDOM_SLOW if op == "inv" else N_RANDOM_TOWER
+    if kinds == ["x", "x"]:
+        items = list(itertools.product(E, E))
+    elif kinds == ["x"]:
+        items = [(a,) for a in E]
+    else:  # each tower edge with four tuples of F2 edges, walking through the F2 edges
+        nf = len(kinds) - 1
+        items = [(a,) + tuple(Q[((4 * i + r) * nf + k) % len(Q)] for k in range(nf)) for i, a in enumerate(E) for r in range(4)]
+    cols = [ref.random_tower(rng, T, n_rand) if k == "x" else ref.random_elem(rng, T.quad, T.m, n_rand) for k in kinds]
+    return items + list(zip(*cols))
+
+
+TOWER_CASES = [(T, op) for T in ref.TOWERS for op in ref.tower_ops(T)]
+
+
+@pytest.mark.parametrize("T,op", TOWER_CASES, ids=[f"{T.name}-{op}" for T, op in TOWER_CASES])
+def test_tower_op(harness, T, op):
+    rng = random.Random(f"{T.name}/{op}")
+    items = tower_inputs(T, op, rng)
+    kinds = ref.TOWER_OPERANDS[op]
+    cols = [ref.pack_elems(T if k == "x" else T.quad, [it[j] for it in items]) for j, k in enumerate(kinds)]
+    cols = cols or [np.zeros((len(items), 1), dtype=np.uint32)]
+    out = harness(T.tid, ref.TOWER_OP[op], cols, 1 if op == "is_one" else T.words)
+    if op == "is_one":
+        got = [int(v) for v in out[:, 0]]
+    else:
+        got = ref.unpack_elems(T, out)
+    if op == "inv":  # a a^-1 = 1, and inv(0) = 0
+        for (a,), r in zip(items, got):
+            av, rv = T.dec(a), T.dec(r)
+            assert (rv == T.zero) if av == T.zero else (T.mul(av, rv) == T.one), f"{T.name} inv {hexs(a)} -> {hexs(r)}"
+        assert T.zero in [T.dec(a) for (a,) in items]
+        return
+    assert_all_equal(f"{T.name} {op}", items, got, [ref.tower_expect(T, op, it) for it in items])
+    if op == "is_one":
+        assert 0 < sum(got) < len(got)
 
 
 # ---- byte formats -------------------------------------------------------------------------------------------------------

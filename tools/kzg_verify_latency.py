@@ -1,6 +1,6 @@
-"""Latency of KZG verification and the BLS12-381 pairing check on the device: b200zk_kzg_verify_proof_batch at n items,
-b200zk_kzg_verify_blob_proof_batch at n blobs, b200zk_bls12_381_pairing_check_batch with n two-pair checks.  Synthetic
-known-tau setup; every input is valid and every answer is checked.  Wall-clock per call (every call returns on the host
+"""Latency of KZG verification and the pairing checks on the device: b200zk_kzg_verify_proof_batch at n items,
+b200zk_kzg_verify_blob_proof_batch at n blobs, b200zk_bls12_381_pairing_check_batch and b200zk_bn254_pairing_check_batch
+with n two-pair checks e(P, Q) e(-P, Q) = 1.  Synthetic known-tau setup; every input is valid and every answer is checked.  Wall-clock per call (every call returns on the host
 with its results); medians over the steps after warm-up.  Prints one JSON line per case, with the card's name and power
 limit read in the same run.
 
@@ -21,6 +21,7 @@ import bls_pairing_ref as B  # noqa: E402
 import bls_ref as bls  # noqa: E402
 import ethrex_b200 as eb  # noqa: E402
 import kzg_ref as ref  # noqa: E402
+import pyref  # noqa: E402
 from kzg_proof_latency import gpu_identity, wall_ms  # noqa: E402
 
 TAU = 0x2F1B7C93D4A5E6F708192A3B4C5D6E7F8091A2B3C4D5E6F708192A3B4C5D6E7F % bls.R
@@ -64,6 +65,10 @@ def main():
     check = B.g1_eip2537(B.G1) + B.g2_eip2537(B.G2) + B.g1_eip2537(B.G1) + B.g2_eip2537(B.g2_neg(B.G2))
     for n in (1, 1024):
         emit("bls12_381_pairing_check_batch", n, timed(lambda: ctx.bls12_381_pairing_check_batch([check] * n), lambda o: o == ([1] * n, [0] * n), a.steps, a.warmup))
+    neg_g1 = (pyref.G1_GEN[0], pyref.P - pyref.G1_GEN[1])
+    bn_check = pyref.g1_to_be(pyref.G1_GEN) + pyref.g2_to_be(pyref.G2_GEN) + pyref.g1_to_be(neg_g1) + pyref.g2_to_be(pyref.G2_GEN)
+    for n in (1, 1024):
+        emit("bn254_pairing_check_batch", n, timed(lambda: ctx.bn254_pairing_check_batch([bn_check] * n), lambda o: o == ([1] * n, [0] * n), a.steps, a.warmup))
     ctx.bases_free(g1)
     ctx.bases_free(g2)
     ctx.close()
