@@ -120,6 +120,7 @@ SIGNATURES = {
     "b200zk_bls12_381_g2_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_secp256k1_ecrecover_batch": (_int, [_ctx, _vp, _vp, _sz, _u32, _vp, _vp]),
     "b200zk_secp256r1_verify_batch": (_int, [_ctx, _vp, _sz, _vp]),
+    "b200zk_modexp_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_g1_mul_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bn254_pairing_check_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

@@ -442,6 +442,33 @@ class Context:
         self._check(F.lib.b200zk_secp256r1_verify_batch(self._h, ip, count, res), "b200zk_secp256r1_verify_batch")
         return [b == 1 for b in res.raw[:count]]
 
+    # ------------------------------------------------------------------ modular exponentiation (MODEXP, precompile 0x05)
+    def modexp_batch(self, items):
+        """items: list of (base, exp, mod) big-endian byte strings, each up to 1024 bytes (EIP-7823) -> ([output],
+        [status]).  Item i's output is len(mod) bytes: (base mod m)^exp mod m, 1 mod m for exp = 0, all zero for m = 0
+        (Crypto::modexp).  status[i] = 2 and an all-zero output when an operand is longer than 1024 bytes."""
+        count = len(items)
+        lens = np.zeros(max(1, 3 * count), dtype=np.uint32)
+        parts = []
+        for i, ops in enumerate(items):
+            if len(ops) != 3:
+                raise B200Error.serialization("b200zk_modexp_batch: each item is (base, exp, mod)")
+            for j, op in enumerate(ops):
+                if len(op) > 0xffffffff:
+                    raise B200Error.serialization("b200zk_modexp_batch: an operand is longer than 2^32 - 1 bytes")
+                lens[3 * i + j] = len(op)
+                parts.append(bytes(op))
+        data = np.frombuffer(b"".join(parts) or b"\0", dtype=np.uint8)
+        mod_lens = [len(ops[2]) for ops in items]
+        out, st = C.create_string_buffer(max(1, sum(mod_lens))), C.create_string_buffer(max(1, count))
+        self._check(F.lib.b200zk_modexp_batch(self._h, data.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p), count, out, st),
+                    "b200zk_modexp_batch")
+        raw, outs, off = out.raw, [], 0
+        for n in mod_lens:
+            outs.append(raw[off:off + n])
+            off += n
+        return outs, list(st.raw[:count])
+
     def kzg_verify_proof_batch(self, g2_setup: int, commitments, z, y, proofs) -> tuple:
         """n items: commitments and proofs n x 48 bytes, z and y n x 32-byte big-endian -> ([result 0/1], [status])"""
         n = _host_len(commitments) // 48

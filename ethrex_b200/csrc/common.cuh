@@ -114,8 +114,8 @@ struct b200zk_ctx {
   b200zk::OnceTable kzg_roots, kzg_cells_tw, secp_gtab, p256_gtab;
   b200zk::DevBuf ws_kzg;      // EIP-4844 / EIP-7594 proofs and cells: blobs, z, quotients, partial sums and encoded results of one call
   b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
-                              // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu) and
-                              // P256VERIFY (secp256r1.cu) batches
+                              // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu),
+                              // P256VERIFY (secp256r1.cu) and MODEXP (modexp.cu: operand bytes, item list, outputs) batches
   int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};

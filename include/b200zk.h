@@ -482,6 +482,27 @@ int b200zk_secp256k1_ecrecover_batch(b200zk_ctx* ctx, const uint8_t* sigs /* cou
  * built on the device on the context's first call (256 KB, kept until b200zk_destroy). */
 int b200zk_secp256r1_verify_batch(b200zk_ctx* ctx, const uint8_t* inputs /* count*160 */, size_t count, uint8_t* result /* count */);
 
+/* ---- modular exponentiation (MODEXP) -------------------------------------------------------------------------------
+ * `count` independent items per call, HOST buffers:
+ *   modexp  Crypto::modexp, provider.rs:334-380 (levm MODEXP 0x05, precompiles.rs:559-643; gas at gas_cost.rs:831-900)
+ * Item i is base b | exponent e | modulus m, three big-endian byte strings of lens[3 i], lens[3 i + 1], lens[3 i + 2]
+ * bytes, stored back to back in `data` (item i + 1 starts where item i's modulus ends).  A length-0 operand is 0, and
+ * leading zero bytes change nothing but the output's length.  The output of item i is exactly len(m_i) bytes,
+ * big-endian, left-padded with zeros (pad_modexp_output, provider.rs:705-716), at offset len(m_0) + .. + len(m_(i-1))
+ * of `out`:
+ *   m = 0          all zero
+ *   e = 0          1 mod m (0 when m = 1)
+ *   otherwise      (b mod m)^e mod m
+ * status[i]: 0 ok; 2 an operand is longer than B200ZK_MODEXP_MAX_BYTES (EIP-7823, on the declared length, leading
+ * zeros included), and the output is all zero.  Items never affect each other.  Gas and the Osaka / pre-Osaka parsing
+ * of the calldata stay with the caller.
+ * count = 0 returns 0; null pointers, more than 2^32 - 1 items, or lengths whose sum overflows size_t return 4 with
+ * b200zk_last_error set.  Every operand is uploaded in one copy and every output comes back in one; see DESIGN section
+ * 4.14 for the size classes. */
+#define B200ZK_MODEXP_MAX_BYTES 1024u
+int b200zk_modexp_batch(b200zk_ctx* ctx, const uint8_t* data, const uint32_t* lens /* 3*count */, size_t count, uint8_t* out,
+                        uint8_t* status /* count */);
+
 /* ---- batched EIP-196 / EIP-197 precompile arithmetic (SURVEY.md section 8(f) rank 4) ------------------------------
  * The three BN254 calls of the reference's `Crypto` trait, `count` independent items per call, HOST buffers:
  *   bn254_g1_add         crates/common/crypto/provider.rs:201-234   (levm ecadd,     crates/vm/levm/src/precompiles.rs:692-716)

@@ -1,7 +1,7 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
 //! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`) and its
-//! BLS12-381 pairing check (`provider.rs:642-672`), its secp256k1 signer recovery (`provider.rs:63-171`) and its P-256
-//! signature verification (`provider.rs:415-459`) on the GPU.  The trait is one item per call; a provider that wants
+//! BLS12-381 pairing check (`provider.rs:642-672`), its secp256k1 signer recovery (`provider.rs:63-171`), its P-256
+//! signature verification (`provider.rs:415-459`) and its modular exponentiation (`provider.rs:334-380`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
 //!
@@ -9,9 +9,9 @@
 //! (`crates/vm/levm/src/precompiles.rs:801-820`, `PrecompileError::CoordinateExceedsFieldModulus`), the provider
 //! reports points off the curve as `CryptoError::InvalidPoint`.
 use ethrex_common::Address;
-use ethrex_crypto::{Crypto, CryptoError};
+use ethrex_crypto::{Crypto, CryptoError, NativeCrypto};
 
-use crate::ffi::{global, ItemStatus, RecoverStatus};
+use crate::ffi::{global, ItemStatus, RecoverStatus, MODEXP_MAX_BYTES};
 
 #[derive(Debug, Default, Clone, Copy)]
 pub struct B200Crypto;
@@ -83,7 +83,44 @@ pub fn verify_p256_batch(items: &[([u8; 32], [u8; 64], [u8; 64])]) -> Vec<bool> 
     }
 }
 
+/// MODEXP (precompile 0x05) for a block's calls in one device call.  Each item is what `Crypto::modexp` takes (base,
+/// exponent, modulus as big-endian bytes); the results are in item order, each exactly `modulus.len()` bytes.  Items
+/// with an operand over EIP-7823's 1024 bytes (possible only before Osaka) go to the reference's own
+/// `ethrex_crypto::NativeCrypto`: the device contract excludes them by design, and this is the only CPU path.  A device
+/// error fails every device item.
+pub fn modexp_batch(items: &[(&[u8], &[u8], &[u8])]) -> Vec<Result<Vec<u8>, CryptoError>> {
+    let over = |(b, e, m): &(&[u8], &[u8], &[u8])| b.len() > MODEXP_MAX_BYTES || e.len() > MODEXP_MAX_BYTES || m.len() > MODEXP_MAX_BYTES;
+    let bounded: Vec<(&[u8], &[u8], &[u8])> = items.iter().filter(|it| !over(*it)).copied().collect();
+    let device = global()
+        .map_err(device_error)
+        .and_then(|g| g.lock().map_err(device_error))
+        .and_then(|mut gpu| gpu.modexp_batch(&bounded).map_err(device_error));
+    let mut device = match device {
+        Ok(v) => v.into_iter().map(|r| r.ok_or_else(|| CryptoError::Other("b200zk refused a bounded modexp item".to_string()))).collect::<Vec<_>>().into_iter(),
+        Err(e) => bounded.iter().map(|_| Err(CryptoError::Other(e.to_string()))).collect::<Vec<_>>().into_iter(),
+    };
+    items
+        .iter()
+        .map(|it| {
+            if over(it) {
+                let (b, e, m) = it;
+                NativeCrypto.modexp(b, e, m)
+            } else {
+                device.next().unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
+            }
+        })
+        .collect()
+}
+
 impl Crypto for B200Crypto {
+    /// One item of [`modexp_batch`]: on the device up to EIP-7823's 1024-byte operands, `NativeCrypto` beyond.
+    fn modexp(&self, base: &[u8], exp: &[u8], modulus: &[u8]) -> Result<Vec<u8>, CryptoError> {
+        modexp_batch(&[(base, exp, modulus)])
+            .into_iter()
+            .next()
+            .unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
+    }
+
     /// The rules and their order are in include/b200zk.h (p256's `verify_prehash` as the reference calls it, EIP-7951).
     fn secp256r1_verify(&self, msg: &[u8; 32], sig: &[u8; 64], pk: &[u8; 64]) -> bool {
         verify_p256_batch(&[(*msg, *sig, *pk)]).first().copied().unwrap_or(false)

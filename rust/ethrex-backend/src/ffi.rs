@@ -20,6 +20,9 @@ unsafe impl Send for B200zk {}
 
 static GLOBAL: OnceLock<Result<Mutex<B200zk>, String>> = OnceLock::new();
 
+/// EIP-7823's bound on each MODEXP operand (`B200ZK_MODEXP_MAX_BYTES`); longer operands are not taken by the device.
+pub const MODEXP_MAX_BYTES: usize = 1024;
+
 /// Lazily initialised process-global context on the device selected by `CUDA_VISIBLE_DEVICES`.
 pub fn global() -> Result<&'static Mutex<B200zk>, BackendError> {
     GLOBAL
@@ -425,6 +428,37 @@ impl B200zk {
         let status = unsafe { sys::b200zk_secp256r1_verify_batch(self.ctx.as_ptr(), inputs.as_ptr(), count, res.as_mut_ptr()) };
         check(self, status)?;
         Ok(res.into_iter().map(|r| r == 1).collect())
+    }
+
+    /// `count` independent MODEXP items (precompile 0x05): `items[i]` = (base, exponent, modulus), big-endian byte
+    /// strings of any length.  Per item `Some(output)` of exactly `modulus.len()` bytes (`Crypto::modexp`'s value), or
+    /// `None` when an operand is longer than [`MODEXP_MAX_BYTES`] (EIP-7823), which the device does not take.
+    pub fn modexp_batch(&mut self, items: &[(&[u8], &[u8], &[u8])]) -> Result<Vec<Option<Vec<u8>>>, BackendError> {
+        let mut data = Vec::new();
+        let mut lens = Vec::with_capacity(items.len().saturating_mul(3));
+        let mut out_len = 0usize;
+        for (b, e, m) in items {
+            for op in [b, e, m] {
+                data.extend_from_slice(op);
+                lens.push(u32::try_from(op.len()).map_err(|_| BackendError::serialization("modexp_batch: an operand is longer than 2^32 - 1 bytes"))?);
+            }
+            out_len = out_len.checked_add(m.len()).ok_or_else(|| BackendError::serialization("modexp_batch: output length overflows"))?;
+        }
+        let count = items.len();
+        let mut out = vec![0u8; out_len];
+        let mut st = vec![0u8; count];
+        // SAFETY: `lens` holds 3 x count lengths whose operands are back to back in `data`, `out` the sum of the modulus
+        // lengths and `st` count bytes, all outliving the synchronous call.
+        let status = unsafe { sys::b200zk_modexp_batch(self.ctx.as_ptr(), data.as_ptr(), lens.as_ptr(), count, out.as_mut_ptr(), st.as_mut_ptr()) };
+        check(self, status)?;
+        let mut rest = out.as_slice();
+        let mut res = Vec::with_capacity(count);
+        for ((_, _, m), s) in items.iter().zip(st) {
+            let (head, tail) = rest.split_at(m.len().min(rest.len()));
+            rest = tail;
+            res.push(if s == 0 { Some(head.to_vec()) } else { None });
+        }
+        Ok(res)
     }
 
     fn bls12_381_add_batch(
