@@ -118,6 +118,8 @@ SIGNATURES = {
     "b200zk_bls12_381_g2_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g1_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g2_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_bls12_381_map_fp_to_g1_batch": (_int, [_ctx, _vp, _sz, _vp, _vp]),
+    "b200zk_bls12_381_map_fp2_to_g2_batch": (_int, [_ctx, _vp, _sz, _vp, _vp]),
     "b200zk_secp256k1_ecrecover_batch": (_int, [_ctx, _vp, _vp, _sz, _u32, _vp, _vp]),
     "b200zk_secp256r1_verify_batch": (_int, [_ctx, _vp, _sz, _vp]),
     "b200zk_modexp_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

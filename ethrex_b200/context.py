@@ -413,6 +413,25 @@ class Context:
         """calls: list of G2MSM calldata byte strings (k x 288 bytes each) -> ([256-byte output per call], [status])"""
         return self._bls12_msm(F.lib.b200zk_bls12_381_g2_msm_batch, "b200zk_bls12_381_g2_msm_batch", calls, 288, 256)
 
+    # Twins of Crypto::bls12_381_fp_to_g1 / _fp2_to_g2 (provider.rs:674-700), the map-to-curve precompiles 0x10 / 0x11
+    def _bls12_map(self, fn, what: str, data, size: int, out_size: int):
+        n = _host_len(data)
+        if n % size:
+            raise B200Error.serialization(f"{what}: input must be a multiple of {size} bytes")
+        count = n // size
+        out, st = C.create_string_buffer(max(1, out_size * count)), C.create_string_buffer(max(1, count))
+        pd, keep = _host_ptr(data)
+        self._check(fn(self._h, pd, count, out, st), what)
+        return out.raw[:out_size * count], list(st.raw[:count])
+
+    def bls12_381_map_fp_to_g1_batch(self, fps: bytes):
+        """fps: count x 64 bytes (EIP-2537 Fp) -> (count x 128 bytes of G1 points, [status])"""
+        return self._bls12_map(F.lib.b200zk_bls12_381_map_fp_to_g1_batch, "b200zk_bls12_381_map_fp_to_g1_batch", fps, 64, 128)
+
+    def bls12_381_map_fp2_to_g2_batch(self, fp2s: bytes):
+        """fp2s: count x 128 bytes (EIP-2537 Fp2, c0 | c1) -> (count x 256 bytes of G2 points, [status])"""
+        return self._bls12_map(F.lib.b200zk_bls12_381_map_fp2_to_g2_batch, "b200zk_bls12_381_map_fp2_to_g2_batch", fp2s, 128, 256)
+
     # ------------------------------------------------------------------ secp256k1 signer recovery (ECRECOVER)
     def secp256k1_ecrecover_batch(self, sigs, msgs, low_s: bool = False):
         """sigs: count x 65 bytes (r | s | recid), msgs: count x 32-byte hashes -> (count x 32 bytes, [status]).

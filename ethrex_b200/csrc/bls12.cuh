@@ -1,6 +1,6 @@
 // bls12.cuh -- BLS12-381 pieces shared by bls381.cu (commitments, proofs), bls_pairing.cu (the pairing, KZG verification)
-// and bls_ops.cu (EIP-2537 addition and MSM): big-endian byte loaders and stores, the 48-byte compressed G1 decoding, the
-// EIP-2537 64-byte field element, Fp2 = Fp[u]/(u^2 + 1) over Fp381 with Fq2's interface, so curve.cuh's XYZZ formulas (and
+// and bls_ops.cu / bls_map.cu (EIP-2537 addition, MSM and map-to-curve): big-endian byte loaders and stores, the 48-byte
+// compressed G1 decoding, the EIP-2537 64-byte field element and padded point, Fp2 = Fp[u]/(u^2 + 1) over Fp381 with Fq2's interface, so curve.cuh's XYZZ formulas (and
 // xyzz_scalar_mul and in_subgroup) instantiate over the twist unchanged, and the workspace carver of the pairing-family
 // calls.  The build has no -rdc: each translation unit keeps its own device copy of the __noinline__
 // functions, and `inline` lets the host linker merge their host-side stubs.
@@ -133,6 +133,28 @@ B2_D void store_be48(uint8_t* out, const Fp381& canonical) {
 #pragma unroll
   for (int k = 0; k < 12; ++k) w[11 - k] = __byte_perm(canonical.v[k], 0, 0x0123);
 }
+
+template <class F> B2_HD constexpr size_t fe_bytes() { return 64 * (sizeof(F) / sizeof(Fp381)); }  // EIP-2537 bytes of one coordinate
+template <class F> B2_HD constexpr size_t point_bytes() { return 2 * fe_bytes<F>(); }                // 128 (G1) / 256 (G2)
+
+// EIP-2537 coordinate -> Montgomery form; false on a nonzero padding byte or a value >= p
+B2_D bool load_fe64(const uint8_t* src, Fp381* out) {
+  Fp381 c;
+  const bool ok = load_fp64(src, &c);
+  *out = Fp381::to_mont(c);
+  return ok;
+}
+B2_D bool load_fe64(const uint8_t* src, Fp2_381* out) { return load_fe64(src, &out->c0) & load_fe64(src + 64, &out->c1); }
+
+B2_D void store_fe64(uint8_t* out, const Fp381& a) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(out);
+  w[0] = w[1] = w[2] = w[3] = 0;
+  store_be48(out + 16, Fp381::from_mont(a));
+}
+B2_D void store_fe64(uint8_t* out, const Fp2_381& a) { store_fe64(out, a.c0); store_fe64(out + 64, a.c1); }
+
+// the precompile's output: padded EIP-2537 coordinates, the identity (0, 0) as all-zero bytes
+template <class F> B2_D void store_point64(uint8_t* out, const Affine<F>& p) { store_fe64(out, p.x); store_fe64(out + fe_bytes<F>(), p.y); }
 
 // native affine -> the 48-byte compressed form, bls_g1_decompress's inverse; the identity is 0xc0 | 0..0 (out 4-byte aligned)
 B2_D void bls_g1_compress(uint8_t* out, const Affine<Fp381>& p) {

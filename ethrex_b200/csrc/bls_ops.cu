@@ -19,31 +19,10 @@ typedef Fp2_381 F2;
 
 constexpr int kFoldThreads = 64;  // XYZZ<F2> is 384 B: the fold tree of a G2 call holds 24 KB of shared memory
 
-template <class F> B2_HD constexpr size_t fe_bytes() { return 64 * (sizeof(F) / sizeof(Fp381)); }  // EIP-2537 bytes of one coordinate
-template <class F> B2_HD constexpr size_t point_bytes() { return 2 * fe_bytes<F>(); }                // 128 (G1) / 256 (G2)
 template <class F> B2_HD constexpr size_t pair_bytes() { return point_bytes<F>() + 32; }              // point | 32-byte big-endian scalar
-
-// EIP-2537 coordinate -> Montgomery form; false on a nonzero padding byte or a value >= p
-B2_D bool load_fe64(const uint8_t* src, Fp381* out) {
-  Fp381 c;
-  const bool ok = load_fp64(src, &c);
-  *out = Fp381::to_mont(c);
-  return ok;
-}
-B2_D bool load_fe64(const uint8_t* src, F2* out) { return load_fe64(src, &out->c0) & load_fe64(src + 64, &out->c1); }
 
 // both coordinates are range-checked whatever the first one gave, so status 2 never depends on the order of the checks
 template <class F> B2_D bool load_point64(const uint8_t* src, Affine<F>* p) { return load_fe64(src, &p->x) & load_fe64(src + fe_bytes<F>(), &p->y); }
-
-B2_D void store_fe64(uint8_t* out, const Fp381& a) {
-  uint32_t* w = reinterpret_cast<uint32_t*>(out);
-  w[0] = w[1] = w[2] = w[3] = 0;
-  store_be48(out + 16, Fp381::from_mont(a));
-}
-B2_D void store_fe64(uint8_t* out, const F2& a) { store_fe64(out, a.c0); store_fe64(out + 64, a.c1); }
-
-// the precompile's output: padded EIP-2537 coordinates, the identity (0, 0) as all-zero bytes
-template <class F> B2_D void store_point64(uint8_t* out, const Affine<F>& p) { store_fe64(out, p.x); store_fe64(out + fe_bytes<F>(), p.y); }
 
 // ---- kernels ----------------------------------------------------------------------------------------------------------
 // one thread per item: out[i] = a[i] + b[i].  Both points are range-checked (status 2) before either curve check (status 3)

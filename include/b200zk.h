@@ -442,6 +442,26 @@ int b200zk_bls12_381_g1_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 160 B
 int b200zk_bls12_381_g2_msm_batch(b200zk_ctx* ctx, const uint8_t* pairs /* 288 B each */, const uint32_t* pair_offsets /* count+1 */,
                                   size_t count, uint8_t* out /* count*256 */, uint8_t* status /* count */);
 
+/* ---- EIP-2537 map-to-curve ----------------------------------------------------------------------------------------
+ * The Prague precompiles 0x10 and 0x11, `count` independent items per call, HOST buffers:
+ *   bls12_381_map_fp_to_g1   Crypto::bls12_381_fp_to_g1, provider.rs:674-685 (levm BLS12_MAP_FP_TO_G1, precompiles.rs:1403-1431)
+ *   bls12_381_map_fp2_to_g2  Crypto::bls12_381_fp2_to_g2, provider.rs:688-700 (levm BLS12_MAP_FP2_TO_G2, precompiles.rs:1433-1479)
+ * Encodings as the addition and MSM calls: an input Fp is 64 bytes, 16 zero bytes then 48 bytes big-endian; an Fp2 is
+ * c0 | c1 (128 B).  The output is clear_cofactor(iso_map(map_to_curve_simple_swu(u))) of RFC 9380 (sections 6.6.2, 6.6.3
+ * and 7, BLS12-381 parameters of 8.8.1 and 8.8.2), as the bls12_381 crate computes it, written as the precompile's own
+ * return data: G1 = x | y (128 B), G2 = x.c0 | x.c1 | y.c0 | y.c1 (256 B).  The input (0, 0) of MAP_FP2_TO_G2 needs no
+ * special case: the call returns levm's FP2_ZERO_MAPPED_TO_G2 (precompiles.rs:44-60), which levm returns without calling
+ * the crate.
+ * The return value reports infrastructure errors only; input errors are per item in status[i]:
+ *   0 ok, 1 ok and the result is the identity (no field element reaches it; kept so the table is the other calls'),
+ *   2 a nonzero padding byte or a value >= p (for G2 in either component).
+ * A failed item's output is all zero; items never affect each other.  count = 0 returns 0; null pointers with count > 0
+ * return 4 with b200zk_last_error set. */
+int b200zk_bls12_381_map_fp_to_g1_batch(b200zk_ctx* ctx, const uint8_t* fps /* count*64 */, size_t count,
+                                        uint8_t* out /* count*128 */, uint8_t* status /* count */);
+int b200zk_bls12_381_map_fp2_to_g2_batch(b200zk_ctx* ctx, const uint8_t* fp2s /* count*128: c0 | c1 */, size_t count,
+                                         uint8_t* out /* count*256 */, uint8_t* status /* count */);
+
 /* ---- secp256k1 signer recovery (ECRECOVER) -------------------------------------------------------------------------
  * `count` independent items per call, HOST buffers:
  *   secp256k1_ecrecover  Crypto::secp256k1_ecrecover, provider.rs:63-88 (levm ECRECOVER 0x01, precompiles.rs:456-510)

@@ -146,6 +146,8 @@ unsafe extern "C" {
     pub fn b200zk_bls12_381_g2_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g1_msm_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g2_msm_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;
+    pub fn b200zk_bls12_381_map_fp_to_g1_batch(ctx: *mut b200zk_ctx, fps: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
+    pub fn b200zk_bls12_381_map_fp2_to_g2_batch(ctx: *mut b200zk_ctx, fp2s: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_secp256k1_ecrecover_batch(ctx: *mut b200zk_ctx, sigs: *const u8, msgs: *const u8, count: usize, flags: u32, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_secp256r1_verify_batch(ctx: *mut b200zk_ctx, inputs: *const u8, count: usize, result: *mut u8) -> c_int;
     pub fn b200zk_modexp_batch(ctx: *mut b200zk_ctx, data: *const u8, lens: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;

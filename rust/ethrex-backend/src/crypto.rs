@@ -1,6 +1,6 @@
 //! `B200Crypto`: the three BN254 calls of the reference's `Crypto` trait
-//! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`) and its
-//! BLS12-381 pairing check (`provider.rs:642-672`), its secp256k1 signer recovery (`provider.rs:63-171`), its P-256
+//! (`crates/common/crypto/provider.rs:201-330`), its EIP-2537 G1/G2 addition and MSM (`provider.rs:549-640`), its
+//! BLS12-381 pairing check (`provider.rs:642-672`) and map-to-curve (`provider.rs:674-700`), its secp256k1 signer recovery (`provider.rs:63-171`), its P-256
 //! signature verification (`provider.rs:415-459`) and its modular exponentiation (`provider.rs:334-380`) on the GPU.  The trait is one item per call; a provider that wants
 //! throughput collects the items of a block (or of the batch being proved) and calls the `*_batch` wrappers of
 //! [`crate::ffi::B200zk`] directly -- the single-item methods below are the drop-in form.
@@ -110,6 +110,57 @@ pub fn modexp_batch(items: &[(&[u8], &[u8], &[u8])]) -> Vec<Result<Vec<u8>, Cryp
             }
         })
         .collect()
+}
+
+/// MAP_FP_TO_G1 (precompile 0x10) for a block's calls in one device call.  Each item is what
+/// `Crypto::bls12_381_fp_to_g1` takes (a 48-byte big-endian field element); the results are in item order, each the
+/// trait's unpadded x | y.  A value >= p is `CryptoError::InvalidInput("invalid Fp element")`, as the provider reports it.
+pub fn map_fp_to_g1_batch(items: &[[u8; 48]]) -> Vec<Result<[u8; 96], CryptoError>> {
+    let mut input = Vec::with_capacity(items.len().saturating_mul(64));
+    for fp in items {
+        input.extend_from_slice(&pad_fps([fp]));
+    }
+    let res = global()
+        .map_err(device_error)
+        .and_then(|g| g.lock().map_err(device_error))
+        .and_then(|mut gpu| gpu.bls12_381_map_fp_to_g1_batch(&input).map_err(device_error));
+    map_results(res, items.len(), 128, unpad::<96>)
+}
+
+/// MAP_FP2_TO_G2 (precompile 0x11) for a block's calls in one device call.  Each item is what
+/// `Crypto::bls12_381_fp2_to_g2` takes (c0, c1 as 48-byte big-endian field elements); the results are in item order,
+/// each the trait's unpadded x.c0 | x.c1 | y.c0 | y.c1.  A component >= p is `CryptoError::InvalidInput`.
+///
+/// One divergence from the provider: (0, 0) maps to the correct point, levm's `FP2_ZERO_MAPPED_TO_G2`, where the
+/// bls12_381 crate's `map_to_curve` does not.  levm returns that constant before calling the trait, so only a direct
+/// caller of the trait sees the difference.
+pub fn map_fp2_to_g2_batch(items: &[([u8; 48], [u8; 48])]) -> Vec<Result<[u8; 192], CryptoError>> {
+    let mut input = Vec::with_capacity(items.len().saturating_mul(128));
+    for (c0, c1) in items {
+        input.extend_from_slice(&pad_fps([c0, c1]));
+    }
+    let res = global()
+        .map_err(device_error)
+        .and_then(|g| g.lock().map_err(device_error))
+        .and_then(|mut gpu| gpu.bls12_381_map_fp2_to_g2_batch(&input).map_err(device_error));
+    map_results(res, items.len(), 256, unpad::<192>)
+}
+
+/// The per-item results of a map-to-curve batch: status 2 is the provider's "invalid Fp element", a device error fails
+/// every item.
+fn map_results<T>(res: Result<(Vec<u8>, Vec<ItemStatus>), CryptoError>, count: usize, size: usize, decode: fn(&[u8]) -> T) -> Vec<Result<T, CryptoError>> {
+    match res {
+        Ok((out, st)) if st.len() == count => st
+            .into_iter()
+            .zip(out.chunks(size))
+            .map(|(s, bytes)| match s {
+                ItemStatus::Ok | ItemStatus::OkIdentity => Ok(decode(bytes)),
+                _ => Err(CryptoError::InvalidInput("invalid Fp element")),
+            })
+            .collect(),
+        Ok(_) => (0..count).map(|_| Err(CryptoError::Other("b200zk returned no result".to_string()))).collect(),
+        Err(e) => (0..count).map(|_| Err(CryptoError::Other(e.to_string()))).collect(),
+    }
 }
 
 impl Crypto for B200Crypto {
@@ -251,6 +302,16 @@ impl Crypto for B200Crypto {
             Some(Err(bad)) => Err(item_error(*bad, "G2 point not on curve or not in subgroup")),
             None => Err(CryptoError::Other("b200zk returned no result".to_string())),
         }
+    }
+
+    /// One item of [`map_fp_to_g1_batch`].
+    fn bls12_381_fp_to_g1(&self, fp: &[u8; 48]) -> Result<[u8; 96], CryptoError> {
+        map_fp_to_g1_batch(&[*fp]).into_iter().next().unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
+    }
+
+    /// One item of [`map_fp2_to_g2_batch`], including its (0, 0) divergence from the provider.
+    fn bls12_381_fp2_to_g2(&self, fp2: ([u8; 48], [u8; 48])) -> Result<[u8; 192], CryptoError> {
+        map_fp2_to_g2_batch(&[fp2]).into_iter().next().unwrap_or_else(|| Err(CryptoError::Other("b200zk returned no result".to_string())))
     }
 }
 

@@ -390,6 +390,18 @@ impl B200zk {
         self.bls12_381_msm_batch(calls, 288, 256, "bls12_381_g2_msm_batch", sys::b200zk_bls12_381_g2_msm_batch)
     }
 
+    /// `count` independent EIP-2537 MAP_FP_TO_G1 items: `fps` = count x 64 bytes.  Returns (count x 128 result bytes,
+    /// per-item status); a failed item's bytes are zero.
+    pub fn bls12_381_map_fp_to_g1_batch(&mut self, fps: &[u8]) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        self.bls12_381_map_batch(fps, 64, 128, "bls12_381_map_fp_to_g1_batch: input must be a multiple of 64 bytes", sys::b200zk_bls12_381_map_fp_to_g1_batch)
+    }
+
+    /// `count` independent EIP-2537 MAP_FP2_TO_G2 items: `fp2s` = count x 128 bytes (c0 | c1).  Returns (count x 256
+    /// result bytes, per-item status); a failed item's bytes are zero.
+    pub fn bls12_381_map_fp2_to_g2_batch(&mut self, fp2s: &[u8]) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        self.bls12_381_map_batch(fp2s, 128, 256, "bls12_381_map_fp2_to_g2_batch: input must be a multiple of 128 bytes", sys::b200zk_bls12_381_map_fp2_to_g2_batch)
+    }
+
     /// `count` independent ECRECOVER items: `sigs` = count x 65 bytes (r | s | recid, r and s big-endian), `msgs` =
     /// count x 32-byte hashes.  `low_s` rejects s > n/2 (EIP-2, as `Crypto::recover_signer`).  Per item
     /// `Ok(keccak256 of the recovered public key)` (the address is bytes 12..32) or its status.
@@ -477,6 +489,26 @@ impl B200zk {
         let mut st = vec![0u8; count];
         // SAFETY: all four buffers hold `count` items of the documented sizes and outlive the synchronous call.
         let status = unsafe { f(self.ctx.as_ptr(), a.as_ptr(), b.as_ptr(), count, out.as_mut_ptr(), st.as_mut_ptr()) };
+        check(self, status)?;
+        Ok((out, st.into_iter().map(ItemStatus::from_code).collect()))
+    }
+
+    fn bls12_381_map_batch(
+        &mut self,
+        input: &[u8],
+        size: usize,
+        out_size: usize,
+        what: &'static str,
+        f: unsafe extern "C" fn(*mut sys::b200zk_ctx, *const u8, usize, *mut u8, *mut u8) -> std::os::raw::c_int,
+    ) -> Result<(Vec<u8>, Vec<ItemStatus>), BackendError> {
+        if input.len() % size != 0 {
+            return Err(BackendError::serialization(what));
+        }
+        let count = input.len() / size;
+        let mut out = vec![0u8; count.saturating_mul(out_size)];
+        let mut st = vec![0u8; count];
+        // SAFETY: all three buffers hold `count` items of the documented sizes and outlive the synchronous call.
+        let status = unsafe { f(self.ctx.as_ptr(), input.as_ptr(), count, out.as_mut_ptr(), st.as_mut_ptr()) };
         check(self, status)?;
         Ok((out, st.into_iter().map(ItemStatus::from_code).collect()))
     }
