@@ -1,7 +1,8 @@
 """MODEXP on the device (b200zk_modexp_batch, precompile 0x05) against Python's `pow` (tests/modexp_ref.py): every size
-class edge, even moduli 2^s q and powers of two, the trivial operands in every combination, base reduction, Fermat
-identities for the curve primes, RSA-2048 / 4096 signatures, the 1024/1024/1024 worst case, a mixed batch against single
-calls, items over the EIP-7823 bound between valid neighbours, and the argument refusals and workspace sharing."""
+class edge, even moduli 2^s q and powers of two, carries and borrows through whole lanes, the trivial operands in every
+combination, base reduction, Fermat identities for the curve primes, RSA-2048 / 4096 signatures, the 1024/1024/1024 worst
+case, a mixed batch against single calls, items over the EIP-7823 bound between valid neighbours, and the argument
+refusals and workspace sharing."""
 import ctypes as C
 import itertools
 import random
@@ -57,6 +58,27 @@ def test_even_moduli(ctx):
         items.append((ref.rand_bytes(rng, 64), ref.rand_bytes(rng, 4), ref.be(m, (k + 8) // 8)))
         items.append((ref.be(3, 1), ref.rand_bytes(rng, 1), ref.be(m, (k + 8) // 8)))
     check(ctx, items)
+
+
+def test_lane_carry_items(ctx):
+    """items whose products send carries and borrows through whole lanes (the carry events of tests/bigmod_ref.py,
+    through the real kernel), in every class: m = 2^(32N) - 1 with base m - 1, whose Montgomery products reach t = R
+    and fold a carry through every lane; m = 2^(32N) - 2^32 + 1 with an all-ones base; and even moduli 2^s q with s on
+    lane boundaries, so that m >> s moves whole lanes, and q = 2^(32N - s) - 1 filling the class"""
+    rng = random.Random(12)
+    items = []
+    for bits in (256, 1024, 2048, 4096, 8192):
+        n = bits // 8
+        m = (1 << bits) - 1
+        items += [(ref.be(m - 1, n), b"\x02", ref.be(m, n)), (ref.be(m - 1, n), ref.rand_bytes(rng, 32), ref.be(m, n))]
+        items.append((b"\xff" * n, ref.rand_bytes(rng, 32), ref.be((1 << bits) - (1 << 32) + 1, n)))
+        for s in (256, 512, 1024, 4096):
+            if s < bits:
+                m = ((1 << (bits - s)) - 1) << s
+                for base in (ref.rand_bytes(rng, n), b"\xff" * n):
+                    items.append((base, ref.rand_bytes(rng, 16), ref.be(m, n)))
+    outs = check(ctx, items)
+    assert outs[0] == ref.be(1, 32)  # (m - 1)^2 = 1
 
 
 def test_trivial_operands_in_every_combination(ctx):
