@@ -626,10 +626,11 @@ int orc_fr_ntt(u64* data, unsigned log_n, unsigned flags, const u64* coset_gen, 
   return 0;
 }
 
-// out = sum_j a[j] * x^j with x = w_n^k (Horner, O(n)): the definition of output k of the forward transform.
-// Lets the tests spot-check transforms that are too large to run on the CPU in full.  Montgomery in/out.
-int orc_fr_ntt_eval_output(const u64* data, unsigned log_n, u64 k, u64* out) {
-  if (log_n > 28) return 4;
+// out = sum_{j < count} a[j] * x^(start + j) with x = w_n^k (Horner, O(count)): the share of coefficients
+// [start, start + count) in output k of the forward transform.  Summed over the chunks of a vector, it is the
+// definition of that output, so a transform too large to hold on the host can be spot-checked.  Montgomery in/out.
+int orc_fr_ntt_eval_output_chunk(const u64* data, size_t count, u64 start, unsigned log_n, u64 k, u64* out) {
+  if (log_n > 28 || start + count > ((u64)1 << log_n)) return 4;
   const Fr* a = (const Fr*)data;
   const size_t n = (size_t)1 << log_n;
   Fr w = fr_root_2_28();
@@ -642,17 +643,111 @@ int orc_fr_ntt_eval_output(const u64* data, unsigned log_n, u64 k, u64* out) {
 #endif
   std::vector<Fr> part(T, Fr::zero());
   std::vector<size_t> lo(T + 1);
-  for (int t = 0; t <= T; ++t) lo[t] = n * t / T;
+  for (int t = 0; t <= T; ++t) lo[t] = count * t / T;
 #pragma omp parallel for num_threads(T) schedule(static, 1)
   for (int t = 0; t < T; ++t) {
     Fr acc = Fr::zero();
     for (size_t j = lo[t + 1]; j-- > lo[t];) acc = acc * x + a[j];  // sum_{j in block} a[j] x^(j - lo)
-    part[t] = acc * fr_pow_u64(x, lo[t]);
+    part[t] = acc * fr_pow_u64(x, start + lo[t]);
   }
   Fr tot = Fr::zero();
   for (auto& p : part) tot = tot + p;
   memcpy(out, tot.v, 32);
   return 0;
+}
+int orc_fr_ntt_eval_output(const u64* data, unsigned log_n, u64 k, u64* out) {
+  if (log_n > 28) return 4;
+  return orc_fr_ntt_eval_output_chunk(data, (size_t)1 << log_n, 0, log_n, k, out);
+}
+
+// Whole-vector check of any transform orc_fr_ntt computes, O(n) and chunk by chunk.  Every mode has the form
+//   y_k = s * d^k * sum_j a_j c^j w^(e j k)
+//   forward: s = d = c = 1, e = +1;  inverse: s = 1/n, e = -1;  coset: c = h;  inverse coset: s = 1/n, d = 1/h, e = -1
+// so, for any z, summing the geometric series over k:
+//   sum_k y_k z^k = s ((dz)^n - 1) sum_j a_j c^j / (dz w^(e j) - 1).
+// The left side is one Horner pass, the right one batch inversion; both are exact in Fr, so a wrong output survives
+// only if z is a root of a nonzero polynomial of degree < n: probability <= n / r over z.
+struct NttIdentity {
+  Fr z, dz, step, c, s;  // step = w^e
+  size_t n;
+};
+static int ntt_identity_setup(unsigned log_n, unsigned flags, const u64* coset_gen, const u64* root_2_28, const u64* z_canonical, NttIdentity* p) {
+  if (log_n > 28) return 4;
+  p->n = (size_t)1 << log_n;
+  Fr g = root_2_28 ? Fr::from_canonical(root_2_28) : fr_root_2_28();
+  Fr w = g;
+  for (unsigned i = log_n; i < 28; ++i) w = w.sqr();
+  const bool inverse = flags & ORC_NTT_INVERSE, coset = flags & ORC_NTT_COSET;
+  Fr h = Fr::from_canonical((const u64[4]){5, 0, 0, 0});
+  if (coset_gen) h = Fr::from_canonical(coset_gen);
+  u64 zc[4];
+  memcpy(zc, z_canonical, 32);
+  reduce_mod_r(zc);
+  p->z = Fr::from_canonical(zc);
+  p->step = inverse ? w.inv() : w;
+  p->dz = (inverse && coset) ? p->z * h.inv() : p->z;
+  p->c = (!inverse && coset) ? h : Fr::one();
+  u64 nc[4] = {p->n, 0, 0, 0};
+  p->s = inverse ? Fr::from_canonical(nc).inv() : Fr::one();
+  return 0;
+}
+
+// acc[0..3] += sum_k y_k z^k and acc[4..7] += sum_j a_j c^j / (dz w^(e j) - 1) over indices [start, start + count):
+// in = a[start..], out = y[start..], Montgomery limbs; acc Montgomery, zero before the first chunk.  Returns 0, 4 on
+// bad arguments, 5 if some dz w^(e j) == 1 (z is unlucky: draw another).
+int orc_fr_ntt_identity_update(const u64* in, const u64* out, size_t start, size_t count, unsigned log_n, unsigned flags,
+                               const u64* coset_gen, const u64* root_2_28, const u64* z, u64* acc, int threads) {
+  NttIdentity p;
+  if (ntt_identity_setup(log_n, flags, coset_gen, root_2_28, z, &p) || start > p.n || count > p.n - start) return 4;
+#ifdef _OPENMP
+  if (threads <= 0) threads = omp_get_max_threads();
+#else
+  threads = 1;
+#endif
+  const Fr* a = (const Fr*)in;
+  const Fr* y = (const Fr*)out;
+  const int T = count < 4096 ? 1 : threads;
+  std::vector<Fr> lhs(T, Fr::zero()), rhs(T, Fr::zero());
+  int bad = 0;
+#pragma omp parallel for num_threads(T) schedule(static, 1) reduction(| : bad)
+  for (int t = 0; t < T; ++t) {
+    const size_t lo = count * t / T, hi = count * (t + 1) / T, m = hi - lo;
+    if (!m) continue;
+    Fr l = Fr::zero();
+    for (size_t k = hi; k-- > lo;) l = l * p.z + y[k];
+    lhs[t] = l * fr_pow_u64(p.z, start + lo);
+    // sum_j num_j / den_j with num_j = a_j c^j, den_j = dz w^(e j) - 1, kept as one fraction num / den (three products
+    // per term) and divided out with one inversion
+    const bool has_c = p.c != Fr::one();
+    Fr x = p.dz * fr_pow_u64(p.step, start + lo), cj = fr_pow_u64(p.c, start + lo), num = Fr::zero(), den = Fr::one();
+    for (size_t j = 0; j < m; ++j) {
+      const Fr dj = x - Fr::one(), nj = has_c ? a[lo + j] * cj : a[lo + j];
+      num = num * dj + nj * den;
+      den = den * dj;
+      x = x * p.step;
+      if (has_c) cj = cj * p.c;
+    }
+    if (den.is_zero()) { bad = 1; continue; }
+    rhs[t] = num * den.inv();
+  }
+  if (bad) return 5;
+  Fr L, Rs;
+  memcpy(L.v, acc, 32);
+  memcpy(Rs.v, acc + 4, 32);
+  for (int t = 0; t < T; ++t) { L = L + lhs[t]; Rs = Rs + rhs[t]; }
+  memcpy(acc, L.v, 32);
+  memcpy(acc + 4, Rs.v, 32);
+  return 0;
+}
+
+// 1 if the sums orc_fr_ntt_identity_update accumulated over all n indices satisfy the identity, 0 if not, 4 on bad arguments
+int orc_fr_ntt_identity_check(const u64* acc, unsigned log_n, unsigned flags, const u64* coset_gen, const u64* root_2_28, const u64* z) {
+  NttIdentity p;
+  if (ntt_identity_setup(log_n, flags, coset_gen, root_2_28, z, &p)) return 4;
+  Fr L, Rs;
+  memcpy(L.v, acc, 32);
+  memcpy(Rs.v, acc + 4, 32);
+  return L == p.s * (fr_pow_u64(p.dz, p.n) - Fr::one()) * Rs ? 1 : 0;
 }
 
 }  // extern "C"

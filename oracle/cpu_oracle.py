@@ -37,6 +37,9 @@ def lib():
         _lib.orc_g1_msm.restype = C.c_int
         _lib.orc_g2_msm.restype = C.c_int
         _lib.orc_fr_ntt.restype = C.c_int
+        _lib.orc_fr_ntt_identity_update.restype = C.c_int
+        _lib.orc_fr_ntt_identity_check.restype = C.c_int
+        _lib.orc_fr_ntt_eval_output_chunk.restype = C.c_int
     return _lib
 
 
@@ -244,3 +247,65 @@ def fr_ntt_eval_output(data_mont: np.ndarray, log_n: int, k: int) -> np.ndarray:
     if rc:
         raise ValueError(f"ntt eval status {rc}")
     return out
+
+
+def fr_ntt_eval_output_chunk(chunk_mont: np.ndarray, start: int, log_n: int, k: int) -> int:
+    """the share of coefficients [start, start + len(chunk)) in output k of the forward NTT, as an integer mod r: summed
+    over the chunks of a vector it is output k by its definition, without holding the vector on the host."""
+    a = np.ascontiguousarray(chunk_mont)
+    out = np.empty((1, 4), dtype=np.uint64)
+    rc = lib().orc_fr_ntt_eval_output_chunk(_p(a), C.c_size_t(a.size // 4), C.c_uint64(start), C.c_uint(log_n), C.c_uint64(k), _p(out))
+    if rc:
+        raise ValueError(f"ntt eval status {rc}")
+    return limbs_to_int(fr_from_mont(out)[0])
+
+
+class NttIdentity:
+    """O(n) whole-vector check that y is the transform of a in one mode of fr_ntt, fed chunk by chunk.
+
+    Every mode is y_k = s d^k sum_j a_j c^j w^(e j k), so at a point z
+        sum_k y_k z^k = s ((dz)^n - 1) sum_j a_j c^j / (dz w^(e j) - 1);
+    update() accumulates both sums over [start, start + len(chunk)) of a and y (Montgomery limbs, any chunking, each
+    index once), ok() compares them.  Exact in Fr: a wrong output passes with probability <= n / r over z."""
+
+    def __init__(self, log_n: int, flags: int = 0, coset_gen: int | None = None, root_2_28: int | None = None,
+                 z: int = 0x1d3a7f5c9e2b48d06a1c3e5f7092b4d6e8fa1c3e5f70921b3d5f7a9cbedf0123, threads: int = 0):
+        self.log_n, self.flags, self.threads = log_n, flags, threads
+        self._keep = [int_to_limbs(z)]
+        self._cg = self._keep_ptr(coset_gen)
+        self._rt = self._keep_ptr(root_2_28)
+        self._z = _p(self._keep[0])
+        self.acc = np.zeros(8, dtype=np.uint64)
+        self.seen = 0
+
+    def _keep_ptr(self, v):
+        if v is None:
+            return None
+        self._keep.append(int_to_limbs(v))
+        return _p(self._keep[-1])
+
+    def update(self, inp_mont: np.ndarray, out_mont: np.ndarray, start: int) -> None:
+        a, y = np.ascontiguousarray(inp_mont), np.ascontiguousarray(out_mont)
+        assert a.size == y.size and a.size % 4 == 0
+        rc = lib().orc_fr_ntt_identity_update(_p(a), _p(y), C.c_size_t(start), C.c_size_t(a.size // 4), C.c_uint(self.log_n),
+                                              C.c_uint(self.flags), self._cg, self._rt, self._z, _p(self.acc), C.c_int(_thr(self.threads)))
+        if rc:
+            raise ValueError(f"ntt identity status {rc}")
+        self.seen += a.size // 4
+
+    def ok(self) -> bool:
+        assert self.seen == 1 << self.log_n, f"fed {self.seen} of {1 << self.log_n} indices"
+        rc = lib().orc_fr_ntt_identity_check(_p(self.acc), C.c_uint(self.log_n), C.c_uint(self.flags), self._cg, self._rt, self._z)
+        if rc not in (0, 1):
+            raise ValueError(f"ntt identity status {rc}")
+        return rc == 1
+
+
+def fr_ntt_identity(inp_mont: np.ndarray, out_mont: np.ndarray, log_n: int, flags: int = 0, coset_gen: int | None = None,
+                    root_2_28: int | None = None, chunk: int = 1 << 20) -> bool:
+    """NttIdentity over two whole vectors held on the host"""
+    chk = NttIdentity(log_n, flags, coset_gen, root_2_28)
+    a, y = inp_mont.reshape(-1, 4), out_mont.reshape(-1, 4)
+    for s in range(0, 1 << log_n, chunk):
+        chk.update(a[s:s + chunk], y[s:s + chunk], s)
+    return chk.ok()
