@@ -1,7 +1,7 @@
 """CPU checks of the BLS12-381 pairing and KZG verification: the independent oracle (tests/bls_pairing_ref.py) against the
 reference's EIP-2537 vectors and bilinearity, G2 compression, the final exponentiation's x-chain identity, every constant
-of ethrex_b200/csrc/bls_pairing.cu recomputed from its definition, a Python verifier over the known-tau setup, and the
-ptxas report of the new kernels."""
+of ethrex_b200/csrc/bls_pairing.cu and bls_pairing.cuh recomputed from its definition, a Python verifier over the known-tau
+setup, and the ptxas report of the new kernels."""
 import json
 import os
 import re
@@ -68,8 +68,8 @@ def _limbs(words):
     return sum(int(w, 16) << (32 * i) for i, w in enumerate(words))
 
 
-def test_constants_of_the_source():
-    src = open(os.path.join(CSRC, "bls_pairing.cu")).read()
+def test_constants_of_the_source_and_header():
+    src = "".join(open(os.path.join(CSRC, f)).read() for f in ("bls_pairing.cuh", "bls_pairing.cu"))
 
     def block(name):
         body = re.search(name + r"[^=]*= \{(.*?)\};", src, re.S).group(1)
