@@ -98,7 +98,6 @@ SIGNATURES = {
     "b200zk_g2_check_device": (_int, [_ctx, _vp, _sz, _vp, C.POINTER(_sz)]),
     "b200zk_set_msm_window": (_int, [_ctx, _u32]),
     "b200zk_set_msm_chunks": (_int, [_ctx, _u32]),
-    "b200zk_set_msm_pair_rounds": (_int, [_ctx, _int]),
     "b200zk_last_msm_phase_ms": (_int, [_ctx, C.POINTER(C.c_float)]),
     "b200zk_set_profiling": (_int, [_ctx, _int]),
     "b200zk_msm_multi_resident_device": (_int, [_ctx, _vp, _sz, _vp, _sz, _u32, _vp, _vp, _vp]),

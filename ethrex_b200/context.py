@@ -121,9 +121,6 @@ class Context:
     def set_msm_chunks(self, chunks: int):
         self._check(F.lib.b200zk_set_msm_chunks(self._h, chunks), "set_msm_chunks")
 
-    def set_msm_pair_rounds(self, rounds: int):
-        self._check(F.lib.b200zk_set_msm_pair_rounds(self._h, rounds), "set_msm_pair_rounds")
-
     def set_profiling(self, on: bool):
         self._check(F.lib.b200zk_set_profiling(self._h, 1 if on else 0), "set_profiling")
 

@@ -237,11 +237,6 @@ int b200zk_set_msm_chunks(b200zk_ctx* ctx, uint32_t chunks) { b200zk::DeviceGuar
   ctx->msm_chunks = chunks;
   return B200ZK_OK;
 }
-int b200zk_set_msm_pair_rounds(b200zk_ctx* ctx, int rounds) { b200zk::DeviceGuard guard(ctx);
-  if (!ctx || rounds > 4) return fail(ctx, B200ZK_ERR_INVALID_ARG, "pair rounds must be <= 4 (negative = automatic)");
-  ctx->msm_pair_rounds = rounds < 0 ? -1 : rounds;
-  return B200ZK_OK;
-}
 int b200zk_set_profiling(b200zk_ctx* ctx, int enabled) { b200zk::DeviceGuard guard(ctx);
   if (!ctx) return B200ZK_ERR_INVALID_ARG;
   ctx->profiling = enabled != 0;

@@ -116,13 +116,11 @@ struct b200zk_ctx {
   b200zk::DevBuf ws_pairing;  // BLS12-381 pairing checks and KZG verification (bls_pairing.cu): inputs, points, lines, Miller values;
                               // also the inputs and outputs of the EIP-2537 (bls_ops.cu), ECRECOVER (secp256k1.cu),
                               // P256VERIFY (secp256r1.cu) and MODEXP (modexp.cu: operand bytes, item list, outputs) batches
-  int msm_pair_rounds = -1;  // batched-affine pair-summing rounds before the XYZZ accumulation; <0 = automatic
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
   cudaEvent_t ev[8] = {};
   // grow-only workspaces (every DevBuf, OnceTable and BasesEntry frees itself when the context is deleted)
-  b200zk::DevBuf ws_buckets, ws_chunkS, ws_chunkV, ws_result, ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segbucket, ws_q0, ws_q1,
-      ws_prefix, ws_info, ws_pairoff0, ws_pairoff1;
+  b200zk::DevBuf ws_buckets, ws_chunkS, ws_chunkV, ws_result, ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segbucket;
   // 2^28-th primitive root of unity of Fr the NTT derives its domain generators from (canonical limbs).
   // Default = ark-poly / gnark-crypto 5^((r-1)/2^28); halo2curves uses 7^((r-1)/2^28) (b200zk_set_ntt_root).
   uint32_t ntt_root[8] = {0x725b19f0u, 0x9bd61b6eu, 0x41112ed4u, 0x402d111eu, 0x8ef62abcu, 0x00e0a7ebu, 0xa58a7e85u, 0x2a3c09f0u};

@@ -515,12 +515,8 @@ struct Fq2 {
   // a*b - c*d over Fq2: each component is a sum of FOUR base-field products under one reduction (Fq::mul4_add):
   //   re = a0 b0 - a1 b1 - c0 d0 + c1 d1        im = a0 b1 + a1 b0 - c0 d1 - c1 d0
   static B2_D Fq2 mul2_sub(const Fq2& a, const Fq2& b, const Fq2& c, const Fq2& d) {
-#ifdef B200ZK_FQ2_NO_MUL4
-    return sub(mul(a, b), mul(c, d));
-#else
     const Fq na1 = Fq::neg(a.c1), nc0 = Fq::neg(c.c0), nc1 = Fq::neg(c.c1);
     return {Fq::mul4_add(a.c0, b.c0, na1, b.c1, nc0, d.c0, c.c1, d.c1), Fq::mul4_add(a.c0, b.c1, a.c1, b.c0, nc0, d.c1, nc1, d.c0)};
-#endif
   }
   static B2_D Fq2 inv(const Fq2& a) {
     Fq d = Fq::inv(Fq::add(Fq::sqr(a.c0), Fq::sqr(a.c1)));

@@ -548,19 +548,18 @@ static constexpr int kScanThreads = 256, kScanItems = 8, kScanTile = kScanThread
 // seg  > 0: scan the flag "bucket i is non-empty and does not start on a multiple of seg" (aux = bucket offsets);
 //           scan_apply then adds ceil(offset/seg), giving run_off[i] = index of the first RUN of bucket i when the
 //           sorted entries are cut at every multiple of seg and at every bucket start (see msm_accumulate).
-// shift: the counts scanned are ceil(in[i] / 2^shift) -- bucket sizes after `shift` rounds of pair-summing.
-B2_D uint32_t scan_value(const uint32_t* in, const uint32_t* aux, size_t i, uint32_t seg, uint32_t shift) {
+B2_D uint32_t scan_value(const uint32_t* in, const uint32_t* aux, size_t i, uint32_t seg) {
   uint32_t v = in[i];
-  if (!seg) return (v + (1u << shift) - 1u) >> shift;
+  if (!seg) return v;
   return (v != 0 && (aux[i] % seg) != 0) ? 1u : 0u;
 }
 
-__global__ void __launch_bounds__(kScanThreads) scan_tile_sums(const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t shift, uint32_t* tile_sums) {
+__global__ void __launch_bounds__(kScanThreads) scan_tile_sums(const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t* tile_sums) {
   __shared__ uint32_t red[kScanThreads / 32];
   size_t base = (size_t)blockIdx.x * kScanTile + (size_t)threadIdx.x * kScanItems;
   uint32_t s = 0;
 #pragma unroll
-  for (int k = 0; k < kScanItems; ++k) if (base + k < G) s += scan_value(in, aux, base + k, seg, shift);
+  for (int k = 0; k < kScanItems; ++k) if (base + k < G) s += scan_value(in, aux, base + k, seg);
 #pragma unroll
   for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
@@ -595,12 +594,12 @@ __global__ void __launch_bounds__(1024) scan_tile_offsets(uint32_t* tile_sums, s
     __syncthreads();
   }
 }
-__global__ void __launch_bounds__(kScanThreads) scan_apply(const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t shift, const uint32_t* tile_offsets, uint32_t* offsets, uint32_t* cursor) {
+__global__ void __launch_bounds__(kScanThreads) scan_apply(const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, const uint32_t* tile_offsets, uint32_t* offsets, uint32_t* cursor) {
   __shared__ uint32_t warp_tot[kScanThreads / 32];
   size_t base = (size_t)blockIdx.x * kScanTile + (size_t)threadIdx.x * kScanItems;
   uint32_t v[kScanItems], s = 0;
 #pragma unroll
-  for (int k = 0; k < kScanItems; ++k) { v[k] = base + k < G ? scan_value(in, aux, base + k, seg, shift) : 0; s += v[k]; }
+  for (int k = 0; k < kScanItems; ++k) { v[k] = base + k < G ? scan_value(in, aux, base + k, seg) : 0; s += v[k]; }
   uint32_t incl = s;
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) { uint32_t t = __shfl_up_sync(0xffffffffu, incl, o); if ((threadIdx.x & 31) >= (unsigned)o) incl += t; }
@@ -661,9 +660,8 @@ B2_D uint32_t bucket_of(const uint32_t* __restrict__ offsets, uint32_t G, uint32
   return lo;
 }
 
-// DIRECT: `points` is already the sorted, sign-applied entry array (output of pair_sum); else entries are
-// idx[e] = base index | sign << 31 into the bases / window table.
-template <class F, bool DIRECT>
+// sorted entry e is idx[e] = base index | sign << 31 into the bases / window table
+template <class F>
 __global__ void __launch_bounds__(128, 1) msm_accumulate(const void* __restrict__ points, const uint32_t* __restrict__ idx,
                                                       const uint32_t* __restrict__ offsets, const uint32_t* __restrict__ run_off,
                                                       uint32_t G, uint32_t kSegLen, void* __restrict__ partials, uint32_t* __restrict__ run_bucket) {
@@ -684,12 +682,12 @@ __global__ void __launch_bounds__(128, 1) msm_accumulate(const void* __restrict_
   uint32_t slot = t + (__ldg(run_off + g) - (off0 + kSegLen - 1) / kSegLen) + ((off0 % kSegLen) ? 1u : 0u);
   uint32_t next = __ldg(offsets + g + 1);  // first entry of the following bucket (> e0)
   XYZZ<F> acc = XYZZ<F>::identity();
-  uint32_t v = DIRECT ? e0 : __ldg(idx + e0);
+  uint32_t v = __ldg(idx + e0);
   Affine<F> p = load_affine_nc<F>(points, v & 0x7fffffffu);
   for (uint32_t e = e0; e < e1; ++e) {
     // software prefetch: issue the next gather before the ~1500-instruction addition
     uint32_t vn = v; Affine<F> pn = p;
-    if (e + 1 < e1) { vn = DIRECT ? e + 1 : __ldg(idx + e + 1); pn = load_affine_nc<F>(points, vn & 0x7fffffffu); }
+    if (e + 1 < e1) { vn = __ldg(idx + e + 1); pn = load_affine_nc<F>(points, vn & 0x7fffffffu); }
     if (e == next) {  // bucket boundary: close the run
       store_xyzz(partials, slot, acc);
       run_bucket[slot] = g;
@@ -698,7 +696,7 @@ __global__ void __launch_bounds__(128, 1) msm_accumulate(const void* __restrict_
       g = bucket_of(offsets, G, g + 1, e);
       next = __ldg(offsets + g + 1);
     }
-    if (!DIRECT && (v >> 31)) p.y = F::neg(p.y);
+    if (v >> 31) p.y = F::neg(p.y);
     xyzz_add_mixed(acc, p.x, p.y);
     v = vn; p = pn;
   }
@@ -871,140 +869,6 @@ __global__ void __launch_bounds__(128, kG2PairBlocks) msm_accumulate_g2_pair(con
   }
   store_half(slot, acc);
   if (!L.hi) run_bucket[slot] = g;
-}
-
-// ---- batched-affine pair summing ---------------------------------------------------------------------------
-// One round halves every bucket: entries (2k, 2k+1) of a bucket are replaced by their AFFINE sum, an odd last
-// entry is carried over.  An affine addition needs 1/(x2 - x1); a thread owns kPairBatch consecutive outputs and
-// inverts all its denominators with ONE field inversion (Montgomery's trick): forward sweep stores the prefix
-// products, backward sweep peels the inverses off.  Cost per pair: 1 (prefix) + 2 (peel) + 3 (lambda, lambda^2,
-// y3) products + 1/kPairBatch of an inversion  ~ 6.7 products, against 10 for an XYZZ mixed addition; after r
-// rounds the XYZZ accumulation only sees M/2^r entries.  Exceptional pairs (equal points -> tangent, opposite
-// points -> identity, identity operands) put 1 (or 2y) in the batch and are resolved in the backward sweep.
-static constexpr uint32_t kPairBatch = 256;
-
-template <class F, bool INDIRECT>
-B2_D Affine<F> pair_load(const void* __restrict__ points, const uint32_t* __restrict__ idx, uint32_t e) {
-  if (INDIRECT) {
-    uint32_t v = __ldg(idx + e);
-    Affine<F> p = load_affine_nc<F>(points, v & 0x7fffffffu);
-    if (v >> 31) p.y = F::neg(p.y);
-    return p;
-  }
-  return load_affine_nc<F>(points, e);
-}
-// denominator of the pair (a, b); kind: 0 = chord, 1 = tangent, 2 = result is `a`, 3 = result is `b`, 4 = identity
-template <class F> B2_D F pair_denominator(const Affine<F>& a, const Affine<F>& b, int* kind) {
-  if (b.is_inf()) { *kind = 2; return F::one(); }
-  if (a.is_inf()) { *kind = 3; return F::one(); }
-  F dx = F::sub(b.x, a.x);
-  if (!dx.is_zero()) { *kind = 0; return dx; }
-  if (a.y == b.y && !a.y.is_zero()) { *kind = 1; return F::dbl(a.y); }
-  *kind = 4; return F::one();
-}
-
-// x coordinates only (the forward sweep needs no y unless the x's collide)
-template <class F, bool INDIRECT>
-B2_D void pair_load_x(const void* __restrict__ points, const uint32_t* __restrict__ idx, uint32_t e, F* x, uint32_t* v) {
-  *v = INDIRECT ? __ldg(idx + e) : e;
-  *x = load_field_nc(points, 2 * (size_t)(*v & 0x7fffffffu), (const F*)nullptr);
-}
-template <class F, bool INDIRECT>
-B2_D F pair_load_y(const void* __restrict__ points, uint32_t v) {
-  F y = load_field_nc(points, 2 * (size_t)(v & 0x7fffffffu) + 1, (const F*)nullptr);
-  if (INDIRECT && (v >> 31)) y = F::neg(y);
-  return y;
-}
-
-template <class F, bool INDIRECT>
-__global__ void __launch_bounds__(128) pair_sum(const void* __restrict__ points, const uint32_t* __restrict__ idx,
-                                                const uint32_t* __restrict__ off_in, const uint32_t* __restrict__ off_out, uint32_t G,
-                                                void* __restrict__ prefix, uint32_t* __restrict__ info, void* __restrict__ out) {
-  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-  const uint32_t Mout = __ldg(off_out + G);
-  const uint64_t o0_64 = (uint64_t)t * kPairBatch;
-  if (o0_64 >= Mout) return;
-  const uint32_t o0 = (uint32_t)o0_64;
-  const uint32_t o1 = (Mout - o0 > kPairBatch) ? o0 + kPairBatch : Mout;
-  uint32_t g;
-  {
-    uint32_t lo = 0, hi = G;
-    while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (__ldg(off_out + mid) <= o0) lo = mid; else hi = mid; }
-    g = lo;
-  }
-  uint32_t next = __ldg(off_out + g + 1);
-  uint32_t base_out = __ldg(off_out + g), base_in = __ldg(off_in + g), end_in = __ldg(off_in + g + 1);
-  // ---- forward sweep: prefix products of the denominators.  The (entry, has_pair) word of every output is
-  // computed one iteration ahead so that the x gathers of output o+1 are in flight during the product of output o.
-  auto locate = [&](uint32_t o) -> uint32_t {
-    if (o == next) {
-      g = bucket_of(off_out, G, g + 1, o);
-      next = __ldg(off_out + g + 1);
-      base_out = __ldg(off_out + g); base_in = __ldg(off_in + g); end_in = __ldg(off_in + g + 1);
-    }
-    const uint32_t ea = base_in + 2 * (o - base_out);
-    return ea | ((ea + 1 < end_in) ? 0x80000000u : 0u);
-  };
-  F prod = F::one();
-  uint32_t w = locate(o0), va = 0, vb = 0;
-  F xa = F::zero(), xb = F::zero();
-  pair_load_x<F, INDIRECT>(points, idx, w & 0x7fffffffu, &xa, &va);
-  if (w >> 31) pair_load_x<F, INDIRECT>(points, idx, (w & 0x7fffffffu) + 1, &xb, &vb);
-  for (uint32_t o = o0; o < o1; ++o) {
-    uint32_t wn = w, van = va, vbn = vb; F xan = xa, xbn = xb;
-    if (o + 1 < o1) {
-      wn = locate(o + 1);
-      pair_load_x<F, INDIRECT>(points, idx, wn & 0x7fffffffu, &xan, &van);
-      if (wn >> 31) pair_load_x<F, INDIRECT>(points, idx, (wn & 0x7fffffffu) + 1, &xbn, &vbn);
-    }
-    info[o] = w;
-    store_field(prefix, o, prod);
-    if (w >> 31) {
-      F d = F::sub(xb, xa);
-      bool plain = !d.is_zero();
-      if (!plain || xa.is_zero() || xb.is_zero()) {  // rare: equal x, or a possible identity operand -> full classification
-        Affine<F> a = {xa, pair_load_y<F, INDIRECT>(points, va)}, b = {xb, pair_load_y<F, INDIRECT>(points, vb)};
-        int kind;
-        d = pair_denominator(a, b, &kind);
-        plain = kind <= 1;
-      }
-      if (plain) prod = F::mul(prod, d);
-    }
-    w = wn; va = van; vb = vbn; xa = xan; xb = xbn;
-  }
-  F inv = F::inv(prod);
-  // ---- backward sweep (next pair's four coordinates prefetched the same way)
-  uint32_t wo = info[o1 - 1];
-  Affine<F> a = pair_load<F, INDIRECT>(points, idx, wo & 0x7fffffffu), b = a;
-  if (wo >> 31) b = pair_load<F, INDIRECT>(points, idx, (wo & 0x7fffffffu) + 1);
-  F pre = load_field(prefix, o1 - 1, (const F*)nullptr);
-  for (uint32_t o = o1; o-- > o0;) {
-    uint32_t won = wo; Affine<F> an = a, bn = b; F pren = pre;
-    if (o > o0) {
-      won = info[o - 1];
-      an = pair_load<F, INDIRECT>(points, idx, won & 0x7fffffffu);
-      if (won >> 31) bn = pair_load<F, INDIRECT>(points, idx, (won & 0x7fffffffu) + 1);
-      pren = load_field(prefix, o - 1, (const F*)nullptr);
-    }
-    Affine<F> r = a;
-    if (wo >> 31) {
-      int kind;
-      F d = pair_denominator(a, b, &kind);
-      if (kind <= 1) {
-        F dinv = F::mul(inv, pre);  // 1/d
-        inv = F::mul(inv, d);
-        F num;
-        if (kind == 0) num = F::sub(b.y, a.y);
-        else { F xx = F::sqr(a.x); num = F::add(F::dbl(xx), xx); }
-        F lam = F::mul(num, dinv);
-        r.x = F::sub(F::sub(F::sqr(lam), a.x), b.x);
-        r.y = F::sub(F::mul(lam, F::sub(a.x, r.x)), a.y);
-      } else if (kind == 3) r = b;
-      else if (kind == 4) r = {F::zero(), F::zero()};
-    }
-    store_affine<F>(out, o, r);
-    wo = won; a = an; b = bn; pre = pren;
-  }
 }
 
 template <class F>
@@ -1389,18 +1253,18 @@ static int launch_accumulate(b200zk_ctx* ctx, cudaStream_t st, const void* pts, 
   if constexpr (IsFq2<F>::value)
     B2_LAUNCH(ctx, msm_accumulate_g2_pair, (unsigned)((2 * slices + 127) / 128), 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
   else
-    B2_LAUNCH(ctx, (msm_accumulate<F, false>), (unsigned)((slices + 127) / 128), 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
+    B2_LAUNCH(ctx, msm_accumulate<F>, (unsigned)((slices + 127) / 128), 128, 0, st, pts, idx, offsets, run_off, G, L, partials, run_bucket);
   return B200ZK_OK;
 }
 
 // exclusive scan of G values (scan_value: counts, or run flags when seg > 0) into out[0..G]; cursor, if given, receives
 // out[0..G) as well.  tsum: one word per kScanTile values.
-static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t shift, uint32_t* tsum,
+static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t* tsum,
                           uint32_t* out, uint32_t* cursor = nullptr) {
   const size_t tiles = (G + kScanTile - 1) / kScanTile;
-  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, shift, tsum);
+  B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, tsum);
   B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);
-  B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, shift, (const uint32_t*)tsum, out, cursor);
+  B2_LAUNCH(ctx, scan_apply, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, (const uint32_t*)tsum, out, cursor);
   return B200ZK_OK;
 }
 
@@ -1422,7 +1286,7 @@ static int sort_digits(b200zk_ctx* ctx, const void* d_scalars, size_t n, uint32_
     const unsigned sgrid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8);
     B2_LAUNCH(ctx, msm_hist, sgrid, 256, 0, st, d_scalars, n, flags, pl, hist, (uint32_t*)s.digits.p);
     phase_mark(ctx, 1, st);
-    B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, 0, tsum, offsets, (uint32_t*)s.cursor.p));
+    B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, tsum, offsets, (uint32_t*)s.cursor.p));
     phase_mark(ctx, 2, st);
     const unsigned wgrid = (unsigned)std::min<size_t>((n * (size_t)pl.W + 255) / 256, (size_t)ctx->sm_count * 32);
     B2_LAUNCH(ctx, msm_scatter, wgrid, 256, 0, st, (const uint32_t*)s.digits.p, n, pl, (uint32_t*)s.cursor.p, idx);
@@ -1440,7 +1304,7 @@ static int sort_digits(b200zk_ctx* ctx, const void* d_scalars, size_t n, uint32_
   B2_CUDA(ctx, cudaMemsetAsync(cnt, 0, (Gc + 1) * 4, st));
   B2_LAUNCH(ctx, msm_sort_count, sp.NC * kSortCountSub, kHistTile, 0, st, d_scalars, n, flags, pl, sp, cnt);
   phase_mark(ctx, 1, st);
-  B2_TRY(exclusive_scan(ctx, st, cnt, nullptr, Gc, 0, 0, tsum, base));
+  B2_TRY(exclusive_scan(ctx, st, cnt, nullptr, Gc, 0, tsum, base));
   phase_mark(ctx, 2, st);
   B2_LAUNCH(ctx, msm_sort_coarse, sp.NC, kSortTile, sizeof(SortCoarseSmem), st, d_scalars, n, flags, pl, sp, (const uint32_t*)base, ent1);
   // fine pass over segments of kFineSeg entries: at most M / kFineSeg + C items (the grid is this bound; surplus CTAs exit)
@@ -1449,7 +1313,7 @@ static int sort_digits(b200zk_ctx* ctx, const void* d_scalars, size_t n, uint32_
   B2_LAUNCH(ctx, msm_sort_items, 1, 1024, 0, st, (const uint32_t*)base, sp, item_start);
   B2_LAUNCH(ctx, msm_sort_fine_count, max_items, 1024, 0, st, (const uint2*)ent1, sp, (const uint32_t*)base, (const uint32_t*)item_start, cnt2);
   B2_LAUNCH(ctx, msm_sort_fine_prefix, (unsigned)(((size_t)sp.C * F + 255) / 256), 256, 0, st, sp, (const uint32_t*)item_start, cnt2, hist);
-  B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, 0, tsum, offsets));
+  B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, tsum, offsets));
   B2_LAUNCH(ctx, msm_sort_fine_place, max_items, 1024, sizeof(SortFineSmem), st, (const uint2*)ent1, sp, (const uint32_t*)base, (const uint32_t*)item_start, (const uint32_t*)cnt2,
             (const uint32_t*)offsets, idx);
   return B200ZK_OK;
@@ -1499,8 +1363,8 @@ static int reduce_buckets(b200zk_ctx* ctx, cudaStream_t st, const MsmPlan& pl, c
 // scalars upload on the copy stream (ctx->stream_upload) while earlier chunks compute, so that only the FIRST chunk's
 // upload is exposed.  Every kernel runs on the caller's stream in the order sort(0), accumulate(0), sort(1), ...: the
 // two-level sort's CTAs want whole SMs, so each kernel has the machine to itself and the copy engine works underneath,
-// one chunk ahead.  Profiled calls, pair-summing rounds, shared sorts (sort_mode 1 / 2) and tiny inputs run one chunk and
-// stage host scalars on the caller's stream.
+// one chunk ahead.  Profiled calls, shared sorts (sort_mode 1 / 2) and tiny inputs run one chunk and stage host scalars
+// on the caller's stream.
 template <class F>
 static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars, size_t n, uint32_t flags, cudaStream_t st, void* d_partial,
                    uint32_t table_c, size_t table_stride, const void* h_scalars, int sort_mode) {
@@ -1525,7 +1389,7 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
   // from 2^22 points up: G1 3 chunks, G2 2 (b200zk_set_msm_chunks overrides the count)
   uint32_t K = ctx->msm_chunks ? ctx->msm_chunks : ((h_scalars && n >= ((size_t)1 << 22)) ? (IsFq2<F>::value ? 2u : 3u) : 1u);
   if (K > kMaxPipelineChunks) K = kMaxPipelineChunks;
-  const bool chunked = sort_mode == 0 && (K > 1 || h_scalars) && !ctx->profiling && ctx->msm_pair_rounds <= 0 && n >= 4096;
+  const bool chunked = sort_mode == 0 && (K > 1 || h_scalars) && !ctx->profiling && n >= 4096;
   if (!chunked) K = 1;
   const size_t G = (size_t)pl.Wr * pl.B;
   const size_t xy = 4 * FieldBytes<F>::value, pt = 2 * FieldBytes<F>::value;
@@ -1548,15 +1412,6 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
       if (hi > bnd[chunks]) bnd[++chunks] = hi;  // empty chunks (tiny n) vanish
     }
   }
-  // pair-summing rounds (one chunk only).  A round is bound by its ~330 B of scattered memory traffic per pair, not by its 6.7
-  // products, and costs more than the XYZZ addition it removes, so the automatic setting is OFF; the path stays available (b200zk_set_msm_pair_rounds)
-  // for parts with a different compute:bandwidth balance and is covered by the parity tests.
-  const size_t M_max = n * (size_t)pl.W;
-  uint32_t rounds = 0;
-  if (ctx->msm_pair_rounds >= 0) rounds = (uint32_t)ctx->msm_pair_rounds;
-  if (rounds > 4) rounds = 4;
-  if (rounds && M_max >= ((size_t)1 << 31)) rounds = 0;
-  if (sort_mode) rounds = 0;
   // per chunk: slice length (each chunk fills whole waves of resident threads); over all chunks: the largest run count and
   // the largest entry count of either sort
   const size_t resident = resident_slices<F>(ctx);
@@ -1564,8 +1419,8 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
   size_t S_max = 0, M_two = 0, M_one = 0;
   for (uint32_t k = 0; k < chunks; ++k) {
     const size_t nk = bnd[k + 1] - bnd[k], Mk = nk * pl.W;
-    Lk[k] = pick_slice_len(Mk >> rounds, resident);
-    S_max = std::max(S_max, (Mk >> rounds) / Lk[k] + 1 + G);
+    Lk[k] = pick_slice_len(Mk, resident);
+    S_max = std::max(S_max, Mk / Lk[k] + 1 + G);
     SortPlan sp;
     size_t& M_sort = make_sort_plan(nk, pl, ctx->sm_count, &sp) ? M_two : M_one;
     M_sort = std::max(M_sort, Mk);
@@ -1585,14 +1440,6 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
     B2_TRY(ensure(ctx, s.idx, std::max(M_two, M_one) * 4));
     if (M_one) { B2_TRY(ensure(ctx, s.cursor, G * 4)); B2_TRY(ensure(ctx, s.digits, M_one * 4)); }
     if (M_two) { B2_TRY(ensure(ctx, s.key, M_two * 8)); B2_TRY(ensure(ctx, s.ctab, sort_ctab_bytes(ctx->sm_count))); B2_TRY(ensure(ctx, s.cnt2, sort_cnt2_bytes(M_two))); }
-  }
-  if (rounds) {
-    B2_TRY(ensure(ctx, ctx->ws_q1, (M_max / 2 + G + 1) * pt));
-    if (rounds > 1) B2_TRY(ensure(ctx, ctx->ws_q0, (M_max / 4 + G + 1) * pt));
-    B2_TRY(ensure(ctx, ctx->ws_prefix, (M_max / 2 + G + 1) * FieldBytes<F>::value));
-    B2_TRY(ensure(ctx, ctx->ws_info, (M_max / 2 + G + 1) * 4));
-    B2_TRY(ensure(ctx, ctx->ws_pairoff0, (G + 1) * 4));
-    B2_TRY(ensure(ctx, ctx->ws_pairoff1, (G + 1) * 4));
   }
   B2_TRY(ensure(ctx, ctx->ws_buckets, S_max * xy));  // run partials (bucket totals after partial_tree)
   B2_TRY(ensure(ctx, ctx->ws_segbucket, S_max * 4));
@@ -1641,30 +1488,11 @@ static int msm_run(b200zk_ctx* ctx, const void* d_points, const void* d_scalars,
     nvtxRangePop();
     phase_mark(ctx, 3, st);
     NvtxRange nvtx_acc("b200zk:msm_accumulate+reduce");
-    // batched-affine pair-summing rounds: each halves the entries the XYZZ accumulation has to fold
-    const uint32_t* cur_off = offsets;
-    const void* cur_pts = (const uint8_t*)d_points + lo * pt;
-    for (uint32_t r = 1; r <= rounds; ++r) {
-      uint32_t* off_r = (uint32_t*)(r & 1 ? ctx->ws_pairoff1.p : ctx->ws_pairoff0.p);
-      B2_TRY(exclusive_scan(ctx, st, hist, nullptr, G, 0, r, tsum, off_r));
-      const size_t out_max = (M_max >> r) + G;
-      void* q = (r & 1) ? ctx->ws_q1.p : ctx->ws_q0.p;
-      const unsigned pgrid = (unsigned)((out_max / kPairBatch + 1 + 127) / 128);
-      if (r == 1) B2_LAUNCH(ctx, (pair_sum<F, true>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
-      else B2_LAUNCH(ctx, (pair_sum<F, false>), pgrid, 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)off_r, (uint32_t)G, ctx->ws_prefix.p, (uint32_t*)ctx->ws_info.p, q);
-      cur_off = off_r;
-      cur_pts = q;
-    }
-    B2_TRY(exclusive_scan(ctx, st, hist, cur_off, G, L, 0, tsum, run_off));
-    const size_t Mk = (nk * pl.W) >> rounds;
-    if (rounds) {
-      // a bucket of h entries leaves ceil(h / 2^rounds): up to G more than Mk
-      const size_t slices = (Mk + G + L - 1) / L;
-      B2_LAUNCH(ctx, (msm_accumulate<F, true>), (unsigned)((slices + 127) / 128), 128, 0, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)run_off, (uint32_t)G, L, ctx->ws_buckets.p, run_bucket);
-    } else {
-      B2_TRY(launch_accumulate<F>(ctx, st, cur_pts, (const uint32_t*)s.idx.p, cur_off, (const uint32_t*)run_off, (uint32_t)G, L, (Mk + L - 1) / L, ctx->ws_buckets.p, run_bucket));
-    }
-    B2_TRY(fold_runs<F>(ctx, st, run_off, run_bucket, (uint32_t)G, (pl.merged ? nk * (size_t)pl.W : nk) >> rounds, L, S_max, ctx->ws_buckets.p));
+    B2_TRY(exclusive_scan(ctx, st, hist, offsets, G, L, tsum, run_off));
+    const size_t Mk = nk * pl.W;
+    const void* pts = (const uint8_t*)d_points + lo * pt;
+    B2_TRY(launch_accumulate<F>(ctx, st, pts, (const uint32_t*)s.idx.p, offsets, (const uint32_t*)run_off, (uint32_t)G, L, (Mk + L - 1) / L, ctx->ws_buckets.p, run_bucket));
+    B2_TRY(fold_runs<F>(ctx, st, run_off, run_bucket, (uint32_t)G, pl.merged ? nk * (size_t)pl.W : nk, L, S_max, ctx->ws_buckets.p));
     phase_mark(ctx, 4, st);
     if (dense_totals) B2_LAUNCH(ctx, bucket_merge<F>, (unsigned)((G + 127) / 128), 128, 0, st, (const void*)ctx->ws_buckets.p, (const uint32_t*)run_off, (uint32_t)G, k == 0 ? 1 : 0, ctx->ws_totals.p);
   }

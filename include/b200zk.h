@@ -211,11 +211,9 @@ int b200zk_g2_check_device(b200zk_ctx* ctx, const void* d_points, size_t n, void
 
 /* tuning knobs (0 = automatic): window bits for the next MSM calls on this context */
 int b200zk_set_msm_window(b200zk_ctx* ctx, uint32_t c);
-/* chunks of the pipelined MSM schedule (sort of chunk k+1 overlaps the accumulation of chunk k); 0 = automatic
- * (4 from 2^22 points), 1 = one shot */
+/* chunks of the pipelined MSM schedule (the host-scalar upload of chunk k+1 overlaps the kernels of chunk k); 0 = automatic
+ * (host scalars from 2^22 points: 3 chunks for a G1 MSM, 2 for G2; otherwise one shot), 1 = one shot */
 int b200zk_set_msm_chunks(b200zk_ctx* ctx, uint32_t chunks);
-/* rounds of batched-affine pair summing run before the bucket accumulation (0..4; negative = automatic) */
-int b200zk_set_msm_pair_rounds(b200zk_ctx* ctx, int rounds);
 /* per-phase device time of the last *_device MSM call, in milliseconds:
  * [0] digit histogram, [1] scan, [2] scatter, [3] bucket accumulation, [4] bucket reduction, [5] final */
 int b200zk_last_msm_phase_ms(b200zk_ctx* ctx, float out_ms[6]);

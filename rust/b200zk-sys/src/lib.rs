@@ -125,7 +125,6 @@ unsafe extern "C" {
 
     pub fn b200zk_set_msm_window(ctx: *mut b200zk_ctx, c: u32) -> c_int;
     pub fn b200zk_set_msm_chunks(ctx: *mut b200zk_ctx, chunks: u32) -> c_int;
-    pub fn b200zk_set_msm_pair_rounds(ctx: *mut b200zk_ctx, rounds: c_int) -> c_int;
     pub fn b200zk_last_msm_phase_ms(ctx: *mut b200zk_ctx, out_ms: *mut f32) -> c_int;
     pub fn b200zk_set_profiling(ctx: *mut b200zk_ctx, enabled: c_int) -> c_int;
 

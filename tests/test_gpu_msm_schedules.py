@@ -1,5 +1,5 @@
 """The MSM schedules that the other parity files do not reach: BLS12-381 (msm_run<Fp381>, 256 scalar bits) through the
-two-level sort, dense bucket totals, pair-sum rounds, the chunked schedule, window tables and forced windows; the
+two-level sort, dense bucket totals, edge bases, the chunked schedule, window tables and forced windows; the
 BN254 partial-sum entry points over resident bases; the profiled schedule; and the refusal of B200ZK_SCALARS_RAW by every
 BN254 MSM entry point.
 
@@ -48,7 +48,7 @@ def table_window(n_bases: int) -> int:
 
 def msm_plan(n: int, forced_c: int = 0, scalar_bits: int = 255, table_c: int = 0) -> Plan:
     """make_plan (msm.cu:54-71), make_sort_plan (msm.cu:260-277) and the reduction choices of msm_run (dense totals
-    msm.cu:1577, bit-sums msm.cu:1478).  scalar_bits: 255 for BN254, 256 for BLS12-381 (ScalarBits<F>)."""
+    msm.cu:1432, bit-sums msm.cu:1342).  scalar_bits: 255 for BN254, 256 for BLS12-381 (ScalarBits<F>)."""
     lg = (n - 1).bit_length()
     forced = table_c or forced_c       # a window table fixes c; set_msm_window does not apply to it
     c = forced if forced else (lg - 4 if lg > 8 else 4)
@@ -65,13 +65,13 @@ def msm_plan(n: int, forced_c: int = 0, scalar_bits: int = 255, table_c: int = 0
     return Plan(c, W, G, bool(table_c), two_level, G >= (1 << 14), T >= 64)
 
 
-def pipelined(n: int, chunks: int = 0, host_scalars: bool = False, profiling: bool = False, pair_rounds: int = -1, g2: bool = False) -> bool:
-    """msm_run's one rule for more than one chunk, or host scalars uploaded on the copy stream (msm.cu:1526-1529): a
-    plain call (sort_mode 0) with K > 1 chunks or host scalars, not profiled, without pair-sum rounds, from 4096 points.
+def pipelined(n: int, chunks: int = 0, host_scalars: bool = False, profiling: bool = False, g2: bool = False) -> bool:
+    """msm_run's one rule for more than one chunk, or host scalars uploaded on the copy stream (msm.cu:1390-1393): a
+    plain call (sort_mode 0) with K > 1 chunks or host scalars, not profiled, from 4096 points.
     Otherwise the call runs one chunk and stages host scalars on the caller's stream.  BLS12-381 calls stage their
     scalars themselves and reach msm_run with device scalars (host_scalars=False)."""
     K = chunks or ((2 if g2 else 3) if host_scalars and n >= (1 << 22) else 1)
-    return (K > 1 or host_scalars) and not profiling and pair_rounds <= 0 and n >= 4096
+    return (K > 1 or host_scalars) and not profiling and n >= 4096
 
 
 def test_plan_mirror_matches_the_documented_defaults():
@@ -238,9 +238,9 @@ def test_bls_two_level_sort_on_skewed_scalars(ctx, bls_mid, table):
         ctx.bases_free(h)
 
 
-# ------------------------------------------------------------------------------------------ BLS12-381: pair sums, chunks
-def test_bls_pair_sum_rounds_edge_bases(ctx, bls_mid):
-    """batched-affine pair-sum rounds 1..4 over Fp381 at c = 6 and 11: repeated bases (tangent case), P and -P (identity),
+# ------------------------------------------------------------------------------------------ BLS12-381: edge bases, chunks
+def test_bls_msm_edge_bases(ctx, bls_mid):
+    """bucket accumulation over Fp381 at c = 6 and 11: repeated bases (a doubling in a bucket), P and -P (identity),
     identity bases, with one heavy bucket, one value everywhere and neighbours that share every digit"""
     raw, logs = bls_mid
     n = 4096
@@ -264,16 +264,13 @@ def test_bls_pair_sum_rounds_edge_bases(ctx, bls_mid):
     }
     h = ctx.bls12_381_g1_bases_upload(bytes(pts), n, 0)
     try:
+        assert not pipelined(n)
         for c in (6, 11):
             ctx.set_msm_window(c)
-            for rounds in (1, 2, 3, 4):
-                assert not pipelined(n, pair_rounds=rounds)
-                ctx.set_msm_pair_rounds(rounds)
-                for name, vals in cases.items():
-                    assert ctx.bls12_381_g1_msm_resident(h, be(vals), n) == bls_expected(vals, logs), (c, rounds, name)
+            for name, vals in cases.items():
+                assert ctx.bls12_381_g1_msm_resident(h, be(vals), n) == bls_expected(vals, logs), (c, name)
     finally:
         ctx.set_msm_window(0)
-        ctx.set_msm_pair_rounds(-1)
         ctx.bases_free(h)
 
 

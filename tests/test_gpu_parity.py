@@ -529,8 +529,9 @@ def test_precomputed_2_20_closed_form(ctx):
         ctx.bases_free(h)
 
 
-def test_pair_sum_rounds_edge_cases(ctx):
-    """batched-affine pre-pass: equal points (tangent), opposite points (identity), identity operands, heavy buckets."""
+def test_msm_edge_bases(ctx):
+    """bucket accumulation at c = 6 and 11: equal points in one bucket (doubling), opposite points (identity), identity
+    bases, one heavy bucket, one value everywhere, neighbours sharing every digit; and a repeated G2 base."""
     k, d = chain_kd()
     n = 4096
     pts = orc.g1_chain(n, k, d)
@@ -548,20 +549,15 @@ def test_pair_sum_rounds_edge_cases(ctx):
     try:
         for c in (6, 11):
             ctx.set_msm_window(c)
-            for rounds in (1, 2, 3, 4):
-                ctx.set_msm_pair_rounds(rounds)
-                for name, s in cases.items():
-                    assert ctx.g1_msm_device(dp, to_dev(s), n) == orc.g1_msm(pts, s), (c, rounds, name)
+            for name, s in cases.items():
+                assert ctx.g1_msm_device(dp, to_dev(s), n) == orc.g1_msm(pts, s), (c, name)
         ctx.set_msm_window(0)
         pts2 = orc.g2_chain(512, k, d)
         pts2[1] = pts2[0]
         s2 = orc.ints_to_array([3] * 512)
-        for rounds in (1, 3):
-            ctx.set_msm_pair_rounds(rounds)
-            assert ctx.g2_msm_device(to_dev(pts2), to_dev(s2), 512) == orc.g2_msm(pts2, s2)
+        assert ctx.g2_msm_device(to_dev(pts2), to_dev(s2), 512) == orc.g2_msm(pts2, s2)
     finally:
         ctx.set_msm_window(0)
-        ctx.set_msm_pair_rounds(-1)
 
 
 def test_pipelined_chunks_match(ctx):

@@ -14,7 +14,6 @@ exp = orc.g1_msm(pts, s)
 dp, ds = dev(pts), dev(s)
 assert ctx.g1_msm_device(dp, ds, n) == exp                       # one-shot plain
 ctx.set_msm_chunks(3); assert ctx.g1_msm_device(dp, ds, n) == exp; ctx.set_msm_chunks(0)   # pipelined
-ctx.set_msm_pair_rounds(2); assert ctx.g1_msm_device(dp, ds, n) == exp; ctx.set_msm_pair_rounds(-1)
 h = ctx.g1_bases_upload(pts, n); ctx.bases_precompute(h, 8)
 assert ctx.g1_msm_resident(h, s, n) == exp                        # table + host scalars
 ctx.bases_free(h)
