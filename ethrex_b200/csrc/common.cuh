@@ -86,6 +86,18 @@ struct BasesEntry {
   OnceTable fk20;
 };
 
+// a snarkjs Groth16 key loaded by b200zk_groth16_zkey_load (zkey.cu): its columns and key terms live in ctx->bases under
+// the handles below; the A and B coefficient rows are one CSR over 2 * domainSize rows (A's rows, then B's)
+struct ZkeyEntry {
+  uint32_t n_vars = 0, n_public = 0, log_n = 0, nnz = 0;
+  uint64_t col[5] = {0, 0, 0, 0, 0};  // A, B1, B2, C (signals n_public+1 ..), H
+  uint64_t terms_g1 = 0, terms_g2 = 0;  // alpha1, beta1, delta1 | beta2, delta2
+  DevBuf row_ptr, sig, val;  // CSR: 2 * domainSize + 1 offsets, nnz signal indices, nnz values (coef * R^2 mod r)
+  DevBuf one;                // the canonical 1: the quotient step's zinv (no division by Z on the odd coset)
+  uint8_t omega[32] = {};    // w_2n, canonical little-endian: the odd coset's generator
+  std::vector<uint8_t> vk;   // alpha1 | beta2 | gamma2 | delta2 | IC, EIP-196/197 bytes
+};
+
 }  // namespace b200zk
 
 struct b200zk_ctx {
@@ -127,6 +139,8 @@ struct b200zk_ctx {
   uint64_t ntt_root_id = 0;  // 0 = default; else a hash of ntt_root (part of the twiddle cache key)
   std::map<uint64_t, b200zk::TwiddleSet> twiddles;
   std::map<uint64_t, b200zk::BasesEntry> bases;
+  std::map<uint64_t, b200zk::ZkeyEntry> zkeys;  // handles share next_handle with the bases
+  b200zk::DevBuf ws_zkey;     // b200zk_groth16_zkey_prove: witness, evaluations and the evaluation's carries
   uint64_t next_handle = 1;
   uint8_t* h_pinned = nullptr;  // 4 KiB pinned staging for results / flags
 };
@@ -369,6 +383,12 @@ int ntt_set_root(b200zk_ctx* ctx, const uint8_t* root_le);
 int fr_quotient_dev(b200zk_ctx* ctx, const void* d_a, const void* d_b, const void* d_c, void* d_out, size_t n, const uint32_t* d_zinv_canonical, cudaStream_t st);
 // *d_zinv = device pointer to 1/(5^(2^log_n) - 1) (canonical limbs), computed once per log_n on `st`
 int fr_coset_zinv_dev(b200zk_ctx* ctx, uint32_t log_n, cudaStream_t st, const uint32_t** d_zinv);
+// the key-term pointers of a b200zk_groth16_zk after checking its handles and r, s (groth16.cu)
+int groth16_zk_terms(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void** g1, const void** g2);
+// exclusive scan of G counts (seg = 0) into out[0..G], out[G] = the total; cursor, if given, receives out[0..G) too;
+// tsum: one word per 2048 values (msm.cu)
+int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t* tsum,
+                   uint32_t* out, uint32_t* cursor = nullptr);
 int groth16_commit_partials(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const void* witness, void* a_evals, void* b_evals, void* c_evals,
                             uint32_t flags, cudaStream_t st, void* d_partials);
 // d_partials: count blocks of 768 B (A | B1 | B2 | L | H as XYZZ); d_out: proof A|B2|C (256 B) | B1 (64 B) | 4 x u32 is_infinity (A, B2, C, B1)

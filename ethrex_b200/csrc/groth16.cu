@@ -106,7 +106,7 @@ static bool fr_canonical(const uint8_t* x) {
 }
 
 // the key terms of a b200zk_groth16_zk: plain (not precomputed) BN254 bases of the right group and point count
-static int zk_terms(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void** g1, const void** g2) {
+int groth16_zk_terms(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void** g1, const void** g2) {
   if (!zk) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16 zk: null argument");
   static const char* kG1 = "groth16 zk: g1_terms must be a plain G1 handle of 3 points (alpha, beta, delta)";
   static const char* kG2 = "groth16 zk: g2_terms must be a plain G2 handle of 2 points (beta, delta)";
@@ -172,7 +172,7 @@ int b200zk_groth16_fold_zk(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const v
   if (!ctx || !proof || (!d_partials && count)) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_fold_zk: null argument");
   DeviceGuard guard(ctx);
   const void *g1 = nullptr, *g2 = nullptr;
-  B2_TRY(zk_terms(ctx, zk, &g1, &g2));
+  B2_TRY(groth16_zk_terms(ctx, zk, &g1, &g2));
   return fold_zk(ctx, zk, g1, g2, d_partials, count, pick_stream(ctx, stream), proof);
 }
 
@@ -181,7 +181,7 @@ int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const b20
   if (!ctx || !proof || !pk) return fail(ctx, B200ZK_ERR_INVALID_ARG, "groth16_prove: null argument");
   DeviceGuard guard(ctx);
   const void *g1 = nullptr, *g2 = nullptr;
-  B2_TRY(zk_terms(ctx, zk, &g1, &g2));
+  B2_TRY(groth16_zk_terms(ctx, zk, &g1, &g2));
   bool r_zero = true;
   for (int i = 0; i < 32; ++i) r_zero = r_zero && !zk->r[i];
   // C = ... + r [B]1: only r = 0 may skip the B_g1 column (what ark-groth16 does)

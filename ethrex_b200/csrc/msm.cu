@@ -1259,8 +1259,8 @@ static int launch_accumulate(b200zk_ctx* ctx, cudaStream_t st, const void* pts, 
 
 // exclusive scan of G values (scan_value: counts, or run flags when seg > 0) into out[0..G]; cursor, if given, receives
 // out[0..G) as well.  tsum: one word per kScanTile values.
-static int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t* tsum,
-                          uint32_t* out, uint32_t* cursor = nullptr) {
+int exclusive_scan(b200zk_ctx* ctx, cudaStream_t st, const uint32_t* in, const uint32_t* aux, size_t G, uint32_t seg, uint32_t* tsum,
+                   uint32_t* out, uint32_t* cursor) {
   const size_t tiles = (G + kScanTile - 1) / kScanTile;
   B2_LAUNCH(ctx, scan_tile_sums, (unsigned)tiles, kScanThreads, 0, st, in, aux, G, seg, tsum);
   B2_LAUNCH(ctx, scan_tile_offsets, 1, 1024, 0, st, tsum, tiles);

@@ -292,6 +292,59 @@ int b200zk_groth16_prove(b200zk_ctx* ctx, const b200zk_groth16_pk* pk, const b20
 int b200zk_groth16_fold_zk(b200zk_ctx* ctx, const b200zk_groth16_zk* zk, const void* d_partials, size_t count,
                            void* stream, uint8_t proof[256]);
 
+/* ---- Groth16 from circom artifacts: a snarkjs .zkey loaded once, each .wtns witness proved in one call ---------------
+ * The two files risc0-groth16's shrink-wrap hands its CUDA prover (a proving key fetched by rzup, a witness written by
+ * circom-witnesscalc + wtns-file), taken as they are.  The layouts are the ones snarkjs (zkey_utils.js, zkey_new.js,
+ * groth16_prove.js) writes and reads; this library defines no format of its own.
+ *
+ * Container (binfileutils): 4-byte magic, u32 version, u32 nSections, then nSections sections of u32 id | u64 size | size
+ * bytes, in any order; every integer little-endian.  .zkey: magic "zkey", version 1, sections 1..9 exactly once each (10,
+ * the ceremony's contributions, and unknown ids are skipped).  .wtns: magic "wtns", version 2, sections 1 and 2.  Nothing
+ * may follow the last section.
+ * .zkey sections (all points Montgomery little-endian, all-zero = identity: the "native" layout above, uploaded as is):
+ *   1  u32 protocol: 1 = Groth16; anything else (PLONK 2, FFLONK 10) is B200ZK_ERR_UNSUPPORTED
+ *   2  660 bytes: u32 n8q = 32 | q (32) | u32 n8r = 32 | r (32) | u32 nVars | u32 nPublic | u32 domainSize |
+ *      alpha1 (G1) | beta1 (G1) | beta2 (G2) | gamma2 (G2) | delta1 (G1) | delta2 (G2); q and r must be BN254's, domainSize
+ *      a power of two no larger than 2^27 (2^28 needs Fr.shift, Fr has no 2^29-th root of unity: UNSUPPORTED), and
+ *      nVars >= nPublic + 1.  nPublic excludes signal 0, the constant 1.
+ *   3  IC: nPublic + 1 G1 points
+ *   4  u32 nCoefs, then nCoefs records of 44 bytes: u32 matrix (0 = A, 1 = B) | u32 constraint | u32 signal | value, the
+ *      coefficient as coef * R^2 mod r (R = 2^256), 32 bytes little-endian: its Montgomery product with a canonical witness
+ *      value is the Montgomery form of coef * w.  snarkjs's rows A[nConstraints + i][i] = 1 (i = 0..nPublic) are among
+ *      them; C is not stored (c = a o b row by row).  A record with matrix > 1, constraint >= domainSize or signal >=
+ *      nVars refuses the key with B200ZK_ERR_INVALID_ARG; a value >= r with B200ZK_ERR_NOT_IN_FIELD.
+ *   5  A, 6  B1: nVars G1 points each     7  B2: nVars G2 points     8  C: nVars - nPublic - 1 G1 points (signals nPublic+1..)
+ *   9  H: domainSize G1 points, H_i = [L_{2i+1}(tau) / delta]1 with L_k the Lagrange polynomials of the doubled domain
+ * .wtns sections: 1  u32 n8 = 32 | the prime (32, must be r) | u32 nWitness (must equal the key's nVars);
+ *                 2  nWitness canonical little-endian 32-byte values, each < r (else B200ZK_ERR_NOT_IN_FIELD).
+ * A malformed container, a size or count that does not match the header, a missing or repeated section: INVALID_ARG;
+ * another version, protocol, curve or element size: UNSUPPORTED.  b200zk_last_error names the section and the field.
+ *
+ * Load checks every coordinate < q (B200ZK_ERR_NOT_IN_FIELD) and every point on its curve (B200ZK_ERR_NOT_ON_CURVE).  It
+ * checks no subgroup membership: neither snarkjs nor rapidsnark does, and on BN254 G1 every curve point is in it.
+ *
+ * The proof is snarkjs's / rapidsnark's for the same r and s:
+ *   a = A w, b = B w on the domain (from the section-4 rows; rows past the last coefficient are zero), c = a o b;
+ *   each of a, b, c through an iNTT, then multiplied by w_2n^j and through an NTT (an NTT on the coset w_2n <w_n>,
+ *   w_2n = the 2n-th root of unity of the ark / gnark / ffjavascript root, preset 0 below);
+ *   P = a b - c there, with no division by Z and no inverse transform: [H]1 = sum P_i H_i = [h(tau) Z(tau) / delta]1;
+ *   A = alpha1 + sum w_i A_i + r delta1      B = beta2 + sum w_i B2_i + s delta2      B1 = beta1 + sum w_i B1_i + s delta1
+ *   C = sum_{i > nPublic} w_i C_i + [H]1 + s A + r B1 - r s delta1
+ *   proof = A (64) | B (128, x_im|x_re|y_im|y_re) | C (64), EIP-196/197 bytes, as b200zk_groth16_prove. */
+/* Parses and validates the file, uploads A, B1, B2, C, H as resident columns and the key terms as the handles
+ * b200zk_groth16_zk takes (window tables for the five columns with precompute = 1), and sorts the section-4 records on the
+ * device into rows.  *key is a handle for the calls below.  A refused key leaves nothing allocated. */
+int b200zk_groth16_zkey_load(b200zk_ctx* ctx, const void* zkey, size_t len, int precompute, uint64_t* key);
+int b200zk_groth16_zkey_free(b200zk_ctx* ctx, uint64_t key);
+/* nVars, nPublic and log2(domainSize) (each pointer may be NULL), and the verifying key as EIP-196/197 bytes: alpha1 (64) |
+ * beta2 (128) | gamma2 (128) | delta2 (128) | IC (64 (nPublic + 1)); vk may be NULL, else vk_len must hold all of it */
+int b200zk_groth16_zkey_info(b200zk_ctx* ctx, uint64_t key, uint32_t* n_vars, uint32_t* n_public, uint32_t* log_n, uint8_t* vk, size_t vk_len);
+/* The proof of the witness in `wtns` (a whole .wtns file, HOST memory).  r, s: canonical little-endian, below the group
+ * order, else B200ZK_ERR_NOT_IN_FIELD; r = s = 0 gives the unblinded proof (the rules of b200zk_groth16_zk).  A context
+ * whose NTT root is not preset 0 is refused with B200ZK_ERR_INVALID_ARG.  One stream, one synchronisation at the end. */
+int b200zk_groth16_zkey_prove(b200zk_ctx* ctx, uint64_t key, const void* wtns, size_t len, const uint8_t r[32], const uint8_t s[32],
+                              void* stream, uint8_t proof[256]);
+
 /* ---- BLS12-381 G1 / EIP-4844 blob commitments (SURVEY.md section 8(f) rank 3) -------------------------------------
  * The L2 committer's "commit" step: /root/reference/crates/common/crypto/kzg.rs:259-272 (blob_to_kzg_commitment_and_proof ->
  * c_kzg blob_to_kzg_commitment), /root/reference/crates/common/types/blobs_bundle.rs:90-118, crates/l2/sequencer/

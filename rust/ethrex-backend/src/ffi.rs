@@ -200,6 +200,51 @@ impl B200zk {
         Ok(proof)
     }
 
+    /// Loads a snarkjs Groth16 proving key (the bytes of a `.zkey` file, as rzup fetches it for risc0-groth16) into HBM:
+    /// validated, columns resident, constraint rows sorted on the device.  `precompute` also builds the columns' window
+    /// tables.  Returns the key handle for `groth16_zkey_prove`.
+    pub fn groth16_zkey_load(&mut self, zkey: &[u8], precompute: bool) -> Result<u64, BackendError> {
+        let mut key = 0u64;
+        // SAFETY: the slice outlives the synchronous call; `key` is a valid out-pointer.
+        let status = unsafe { sys::b200zk_groth16_zkey_load(self.ctx.as_ptr(), zkey.as_ptr().cast(), zkey.len(), precompute as i32, &mut key) };
+        check(self, status)?;
+        Ok(key)
+    }
+
+    pub fn groth16_zkey_free(&mut self, key: u64) -> Result<(), BackendError> {
+        // SAFETY: plain handle; the library refuses unknown ones.
+        let status = unsafe { sys::b200zk_groth16_zkey_free(self.ctx.as_ptr(), key) };
+        check(self, status).map(|_| ())
+    }
+
+    /// (nVars, nPublic, log2 domainSize, verifying key alpha1 | beta2 | gamma2 | delta2 | IC as EIP-196/197 bytes)
+    pub fn groth16_zkey_info(&mut self, key: u64) -> Result<(u32, u32, u32, Vec<u8>), BackendError> {
+        let (mut nv, mut np, mut log_n) = (0u32, 0u32, 0u32);
+        // SAFETY: valid out-pointers; vk NULL asks for the sizes only.
+        let status = unsafe { sys::b200zk_groth16_zkey_info(self.ctx.as_ptr(), key, &mut nv, &mut np, &mut log_n, std::ptr::null_mut(), 0) };
+        check(self, status)?;
+        let mut vk = vec![0u8; 448 + 64 * (np as usize + 1)];
+        // SAFETY: vk holds the whole verifying key of this key (its length is passed).
+        let status = unsafe {
+            sys::b200zk_groth16_zkey_info(self.ctx.as_ptr(), key, std::ptr::null_mut(), std::ptr::null_mut(), std::ptr::null_mut(), vk.as_mut_ptr(), vk.len())
+        };
+        check(self, status)?;
+        Ok((nv, np, log_n, vk))
+    }
+
+    /// The Groth16 proof A | B2 | C (what snarkjs / rapidsnark return for the same r, s) of the witness in `wtns` (the bytes
+    /// of a `.wtns` file) under a key of `groth16_zkey_load`.  r, s: canonical little-endian, below the group order.
+    pub fn groth16_zkey_prove(&mut self, key: u64, wtns: &[u8], r: &[u8; 32], s: &[u8; 32]) -> Result<[u8; 256], BackendError> {
+        let mut proof = [0u8; 256];
+        // SAFETY: the buffers outlive the synchronous call; the library parses `wtns` within its length; NULL stream = the
+        // context's own.
+        let status = unsafe {
+            sys::b200zk_groth16_zkey_prove(self.ctx.as_ptr(), key, wtns.as_ptr().cast(), wtns.len(), r.as_ptr(), s.as_ptr(), std::ptr::null_mut(), proof.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(proof)
+    }
+
     pub fn g1_msm_resident(&mut self, handle: u64, scalars: &[u8], flags: u32) -> Result<[u8; 64], BackendError> {
         let mut out = [0u8; 64];
         // SAFETY: slice valid; n derived from its length.
