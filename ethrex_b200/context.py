@@ -527,6 +527,30 @@ class Context:
                     "b200zk_kzg_blob_to_commitment_and_cell_proofs")
         return [cm.raw[48 * i:48 * i + 48] for i in range(k)], [pr.raw[48 * i:48 * i + 48] for i in range(128 * k)]
 
+    def kzg_recover_cells_and_cell_proofs(self, g1_monomial: int, items) -> tuple:
+        """items: per blob an (indices, cells) pair, any 64 to 128 distinct cell indices and the 2048-byte cells at them
+        (a list of cells or their concatenation) -> ([128 cells per blob], [128 48-byte proofs per blob]), each flat,
+        blob-major with the cell index inner.  g1_monomial: a 4096-point G1 handle of the setup's [tau^i]1 points."""
+        k = len(items)
+        offsets = np.zeros(k + 1, dtype=np.uint32)
+        idx, data = [], []
+        for b, (indices, cells) in enumerate(items):
+            raw = cells if isinstance(cells, (bytes, bytearray, memoryview)) else b"".join(cells)
+            if len(raw) != 2048 * len(indices):
+                raise B200Error.serialization(f"blob {b}: {len(indices)} indices need {2048 * len(indices)} bytes of cells, got {len(raw)}")
+            offsets[b + 1] = offsets[b] + len(indices)
+            idx += [int(i) for i in indices]
+            data.append(bytes(raw))
+        ind = np.array(idx or [0], dtype=np.uint64)  # never a null pointer: an empty blob is the library's to refuse
+        blob = np.frombuffer(b"".join(data) or b"\0", dtype=np.uint8)
+        cells_out, proofs_out = C.create_string_buffer(max(1, 262144 * k)), C.create_string_buffer(max(1, 128 * 48 * k))
+        self._check(F.lib.b200zk_kzg_recover_cells_and_cell_proofs(self._h, g1_monomial, offsets.ctypes.data_as(C.c_void_p),
+                                                                   ind.ctypes.data_as(C.c_void_p),
+                                                                   blob.ctypes.data_as(C.c_void_p), k, cells_out, proofs_out),
+                    "b200zk_kzg_recover_cells_and_cell_proofs")
+        cr, pr = cells_out.raw, proofs_out.raw
+        return [cr[2048 * i:2048 * i + 2048] for i in range(128 * k)], [pr[48 * i:48 * i + 48] for i in range(128 * k)]
+
     def kzg_verify_cell_proof_batch(self, g1_setup: int, g2_setup: int, blobs, commitments, proofs) -> bool:
         """blobs: k x 131072 bytes, commitments k x 48 bytes, proofs k x 128 x 48 bytes (blob-major, cell index inner) ->
         one bool for every cell of every blob"""

@@ -9,6 +9,7 @@
 // So each blob takes an inverse and a forward NTT of size 4096 (128 KiB of Fr381, one CTA's shared memory), and the
 // 256 KiB of the full extension never has to sit in one CTA.
 #include "bls12.cuh"
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -49,9 +50,10 @@ __global__ void __launch_bounds__(256) kzg_cells_tw_build(void* __restrict__ tw)
 // In place over the 4096 elements in s, all threads of the CTA, s written and synchronised by the caller.  Twiddles of a
 // butterfly span 2h are powers of w_2h = w_8192^(8192 / 2h).  Elements may be canonical or Montgomery: the twiddles are
 // Montgomery, so mul keeps the input's form.
-// Inverse, Cooley-Tukey: bit-reversed values in, natural-order coefficients out, times 4096 (no scaling)
-B2_D void ntt_inverse_brp(uint4* s, const void* tw) {
-  for (uint32_t h = 1; h < kN; h <<= 1) {
+// Inverse, Cooley-Tukey: bit-reversed values in, natural-order coefficients out, times 4096 (no scaling).  With size < 4096
+// only the first log2(size) stages run: independent inverse NTTs of that size (times size) on each block of size elements.
+B2_D void ntt_inverse_brp(uint4* s, const void* tw, uint32_t size = kN) {
+  for (uint32_t h = 1; h < size; h <<= 1) {
     const uint32_t step = kExtN / (2 * h);
 #pragma unroll 1
     for (uint32_t b = threadIdx.x; b < kN / 2; b += kThreads) {
@@ -348,6 +350,110 @@ __global__ void __launch_bounds__(kDft / 2, 1) kzg_fk20_proofs(const void* __res
   bls_g1_compress(proofs + 48 * (base + kCellN + t), xyzz_to_affine(load_xyzz<Fp381>(s_pts, kCellN + t)));
 }
 
+// ---- cell recovery (c-kzg recover_cells_and_kzg_proofs) ------------------------------------------------------------
+// Write p = sum_(j<64) X^j P_j(X^64), deg P_j < 64, so c_(64 m + j) = P_j[m].  Cell c holds I_c = p mod (X^64 - s_c) on
+// its coset h_c <w_64> (point t at h_c w_64^brp6(t)), and I_c's coefficient j is P_j(s_c).  So per blob, from the first
+// 64 given cells k (indices c_k, distinct, hence distinct s_k = w_128^brp7(c_k)):
+//   E[k][j] = P_j(s_k) = NTT64^-1(cell k)[j] h_k^-j / 64           (64 inverse NTTs of size 64)
+//   P_j[m]  = sum_k E[k][j] Q_k[m] / Z'(s_k)                     (Lagrange on the s_k: Z = prod (X - s_k), Q_k = Z / (X - s_k))
+// one 64 x 64 by 64 x 64 product.  The forward NTT of the coefficients is the blob; tests/kzg_recover_ref.py restates
+// this method with the same indexing and checks it against the consensus-spec recovery.
+
+// One CTA per blob: blobs[b] (big-endian, as kzg_cells_extend takes it) from the first 64 of its given cells.  in: the
+// given cells of every blob in order (big-endian, checked < r), offsets[b] its first, idx their cell indices.  Scratch
+// per blob: lag (Q_k[m] at 64 k + m, Montgomery) and coef (c_i, canonical), 4096 elements each.
+__global__ void __launch_bounds__(kThreads, 1) kzg_recover_blob(const uint8_t* __restrict__ in, const uint32_t* __restrict__ offsets,
+                                                              const uint32_t* __restrict__ idx, const void* __restrict__ tw, void* lag,
+                                                              void* coef, uint8_t* __restrict__ blobs) {
+  extern __shared__ uint4 cells_smem[];
+  __shared__ uint4 s_pt[2 * kCellN];        // s_k (Montgomery)
+  __shared__ uint4 s_z[2 * (kCellN + 1)];   // Z's 65 coefficients (Montgomery)
+  __shared__ uint4 s_w[2 * kCellN];         // 1 / (64 Z'(s_k)) (Montgomery)
+  __shared__ uint32_t s_h[kCellN];          // brp7(c_k): h_k = w_8192^s_h[k]
+  const uint32_t t = threadIdx.x, first = offsets[blockIdx.x];
+  const uint8_t* given = in + (size_t)first * kCellN * 32;
+  void* q = (uint8_t*)lag + (size_t)blockIdx.x * kN * 32;
+  void* c = (uint8_t*)coef + (size_t)blockIdx.x * kN * 32;
+  for (uint32_t i = t; i < kN; i += kThreads) store_fe(cells_smem, i, load_be32(given + 32 * i));
+  if (t < kCellN) {
+    s_h[t] = brp7(idx[first + t]);
+    store_fe(s_pt, t, tw_at(tw, kCellN * s_h[t]));
+  }
+  if (t <= kCellN) store_fe(s_z, t, t ? Fr381::zero() : Fr381::one());
+  __syncthreads();
+  ntt_inverse_brp(cells_smem, tw, kCellN);
+  // Z = prod_k (X - s_k): coefficient t of Z (X - s_k) is z[t - 1] - s_k z[t]
+#pragma unroll 1
+  for (uint32_t k = 0; k < kCellN; ++k) {
+    Fr381 z;
+    if (t <= kCellN) z = Fr381::sub(t ? load_fe<Fr381>(s_z, t - 1) : Fr381::zero(), Fr381::mul(load_fe<Fr381>(s_pt, k), load_fe<Fr381>(s_z, t)));
+    __syncthreads();
+    if (t <= kCellN) store_fe(s_z, t, z);
+    __syncthreads();
+  }
+  // thread k: Q_k by synthetic division (Z is monic), and 1 / (64 Z'(s_k)) with Z'(s_k) = prod_(l != k) (s_k - s_l)
+  if (t < kCellN) {
+    const Fr381 s = load_fe<Fr381>(s_pt, t);
+    Fr381 a = Fr381::one();
+    store_fe(q, kCellN * t + kCellN - 1, a);
+#pragma unroll 1
+    for (uint32_t m = kCellN - 1; m; --m) {
+      a = Fr381::add(load_fe<Fr381>(s_z, m), Fr381::mul(s, a));
+      store_fe(q, kCellN * t + m - 1, a);
+    }
+    Fr381 d = Fr381::one();
+#pragma unroll 1
+    for (uint32_t l = 0; l < kCellN; ++l)
+      if (l != t) d = Fr381::mul(d, Fr381::sub(s, load_fe<Fr381>(s_pt, l)));
+#pragma unroll 1
+    for (int k = 0; k < 6; ++k) d = Fr381::dbl(d);
+    store_fe(s_w, t, Fr381::inv(d));
+  }
+  __syncthreads();
+  // E[k][j] (canonical) in place
+  for (uint32_t i = t; i < kN; i += kThreads) {
+    const uint32_t k = i / kCellN, j = i % kCellN;
+    const Fr381 unshift = Fr381::mul(tw_at(tw, (kExtN - s_h[k] * j) & (kExtN - 1)), load_fe<Fr381>(s_w, k));
+    store_fe(cells_smem, i, Fr381::mul(load_fe<Fr381>(cells_smem, i), unshift));
+  }
+  __syncthreads();
+  // c_(64 m + j) = sum_k E[k][j] Q_k[m]: a warp takes 32 consecutive j (one coalesced store) of one m
+  const uint32_t j = t % kCellN;
+#pragma unroll 1
+  for (uint32_t m = t / kCellN; m < kCellN; m += kThreads / kCellN) {
+    Fr381 acc = Fr381::zero();
+#pragma unroll 1
+    for (uint32_t k = 0; k < kCellN; ++k) acc = Fr381::add(acc, Fr381::mul(load_fe<Fr381>(cells_smem, kCellN * k + j), load_fe<Fr381>(q, kCellN * k + m)));
+    store_fe(c, kCellN * m + j, acc);
+  }
+  __syncthreads();
+  for (uint32_t i = t; i < kN; i += kThreads) store_fe(cells_smem, i, load_fe<Fr381>(c, i));
+  __syncthreads();
+  ntt_forward_brp(cells_smem, tw);
+  uint8_t* blob = blobs + (size_t)blockIdx.x * kN * 32;
+  for (uint32_t i = t; i < kN; i += kThreads) store_be32(blob + 32 * i, load_fe<Fr381>(cells_smem, i));
+}
+
+// One CTA per blob: bad[b] = the first position among the blob's given cells whose bytes differ from the rebuilt cell of
+// its index in ext (n x 8192 x 32 bytes), or 0xffffffff when every given cell agrees
+__global__ void __launch_bounds__(kThreads) kzg_recover_check(const uint8_t* __restrict__ in, const uint32_t* __restrict__ offsets,
+                                                              const uint32_t* __restrict__ idx, const uint8_t* __restrict__ ext, uint32_t* __restrict__ bad) {
+  __shared__ uint32_t s_bad;
+  if (!threadIdx.x) s_bad = 0xffffffffu;
+  __syncthreads();
+  constexpr uint32_t kWords = kCellN * 32 / 16;  // 16-byte words per cell
+  const uint32_t first = offsets[blockIdx.x], count = offsets[blockIdx.x + 1] - first;
+  const uint4* given = reinterpret_cast<const uint4*>(in) + (size_t)first * kWords;
+  const uint4* rebuilt = reinterpret_cast<const uint4*>(ext) + (size_t)blockIdx.x * kCells * kWords;
+  for (uint32_t w = threadIdx.x; w < count * kWords; w += kThreads) {
+    const uint32_t pos = w / kWords;
+    const uint4 a = __ldg(given + w), e = __ldg(rebuilt + idx[first + pos] * kWords + w % kWords);
+    if (a.x != e.x || a.y != e.y || a.z != e.z || a.w != e.w) atomicMin(&s_bad, pos);
+  }
+  __syncthreads();
+  if (!threadIdx.x) bad[blockIdx.x] = s_bad;
+}
+
 // the twiddle table, built on first use
 int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
   B2_TRY(once_table(ctx, ctx->kzg_cells_tw, (kExtN + 1) * 32, st, [&](void* t) -> int {
@@ -359,6 +465,7 @@ int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_fk20_columns, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColSmem));
+    B2_CUDA(ctx, cudaFuncSetAttribute(kzg_recover_blob, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     ctx->attr_kzg_cells = true;
   }
   return B200ZK_OK;
@@ -370,6 +477,42 @@ int fk20_table(b200zk_ctx* ctx, BasesEntry& e, const void* tw, cudaStream_t st, 
     B2_LAUNCH(ctx, kzg_fk20_table, kCellN, kDft / 2, 0, st, (const void*)e.d.p, tw, t);
     return B200ZK_OK;
   }, table);
+}
+
+// the 128 proofs of each of n blobs (d_blobs, checked < r) by FK20 into d_proofs; scratch hat n x 128 x 64 x 32 bytes, u
+// n x 128 x 192 bytes
+int fk20_run(b200zk_ctx* ctx, BasesEntry& mono, const uint8_t* d_blobs, size_t n, void* d_hat, void* d_u, uint8_t* d_proofs, cudaStream_t st) {
+  const void *tw = nullptr, *table = nullptr;
+  B2_TRY(cells_tw(ctx, st, &tw));
+  B2_TRY(fk20_table(ctx, mono, tw, st, &table));
+  B2_LAUNCH(ctx, kzg_fk20_columns, (unsigned)n, kThreads, kColSmem, st, d_blobs, tw, d_hat);
+  const size_t n_msm = n * kDft;
+  B2_LAUNCH(ctx, kzg_fk20_msm, (unsigned)((n_msm + kMsmWarps - 1) / kMsmWarps), 32 * kMsmWarps, 0, st, table, (const void*)d_hat, n_msm, d_u);
+  B2_LAUNCH(ctx, kzg_fk20_proofs, (unsigned)n, kDft / 2, 0, st, (const void*)d_u, tw, d_proofs);
+  return B200ZK_OK;
+}
+
+// host checks of a recovery batch: offsets, 64..128 cells per blob, indices < 128 and distinct within a blob (status 2)
+int check_recover_indices(b200zk_ctx* ctx, const uint32_t* offsets, const uint64_t* indices, size_t n, const char* what) {
+  B2_TRY(check_offsets(ctx, offsets, n, what));
+  char msg[192];
+  for (size_t b = 0; b < n; ++b) {
+    const uint32_t count = offsets[b + 1] - offsets[b];
+    if (count < kCellN || count > kCells) {
+      snprintf(msg, sizeof msg, "%s: blob %zu has %u cells; recovery takes 64 to 128", what, b, count);
+      return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+    }
+    bool seen[kCells] = {};
+    for (uint32_t k = 0; k < count; ++k) {
+      const uint64_t c = indices[offsets[b] + k];
+      if (c >= kCells || seen[c]) {
+        snprintf(msg, sizeof msg, "%s: blob %zu, cell %u: index %llu is %s", what, b, k, (unsigned long long)c, c >= kCells ? "not below 128" : "repeated");
+        return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+      }
+      seen[c] = true;
+    }
+  }
+  return B200ZK_OK;
 }
 
 }  // namespace
@@ -439,19 +582,79 @@ int b200zk_kzg_blob_to_commitment_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_l
   }));
   B2_CUDA(ctx, cudaMemcpyAsync(d_blobs, blobs, n_blobs * kN * 32, cudaMemcpyHostToDevice, st));
   B2_TRY(check_blobs(ctx, d_blobs, n_blobs, 0, st, what));
-  const void *tw = nullptr, *table = nullptr;
-  B2_TRY(cells_tw(ctx, st, &tw));
-  B2_TRY(fk20_table(ctx, *mono, tw, st, &table));
-  B2_LAUNCH(ctx, kzg_fk20_columns, (unsigned)n_blobs, kThreads, kColSmem, st, (const uint8_t*)d_blobs, tw, (void*)d_hat);
-  const size_t n_msm = n_blobs * kDft;
-  B2_LAUNCH(ctx, kzg_fk20_msm, (unsigned)((n_msm + kMsmWarps - 1) / kMsmWarps), 32 * kMsmWarps, 0, st, table, (const void*)d_hat, n_msm, (void*)d_u);
-  B2_LAUNCH(ctx, kzg_fk20_proofs, (unsigned)n_blobs, kDft / 2, 0, st, (const void*)d_u, tw, d_proofs);
+  B2_TRY(fk20_run(ctx, *mono, d_blobs, n_blobs, d_hat, d_u, d_proofs, st));
   B2_TRY(kzg_msms(ctx, *lag, d_blobs, n_blobs, B200ZK_SCALARS_BE, d_partials, d_enc, st));
   std::vector<uint8_t> enc(n_blobs * 128);
   B2_CUDA(ctx, cudaMemcpyAsync(enc.data(), d_enc, enc.size(), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(proofs, d_proofs, n_blobs * kCells * 48, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   for (size_t b = 0; b < n_blobs; ++b) memcpy(commitments + 48 * b, &enc[128 * b], 48);
+  return B200ZK_OK;
+}
+
+int b200zk_kzg_recover_cells_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_monomial, const uint32_t* cell_offsets, const uint64_t* cell_indices,
+                                             const uint8_t* cells, size_t n_blobs, uint8_t* cells_out, uint8_t* proofs_out) {
+  static const char* what = "kzg_recover_cells_and_cell_proofs";
+  if (!ctx || (n_blobs && (!cell_offsets || !cell_indices || !cells || !cells_out || !proofs_out)))
+    return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_recover_cells_and_cell_proofs: null argument");
+  NvtxRange nvtx("b200zk:kzg_recover_cells_and_cell_proofs");
+  DeviceGuard guard(ctx);
+  BasesEntry* mono = nullptr;
+  B2_TRY(kzg_setup(ctx, g1_monomial, "kzg_recover_cells_and_cell_proofs (g1_monomial)", &mono));
+  if (!n_blobs) return B200ZK_OK;
+  B2_TRY(check_recover_indices(ctx, cell_offsets, cell_indices, n_blobs, what));
+  const size_t total = cell_offsets[n_blobs];
+  std::vector<uint32_t> meta(n_blobs + 1 + total);  // offsets, then the indices
+  for (size_t b = 0; b <= n_blobs; ++b) meta[b] = cell_offsets[b];
+  for (size_t k = 0; k < total; ++k) meta[n_blobs + 1 + k] = (uint32_t)cell_indices[k];
+  cudaStream_t st = ctx->stream;
+  const size_t cells_bytes = n_blobs * kExtN * 32, proofs_bytes = n_blobs * kCells * 48;
+  uint8_t *d_in, *d_lag, *d_coef, *d_blobs, *d_hat, *d_u, *d_out;
+  uint32_t* d_meta;
+  B2_TRY(carve(ctx, ctx->ws_kzg, [&](Carve& c) {
+    d_in = c.take<uint8_t>(total * kCellN * 32);
+    d_meta = c.take<uint32_t>(meta.size());
+    d_lag = c.take<uint8_t>(n_blobs * kN * 32);
+    d_coef = c.take<uint8_t>(n_blobs * kN * 32);
+    d_blobs = c.take<uint8_t>(n_blobs * kN * 32);
+    d_hat = c.take<uint8_t>(n_blobs * kDft * kCellN * 32);
+    d_u = c.take<uint8_t>(n_blobs * kDft * 192);
+    d_out = c.take<uint8_t>(cells_bytes + proofs_bytes + n_blobs * 4);  // cells | proofs | bad: one copy back
+  }));
+  uint8_t* d_proofs = d_out + cells_bytes;
+  uint32_t* d_bad = reinterpret_cast<uint32_t*>(d_proofs + proofs_bytes);
+  B2_CUDA(ctx, cudaMemcpyAsync(d_in, cells, total * kCellN * 32, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(d_meta, meta.data(), meta.size() * 4, cudaMemcpyHostToDevice, st));
+  size_t bad = total * kCellN;
+  B2_TRY(bls_scalars_check(ctx, d_in, total * kCellN, true, st, &bad));
+  if (bad < total * kCellN) {
+    const size_t pos = bad / kCellN, b = std::upper_bound(cell_offsets, cell_offsets + n_blobs + 1, (uint32_t)pos) - cell_offsets - 1;
+    char msg[192];
+    snprintf(msg, sizeof msg, "%s: blob %zu, cell %zu, element %zu is >= the BLS12-381 group order", what, b, pos - cell_offsets[b], bad % kCellN);
+    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+  }
+  const uint32_t* d_offsets = d_meta;
+  const uint32_t* d_idx = d_meta + n_blobs + 1;
+  const void* tw = nullptr;
+  B2_TRY(cells_tw(ctx, st, &tw));
+  B2_LAUNCH(ctx, kzg_recover_blob, (unsigned)n_blobs, kThreads, kSmem, st, (const uint8_t*)d_in, d_offsets, d_idx, tw, (void*)d_lag, (void*)d_coef, d_blobs);
+  B2_TRY(kzg_cells_run(ctx, d_blobs, n_blobs, d_out, st));
+  B2_LAUNCH(ctx, kzg_recover_check, (unsigned)n_blobs, kThreads, 0, st, (const uint8_t*)d_in, d_offsets, d_idx, (const uint8_t*)d_out, d_bad);
+  B2_TRY(fk20_run(ctx, *mono, d_blobs, n_blobs, d_hat, d_u, d_proofs, st));
+  std::vector<uint8_t> h(cells_bytes + proofs_bytes + n_blobs * 4);
+  B2_CUDA(ctx, cudaMemcpyAsync(h.data(), d_out, h.size(), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  for (size_t b = 0; b < n_blobs; ++b) {
+    uint32_t pos;
+    memcpy(&pos, &h[cells_bytes + proofs_bytes + 4 * b], 4);
+    if (pos == 0xffffffffu) continue;
+    char msg[224];
+    snprintf(msg, sizeof msg, "%s: blob %zu, cell %u (index %llu) does not lie on the polynomial of its first 64 cells", what, b, pos,
+             (unsigned long long)cell_indices[cell_offsets[b] + pos]);
+    return fail(ctx, B200ZK_ERR_NOT_ON_CURVE, msg);
+  }
+  memcpy(cells_out, h.data(), cells_bytes);
+  memcpy(proofs_out, h.data() + cells_bytes, proofs_bytes);
   return B200ZK_OK;
 }
 

@@ -25,6 +25,8 @@ device (`b200zk_kzg_compute_cells`, `b200zk_kzg_verify_cell_proof_batch`); verif
 points ([tau^64]2 is point 64).  `blob_to_commitment_and_cell_proofs` (kzg.rs:275-293, what `BlobsBundle::create_from_blobs`
 calls per blob for wrapper version 1) computes the commitment and the 128 cell proofs by FK20 on the device
 (`b200zk_kzg_blob_to_commitment_and_cell_proofs`); it needs `g1_monomial`, the setup's 4096 points [tau^i]1.
+`recover_cells_and_kzg_proofs` rebuilds all 128 cells and their proofs from any half of a blob's cells on the device
+(`b200zk_kzg_recover_cells_and_cell_proofs`), with the same `g1_monomial`.
 """
 from __future__ import annotations
 
@@ -249,6 +251,34 @@ class KzgSettings:
             if e.status == 2:
                 raise ValueError(str(e)) from e
             raise
+
+    def recover_cells_and_kzg_proofs(self, cell_indices, cells) -> tuple:
+        """c-kzg recover_cells_and_kzg_proofs: from any 64 or more of a blob's cells (distinct indices < 128, any order,
+        2048 bytes each), ([128 cells], [128 cell proofs]).  ValueError on malformed input, and when more than 64 cells
+        do not all lie on one blob's extension (this library refuses such input rather than choose among the cells)."""
+        cells_out, proofs = self.recover_cells_and_kzg_proofs_batch([(cell_indices, cells)])
+        return cells_out[0], proofs[0]
+
+    def recover_cells_and_kzg_proofs_batch(self, items) -> tuple:
+        """items: per blob a (cell_indices, cells) pair -> ([[128 cells] per blob], [[128 cell proofs] per blob]) in one
+        device call (`b200zk_kzg_recover_cells_and_cell_proofs`)"""
+        if not hasattr(self.ctx, "kzg_recover_cells_and_cell_proofs"):
+            raise TypeError("cell recovery runs on the device: KzgSettings needs a Context")
+        if not self.g1_monomial_handle:
+            raise ValueError("cell proofs need the setup's monomial G1 points: pass g1_monomial")
+        items = [(list(ix), list(cs)) for ix, cs in items]
+        if any(len(ix) != len(cs) or any(len(c) != BYTES_PER_CELL for c in cs) for ix, cs in items):
+            raise ValueError("one 2048-byte cell per cell index")
+        if not items:
+            return [], []
+        try:
+            cells, proofs = self.ctx.kzg_recover_cells_and_cell_proofs(self.g1_monomial_handle, items)
+        except B200Error as e:
+            if e.status in (2, 3):
+                raise ValueError(str(e)) from e
+            raise
+        n = CELLS_PER_EXT_BLOB
+        return [cells[n * b:n * (b + 1)] for b in range(len(items))], [proofs[n * b:n * (b + 1)] for b in range(len(items))]
 
     def verify_cell_kzg_proof_batch(self, blobs, commitments, cell_proofs) -> bool:
         """verify_cell_kzg_proof_batch over whole blobs, as the reference calls it: every cell of every blob, each

@@ -444,6 +444,23 @@ int b200zk_kzg_compute_cells(b200zk_ctx* ctx, const uint8_t* blobs, size_t n_blo
  * commitments: n_blobs x 48 bytes; proofs: n_blobs x 128 x 48 bytes, blob-major with the cell index inner (compressed G1). */
 int b200zk_kzg_blob_to_commitment_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_lagrange, uint64_t g1_monomial, const uint8_t* blobs,
                                                   size_t n_blobs, uint8_t* commitments /* 48 n */, uint8_t* proofs /* 128 x 48 n */);
+/* c-kzg recover_cells_and_kzg_proofs for n_blobs blobs: from any 64 or more of a blob's 128 cells, all 128 cells and their
+ * 128 proofs.  Blob b's given cells are entries cell_offsets[b] .. cell_offsets[b+1] (cell_offsets[0] = 0, never
+ * decreasing, as pair_offsets): cell_indices[k] is entry k's cell index, cells + 2048 k its 64 elements.  Indices may come
+ * in any order.  cells_out: n_blobs x 128 x 2048 bytes, every cell in index order; proofs_out: n_blobs x 128 x 48 bytes,
+ * blob-major with the cell index inner, as b200zk_kzg_blob_to_commitment_and_cell_proofs returns them.
+ * g1_monomial: the 4096-point [tau^i]1 handle of that call, with the same rules (status 4 otherwise) and the same FK20
+ * table.  Rules, all checked before anything is written (nothing is written on failure; b200zk_last_error names the blob
+ * and the cell, or element, at fault): fewer than 64 or more than 128 cells for a blob, an index >= 128, an index repeated
+ * within a blob, or an element >= r return 2; null pointers with n_blobs > 0 return 4; n_blobs = 0 returns 0.
+ * Inconsistent input is refused, this library's own rule: the blob is rebuilt from its first 64 given cells, and when
+ * any other given cell differs from the rebuilt cell of its index (more than 64 cells that do not all lie on one
+ * polynomial of degree < 4096) the call returns 3 and names the first such cell; it never returns a best-effort answer.
+ * The proofs cost what the FK20 call's do. */
+int b200zk_kzg_recover_cells_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_monomial, const uint32_t* cell_offsets /* n_blobs + 1 */,
+                                             const uint64_t* cell_indices /* cell_offsets[n_blobs] */,
+                                             const uint8_t* cells /* cell_offsets[n_blobs] x 2048 B */, size_t n_blobs,
+                                             uint8_t* cells_out /* n_blobs x 128 x 2048 B */, uint8_t* proofs_out /* n_blobs x 128 x 48 B */);
 /* verify_cell_kzg_proof_batch over whole blobs, the shape the reference calls it with: every blob's 128 cells, cell
  * indices 0..127, each commitment standing for its blob's 128 cells; proofs are blob-major, 128 per blob, cell index inner
  * (48-byte compressed G1 each).  One answer, *valid = 1 or 0, from one two-pairing check of the universal equation

@@ -679,6 +679,31 @@ impl B200zk {
         Ok((commitments, proofs))
     }
 
+    /// c-kzg `recover_cells_and_kzg_proofs` for n = `cell_offsets.len() - 1` blobs: blob b's given cells are entries
+    /// `cell_offsets[b] .. cell_offsets[b + 1]` of `cell_indices` and `cells` (2048 bytes each), 64 to 128 distinct indices
+    /// below 128 in any order.  Returns (n x 128 cells of 2048 bytes, n x 128 x 48 cell-proof bytes), both blob-major with
+    /// the cell index inner.  `g1_monomial` is the setup's 4096 points [tau^i]1.  Malformed input, or given cells that do
+    /// not all lie on one blob's extension, is an error.
+    pub fn kzg_recover_cells_and_cell_proofs(&mut self, g1_monomial: u64, cell_offsets: &[u32], cell_indices: &[u64], cells: &[u8]) -> Result<(Vec<u8>, Vec<u8>), BackendError> {
+        const CELL: usize = 64 * 32;
+        let n = cell_offsets.len().saturating_sub(1);
+        let total = cell_offsets.last().map_or(0, |&t| t as usize);
+        if cell_offsets.is_empty() || cell_indices.len() != total || cells.len() != CELL * total {
+            return Err(BackendError::serialization("kzg_recover_cells_and_cell_proofs: need n + 1 offsets, and an index and 2048 bytes per given cell"));
+        }
+        let mut cells_out = vec![0u8; 128 * CELL * n];
+        let mut proofs = vec![0u8; 128 * 48 * n];
+        // SAFETY: `cell_offsets` holds n + 1 entries, `cell_indices` and `cells` one index and 2048 bytes for each of the
+        // `cell_offsets[n]` given cells (the library checks the offsets before reading through them); the outputs hold 128
+        // cells and 128 proofs per blob.
+        let status = unsafe {
+            sys::b200zk_kzg_recover_cells_and_cell_proofs(self.ctx.as_ptr(), g1_monomial, cell_offsets.as_ptr(), cell_indices.as_ptr(), cells.as_ptr(), n,
+                                                          cells_out.as_mut_ptr(), proofs.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok((cells_out, proofs))
+    }
+
     /// `verify_cell_kzg_proof_batch` over whole blobs (every cell, each commitment once per blob, proofs blob-major with
     /// 128 per blob): one answer; malformed input is an error.  `g1_setup` is the 4096-point Lagrange setup, `g2_setup`
     /// the setup's 65 G2 points.
