@@ -180,6 +180,7 @@ int b200zk_init(int device, b200zk_ctx** out) {
     return B200ZK_ERR_CUDA;
   }
   for (auto& e : ctx->ev) cudaEventCreate(&e);
+  for (auto& e : ctx->ev_plonk) cudaEventCreate(&e);
   {
     // The accumulation gathers 64-byte affine points at random: with the default L2 fetch granularity every gather pulls
     // 128 bytes out of HBM, twice the bytes the gather uses.  A 64-byte granularity is
@@ -213,6 +214,7 @@ void b200zk_destroy(b200zk_ctx* ctx) {
   if (ctx->stream_upload) cudaStreamDestroy(ctx->stream_upload);
   for (auto& kv : ctx->twiddles) { cudaFree(kv.second.d); if (kv.second.ready) cudaEventDestroy(kv.second.ready); }
   for (auto& e : ctx->ev) if (e) cudaEventDestroy(e);
+  for (auto& e : ctx->ev_plonk) if (e) cudaEventDestroy(e);
   if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   const int own = ctx->device;

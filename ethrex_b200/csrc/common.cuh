@@ -98,6 +98,21 @@ struct ZkeyEntry {
   std::vector<uint8_t> vk;   // alpha1 | beta2 | gamma2 | delta2 | IC, EIP-196/197 bytes
 };
 
+// a snarkjs PLONK key loaded by b200zk_plonk_zkey_load (plonk.cu): PTau lives in ctx->bases under `ptau`; the rest is
+// the key's own (all Fr values Montgomery)
+struct PlonkEntry {
+  uint32_t n_vars = 0, n_public = 0, log_n = 0, n_additions = 0, n_constraints = 0;
+  uint64_t ptau = 0;
+  DevBuf coef;     // Qm Ql Qr Qo Qc S1 S2 S3: domainSize coefficients each
+  DevBuf coset;    // the same 8, then L1, on the coset 5 <w_4n>: 4 domainSize values each
+  DevBuf sigma_h;  // S1 S2 S3 on the domain <w_n>
+  DevBuf maps;     // the A, B, C maps: nConstraints u32 each
+  DevBuf adds;     // the additions in level order: uint4 (dst, s1, s2, 0) each, then f1 and f2 as two Fr arrays
+  std::vector<uint32_t> level_off;  // additions of level k are [level_off[k], level_off[k + 1])
+  DevBuf consts;   // the constants of plonk.cu's kC* slots, then the verifying key's 736 bytes
+  std::vector<uint8_t> vk;
+};
+
 }  // namespace b200zk
 
 struct b200zk_ctx {
@@ -131,6 +146,8 @@ struct b200zk_ctx {
   bool profiling = false;
   float phase_ms[6] = {0, 0, 0, 0, 0, 0};
   cudaEvent_t ev[8] = {};
+  cudaEvent_t ev_plonk[6] = {};  // with profiling: the round boundaries of the last b200zk_plonk_zkey_prove
+  float plonk_round_ms[5] = {0, 0, 0, 0, 0};
   // grow-only workspaces (every DevBuf, OnceTable and BasesEntry frees itself when the context is deleted)
   b200zk::DevBuf ws_buckets, ws_chunkS, ws_chunkV, ws_result, ws_points, ws_scalars, ws_ntt, ws_misc, ws_out, ws_segbucket;
   // 2^28-th primitive root of unity of Fr the NTT derives its domain generators from (canonical limbs).
@@ -141,6 +158,8 @@ struct b200zk_ctx {
   std::map<uint64_t, b200zk::BasesEntry> bases;
   std::map<uint64_t, b200zk::ZkeyEntry> zkeys;  // handles share next_handle with the bases
   b200zk::DevBuf ws_zkey;     // b200zk_groth16_zkey_prove: witness, evaluations and the evaluation's carries
+  std::map<uint64_t, b200zk::PlonkEntry> plonk_keys;  // b200zk_plonk_zkey_load; handles share next_handle too
+  b200zk::DevBuf ws_plonk;    // b200zk_plonk_zkey_prove: witness, polynomials, coset values, scans, challenges, proof
   uint64_t next_handle = 1;
   uint8_t* h_pinned = nullptr;  // 4 KiB pinned staging for results / flags
 };

@@ -1,4 +1,4 @@
-// zkey_parse.h -- the snarkjs .zkey (Groth16) and .wtns containers, parsed and validated on the host.
+// zkey_parse.h -- the snarkjs .zkey (Groth16 and PLONK) and .wtns containers, parsed and validated on the host.
 //
 // Plain C++ with no CUDA types, so that tests can build it into a CPU program.  The one piece the device shares is
 // zkey_coef_check, the check of a section-4 coefficient record: the key loader runs it on every record in a kernel
@@ -33,7 +33,26 @@ struct ZkeyLayout {
   const uint8_t *a = nullptr, *b1 = nullptr, *b2 = nullptr, *c = nullptr, *h = nullptr;  // sections 5..9
 };
 
+// A snarkjs PLONK key (protocol 2).  Points are native affine G1 (64 B) / G2 (128 B), Fr values Montgomery little-endian.
+// Every range below has been size-checked, every map entry, addition operand and Fr value range-checked, and every
+// coordinate checked < q (the curve check is the loader's, on the device).
+struct PlonkLayout {
+  uint32_t n_vars = 0, n_public = 0, domain_size = 0, log_n = 0, n_additions = 0, n_constraints = 0;
+  const uint8_t *k1 = nullptr, *k2 = nullptr;   // section 2, 32 bytes each
+  const uint8_t* points = nullptr;              // section 2: Qm Ql Qr Qo Qc S1 S2 S3 (G1), then X_2 (G2)
+  const uint8_t* additions = nullptr;           // section 3: n_additions records of kPlonkAddBytes
+  const uint8_t* map[3] = {nullptr, nullptr, nullptr};  // sections 4..6: n_constraints u32 each
+  const uint8_t* q[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // sections 7..11: n coefficients, then 4n evaluations
+  const uint8_t* sigma = nullptr;               // section 12: S1, S2, S3 in the same form, 5n values apart
+  const uint8_t* ptau = nullptr;                // section 14: domainSize + 6 G1 points
+};
+constexpr size_t kPlonkAddBytes = 72;     // u32 s1 | u32 s2 | f1 | f2 (Montgomery)
+constexpr size_t kPlonkHeaderBytes = 796;
+constexpr uint32_t kPlonkMaxLogN = 26;    // the coset transforms run at 4 domainSize <= 2^28
+constexpr uint32_t kPlonkMinLogN = 3;     // T's 3n + 6 coefficients must fit in 4n
+
 // Returns a B200ZK_* status; on a refusal *err names the section and the field.
+int plonk_zkey_parse(const uint8_t* data, size_t len, PlonkLayout* out, std::string* err);
 int zkey_parse(const uint8_t* data, size_t len, ZkeyLayout* out, std::string* err);
 // The witness of a key with n_vars signals: *values = section 2, n_vars canonical little-endian 32-byte values
 // (their range is checked on the device).

@@ -345,6 +345,70 @@ int b200zk_groth16_zkey_info(b200zk_ctx* ctx, uint64_t key, uint32_t* n_vars, ui
 int b200zk_groth16_zkey_prove(b200zk_ctx* ctx, uint64_t key, const void* wtns, size_t len, const uint8_t r[32], const uint8_t s[32],
                               void* stream, uint8_t proof[256]);
 
+/* ---- PLONK from circom artifacts: a snarkjs PLONK .zkey loaded once, each .wtns witness proved in one call ------------
+ * snarkjs 0.7's PLONK (plonk_setup.js, zkey_utils.js readHeaderPlonk, plonk_prove.js, plonk_verify.js): the proof system the
+ * same circom witness feeds without a per-circuit ceremony.  Same container and .wtns as the Groth16 zkey above; the .wtns
+ * holds nVars - nAdditions values.  PLONK keys have their own handles: a Groth16 key passed to these calls, or a PLONK key
+ * passed to the Groth16 ones, is an unknown key (B200ZK_ERR_INVALID_ARG).
+ * .zkey sections 1..14 exactly once each (unknown ids are skipped).  All Fr values Montgomery little-endian, all points the
+ * native layout (all-zero = identity):
+ *   1  u32 protocol = 2
+ *   2  796 bytes: u32 n8q = 32 | q | u32 n8r = 32 | r | u32 nVars | u32 nPublic | u32 domainSize | u32 nAdditions |
+ *      u32 nConstraints | k1 | k2 (Fr) | Qm Ql Qr Qo Qc S1 S2 S3 (G1) | X_2 (G2).  nVars counts the additions.
+ *      domainSize: a power of two, 8 <= domainSize and 4 domainSize <= 2^28 (else UNSUPPORTED); nPublic <= nConstraints <=
+ *      domainSize; nVars >= nAdditions + nPublic + 1.
+ *   3  nAdditions records of 72 bytes: u32 s1 | u32 s2 | f1 | f2: signal nVars - nAdditions + i = f1 w[s1] + f2 w[s2].
+ *      Record i may read only signals < nVars - nAdditions + i.  snarkjs never writes anything else (it would read zero for
+ *      a later one); refusing such a key (INVALID_ARG) is this library's rule.
+ *   4, 5, 6  the A, B and C maps: nConstraints u32 signal ids each, every one < nVars.  Rows >= nConstraints are zero.
+ *   7..11  Qm, Ql, Qr, Qo, Qc: domainSize coefficients, then 4 domainSize evaluations on the 4n-th roots of unity
+ *   12  S1, S2, S3, each in that form
+ *   13  the Lagrange polynomials L_1 .. L_max(nPublic, 1) in that form (snarkjs's plonk_setup.js writes L_1 even for a
+ *       circuit without public inputs; read from its source, not checked against a snarkjs-written file)
+ *   14  PTau: domainSize + 6 G1 points [tau^i]1
+ * The 4n evaluations and section 13 are size- and range-checked, then not used.  Every Fr value must be < r
+ * (NOT_IN_FIELD), every coordinate < q (NOT_IN_FIELD), every point on its curve (NOT_ON_CURVE).  b200zk_last_error names
+ * the section and the field.  A refused key leaves nothing allocated.
+ *
+ * The proof is snarkjs 0.7's (9 G1 points and 6 evaluations, no eval_r, T in three parts) for the blinding b1..b11:
+ *   a, b, c: w through the maps; A = iNTT(a) + (b1 X + b2) Z_H, B likewise with b3, b4, C with b5, b6 (Z_H = X^n - 1)
+ *   Z(w^0) = 1, Z(w^(i+1)) = Z(w^i) num_i / den_i with num_i = (a + beta w^i + gamma)(b + beta k1 w^i + gamma)(c + beta
+ *     k2 w^i + gamma) and den_i = (a + beta S1 + gamma)(b + beta S2 + gamma)(c + beta S3 + gamma); Z += (b7 X^2 + b8 X +
+ *     b9) Z_H.  The product over all rows must be 1, else INVALID_ARG "witness does not satisfy the copy constraints".
+ *   T = (gates + PI + alpha (permutation) + alpha^2 (Z - 1) L1) / Z_H with PI = -sum_{i < nPublic} a_i L_i; T's
+ *     coefficients at 3n + 6 and above must be zero, else INVALID_ARG "witness does not satisfy the gates".
+ *     T1 = T[0, n) + b10 X^n, T2 = T[n, 2n) - b10 + b11 X^n, T3 = T[2n, 3n + 6) - b11.
+ *   the evaluations a, b, c, S1, S2 at xi and Z at xi w; the linearisation R of plonk_verify.js with its constant r0, so
+ *     that Wxi = (R + v1 (A - a) + v2 (B - b) + v3 (C - c) + v4 (S1 - s1) + v5 (S2 - s2)) / (X - xi) and
+ *     Wxiw = (Z - zw) / (X - xi w).
+ *   Every commitment is an MSM over PTau.  w = w_n of the preset-0 root (snarkjs's Fr.w).
+ * Transcript (snarkjs's Keccak256Transcript): each challenge is keccak256 of the concatenation, read big-endian, mod r.
+ *   A G1 point is 64 bytes x | y big-endian affine, an Fr value 32 bytes big-endian canonical.
+ *   beta = H(Qm Ql Qr Qo Qc S1 S2 S3, the public inputs (a_0 .. a_(nPublic-1)), A, B, C)   gamma = H(beta)
+ *   alpha = H(beta, gamma, Z)   xi = H(alpha, T1, T2, T3)   v1 = H(xi, the six evaluations), v_i = v1^i (i <= 5)
+ *   (the verifier adds u = H(Wxi, Wxiw)).  An identity commitment enters as 64 zero bytes; ffjavascript's
+ *   toRprUncompressed may flag it with 0x40 instead (not verified: it needs a degenerate circuit or all-zero blinding).
+ * Proof, 768 bytes, snarkjs's Solidity calldata order: A B C Z T1 T2 T3 Wxi Wxiw (64 bytes each, x | y big-endian,
+ * identity all-zero), then eval_a eval_b eval_c eval_s1 eval_s2 eval_zw (32 bytes big-endian each). */
+/* Parses and validates the file, uploads PTau as a resident handle (window tables with precompute = 1) and precomputes
+ * the key's polynomials on the domain and on the quotient's coset.  A context whose NTT root is not preset 0 is refused
+ * with B200ZK_ERR_INVALID_ARG. */
+int b200zk_plonk_zkey_load(b200zk_ctx* ctx, const void* zkey, size_t len, int precompute, uint64_t* key);
+int b200zk_plonk_zkey_free(b200zk_ctx* ctx, uint64_t key);
+/* nVars, nPublic, log2(domainSize) (each may be NULL) and the verifying key, 736 bytes (vk may be NULL): Qm Ql Qr Qo Qc S1 S2
+ * S3 (64 each, EIP-196) | X_2 (128, x_im | x_re | y_im | y_re) | k1 | k2 | w (32 each, big-endian canonical) */
+int b200zk_plonk_zkey_info(b200zk_ctx* ctx, uint64_t key, uint32_t* n_vars, uint32_t* n_public, uint32_t* log_n, uint8_t* vk, size_t vk_len);
+/* The proof of the witness in `wtns` (a whole .wtns file, HOST memory).  blinding = b1..b11, 32 bytes each, canonical
+ * little-endian and < r (else B200ZK_ERR_NOT_IN_FIELD); the library draws no randomness, and all zeros gives the proof
+ * without blinding.  Statuses: a witness count other than nVars - nAdditions INVALID_ARG, a witness value >= r
+ * NOT_IN_FIELD, the copy-constraint and gate failures above INVALID_ARG, a context whose NTT root is not preset 0
+ * INVALID_ARG.  Nothing is written to proof on failure.  One stream, one synchronisation at the end. */
+int b200zk_plonk_zkey_prove(b200zk_ctx* ctx, uint64_t key, const void* wtns, size_t len, const uint8_t blinding[11 * 32], void* stream,
+                            uint8_t proof[768]);
+/* with b200zk_set_profiling on: device time of rounds 1..5 of the last b200zk_plonk_zkey_prove on this context, in
+ * milliseconds, from CUDA events at the round boundaries (profiling also makes the MSMs run unchunked) */
+int b200zk_plonk_last_round_ms(b200zk_ctx* ctx, float out_ms[5]);
+
 /* ---- BLS12-381 G1 / EIP-4844 blob commitments (SURVEY.md section 8(f) rank 3) -------------------------------------
  * The L2 committer's "commit" step: /root/reference/crates/common/crypto/kzg.rs:259-272 (blob_to_kzg_commitment_and_proof ->
  * c_kzg blob_to_kzg_commitment), /root/reference/crates/common/types/blobs_bundle.rs:90-118, crates/l2/sequencer/

@@ -245,6 +245,46 @@ impl B200zk {
         Ok(proof)
     }
 
+    /// Loads a snarkjs 0.7 PLONK proving key (the bytes of a PLONK `.zkey`) into HBM: PTau as resident bases (window tables
+    /// with `precompute`), the selector and permutation polynomials on the domain and on the quotient's coset.  Returns
+    /// the key handle for `plonk_zkey_prove`; Groth16 handles are not accepted there, nor PLONK handles by the Groth16 calls.
+    pub fn plonk_zkey_load(&mut self, zkey: &[u8], precompute: bool) -> Result<u64, BackendError> {
+        let mut key = 0u64;
+        // SAFETY: the library parses `zkey` within its length and copies what it keeps.
+        let status = unsafe { sys::b200zk_plonk_zkey_load(self.ctx.as_ptr(), zkey.as_ptr().cast(), zkey.len(), precompute as i32, &mut key) };
+        check(self, status)?;
+        Ok(key)
+    }
+
+    pub fn plonk_zkey_free(&mut self, key: u64) -> Result<(), BackendError> {
+        // SAFETY: plain handle.
+        let status = unsafe { sys::b200zk_plonk_zkey_free(self.ctx.as_ptr(), key) };
+        check(self, status)
+    }
+
+    /// (nVars, nPublic, log2 domainSize, vk): vk = Qm Ql Qr Qo Qc S1 S2 S3 | X_2 | k1 | k2 | w, 736 bytes.
+    pub fn plonk_zkey_info(&mut self, key: u64) -> Result<(u32, u32, u32, Vec<u8>), BackendError> {
+        let (mut nv, mut np, mut log_n) = (0u32, 0u32, 0u32);
+        let mut vk = vec![0u8; 736];
+        // SAFETY: out-pointers and a 736-byte buffer, all live for the call.
+        let status = unsafe { sys::b200zk_plonk_zkey_info(self.ctx.as_ptr(), key, &mut nv, &mut np, &mut log_n, vk.as_mut_ptr(), vk.len()) };
+        check(self, status)?;
+        Ok((nv, np, log_n, vk))
+    }
+
+    /// The 768-byte snarkjs 0.7 PLONK proof (A B C Z T1 T2 T3 Wxi Wxiw, then the six evaluations) of a `.wtns` witness.
+    /// blinding = b1..b11, 32 bytes each, canonical little-endian below the group order; the caller draws them.
+    pub fn plonk_zkey_prove(&mut self, key: u64, wtns: &[u8], blinding: &[[u8; 32]; 11]) -> Result<[u8; 768], BackendError> {
+        let mut proof = [0u8; 768];
+        // SAFETY: the buffers outlive the synchronous call ([[u8; 32]; 11] is 352 contiguous bytes); NULL stream = the
+        // context's own.
+        let status = unsafe {
+            sys::b200zk_plonk_zkey_prove(self.ctx.as_ptr(), key, wtns.as_ptr().cast(), wtns.len(), blinding.as_ptr().cast(), std::ptr::null_mut(), proof.as_mut_ptr())
+        };
+        check(self, status)?;
+        Ok(proof)
+    }
+
     pub fn g1_msm_resident(&mut self, handle: u64, scalars: &[u8], flags: u32) -> Result<[u8; 64], BackendError> {
         let mut out = [0u8; 64];
         // SAFETY: slice valid; n derived from its length.
