@@ -123,6 +123,7 @@ SIGNATURES = {
     "b200zk_kzg_blob_to_commitment_and_cell_proofs": (_int, [_ctx, _u64, _u64, _vp, _sz, _vp, _vp]),
     "b200zk_kzg_verify_cell_proof_batch": (_int, [_ctx, _u64, _u64, _vp, _vp, _vp, _sz, C.POINTER(_int)]),
     "b200zk_kzg_recover_cells_and_cell_proofs": (_int, [_ctx, _u64, _vp, _vp, _vp, _sz, _vp, _vp]),
+    "b200zk_kzg_verify_cells": (_int, [_ctx, _u64, _u64, _vp, _vp, _vp, _vp, _sz, C.POINTER(_int)]),
     "b200zk_bls12_381_g1_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g2_add_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),
     "b200zk_bls12_381_g1_msm_batch": (_int, [_ctx, _vp, _vp, _sz, _vp, _vp]),

@@ -563,6 +563,20 @@ class Context:
                     "b200zk_kzg_verify_cell_proof_batch")
         return valid.value == 1
 
+    def kzg_verify_cells(self, g1_setup: int, g2_setup: int, commitments, cell_indices, cells, proofs) -> bool:
+        """c-kzg verify_cell_kzg_proof_batch over any n cells: commitments n x 48 bytes, cell_indices n ints, cells n x 2048
+        bytes, proofs n x 48 bytes (each a list of items or their concatenation) -> one bool for every cell"""
+        n = len(cell_indices)
+        raws = [c if isinstance(c, (bytes, bytearray, memoryview)) else b"".join(c) for c in (commitments, cells, proofs)]
+        for raw, size, name in zip(raws, (48, 2048, 48), ("commitments", "cells", "proofs")):
+            _need(raw, size * n, f"b200zk_kzg_verify_cells {name}")
+        ind = np.array([int(i) for i in cell_indices], dtype=np.uint64)
+        bufs = [_host_ptr(b) if n else (None, None) for b in (raws[0], ind, raws[1], raws[2])]
+        valid = C.c_int(-1)
+        self._check(F.lib.b200zk_kzg_verify_cells(self._h, g1_setup, g2_setup, *[p for p, _ in bufs], n, C.byref(valid)),
+                    "b200zk_kzg_verify_cells")
+        return valid.value == 1
+
     # ------------------------------------------------------------------ NTT root of unity (SURVEY.md section 8c)
     NTT_ROOT_ARK, NTT_ROOT_HALO2 = 0, 1
 

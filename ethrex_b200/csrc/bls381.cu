@@ -8,6 +8,7 @@
 // The proof (c-kzg compute_kzg_proof / compute_blob_kzg_proof) evaluates p at z and builds the quotient on the device
 // (kzg_eval_quotient, over the scalar field Fr381), then commits to it with the same MSM.
 #include "bls12.cuh"
+#include "cell_batch.h"
 #include "sha256.h"
 #include <cstring>
 #include <vector>
@@ -217,6 +218,11 @@ int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big
   return B200ZK_OK;
 }
 
+int bls_scalars_check_enqueue(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big_endian, cudaStream_t st, unsigned long long* d_bad) {
+  if (n) B2_LAUNCH(ctx, bls_scalar_check, (unsigned)((n + 255) / 256), 256, 0, st, (const uint8_t*)d_scalars, n, big_endian ? 1 : 0, d_bad);
+  return B200ZK_OK;
+}
+
 }  // namespace b200zk
 
 using namespace b200zk;
@@ -306,20 +312,6 @@ void b200zk::kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], ui
   uint8_t d[32];
   h.final(d);
   hash_to_bls_field(d, z_be);
-}
-
-// the digest read as a big-endian integer and reduced mod r (< 2^256 < 3r: at most two subtractions)
-void b200zk::hash_to_bls_field(const uint8_t d[32], uint8_t z_be[32]) {
-  uint32_t v[8];
-  for (int k = 0; k < 8; ++k) v[k] = (uint32_t)d[31 - 4 * k] | (uint32_t)d[30 - 4 * k] << 8 | (uint32_t)d[29 - 4 * k] << 16 | (uint32_t)d[28 - 4 * k] << 24;
-  for (int pass = 0; pass < 2; ++pass) {
-    uint32_t s[8];
-    uint64_t br = 0;
-    for (int k = 0; k < 8; ++k) { const uint64_t x = (uint64_t)v[k] - bls_r_limb(k) - br; s[k] = (uint32_t)x; br = (x >> 32) & 1u; }
-    if (!br) memcpy(v, s, sizeof v);  // v >= r
-  }
-  for (int k = 0; k < 8; ++k)
-    for (int j = 0; j < 4; ++j) z_be[31 - 4 * k - j] = (uint8_t)(v[k] >> (8 * j));
 }
 
 // y = p(z) of n blobs (kzg_eval_quotient, one CTA per blob); the quotient goes to q (n x 4096 x 32 bytes)

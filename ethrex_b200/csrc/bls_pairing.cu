@@ -17,6 +17,7 @@
 // order-r group mu_r.  tests/test_bls12_pairing_host.py recomputes every constant of this file and of
 // bls_pairing.cuh, which holds the pairing's stages, and checks the identity.
 #include "bls_pairing.cuh"
+#include "cell_batch.h"
 #include "sha256.h"
 #include <cstring>
 #include <vector>
@@ -225,6 +226,58 @@ int pairing_run(b200zk_ctx* ctx, const Affine<Fp381>* P, const BlsLine* lines, u
   return B200ZK_OK;
 }
 
+// the handles of a cell-proof check: the 4096-point Lagrange G1 setup, and a G2 setup of at least 65 points whose point 0
+// is the generator (point 64 is [tau^64]2)
+int cell_setups(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const char* what, const BasesEntry** g1, const BasesEntry** g2) {
+  const std::string msg = what;
+  *g1 = find_bases(ctx, g1_setup, Group::Bls12G1, (msg + ": unknown G1 setup handle").c_str());
+  if (!*g1) return B200ZK_ERR_INVALID_ARG;
+  if ((*g1)->n != 4096) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the G1 setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points").c_str());
+  B2_TRY(kzg_g2_setup(ctx, g2_setup, what, g2));
+  if ((*g2)->n < 65) return fail(ctx, B200ZK_ERR_INVALID_ARG, (msg + ": the G2 setup must hold at least 65 points ([tau^64]2 is point 64)").c_str());
+  return B200ZK_OK;
+}
+
+// the workspace of cell_check_tail, carved behind the caller's own buffers
+struct CellTail {
+  XYZZ<Fp381>* parts;
+  Affine<F2>* q2;
+  BlsLine* lines;
+  Affine<Fp381>* P;
+  uint8_t* pst;
+  F12* f;
+  uint32_t* offs;
+  uint8_t* res;
+  uint8_t* sts;
+  void take(Carve& c) {
+    parts = c.take<XYZZ<Fp381>>(3); q2 = c.take<Affine<F2>>(2); lines = c.take<BlsLine>(2 * kLines);
+    P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<F12>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
+  }
+};
+
+// The end of both cell-proof checks, from their scalars on the device: three MSMs (sum r^k pi_k over the m proofs; the
+// n_c commitments' weights and the r^k h_k^64 pi_k terms over pts = the n_c commitments then the m proofs; [A(tau)]1 over
+// the Lagrange setup with its window table), kzg_cell_fold, and one 2-pair check against (G2, [tau^64]2) into *valid
+int cell_check_tail(b200zk_ctx* ctx, const BasesEntry& g1, const BasesEntry& g2, const Affine<Fp381>* pts, size_t n_c, size_t m, const void* s_proof,
+                    const void* s_lin, const void* s_setup, const CellTail& w, cudaStream_t st, int* valid) {
+  B2_TRY(msm_run_bls(ctx, pts + n_c, s_proof, m, 0, st, w.parts));
+  B2_TRY(msm_run_bls(ctx, pts, s_lin, n_c + m, 0, st, w.parts + 1));
+  B2_TRY(msm_run_bls(ctx, g1.d.p, s_setup, g1.n, 0, st, w.parts + 2, g1.table_c, g1.n));
+  B2_LAUNCH(ctx, kzg_cell_fold, 1, 32, 0, st, (const XYZZ<Fp381>*)w.parts, w.P, w.pst);
+  const Affine<F2>* g2pts = (const Affine<F2>*)g2.d.p;
+  B2_CUDA(ctx, cudaMemcpyAsync(w.q2, g2pts, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(w.q2 + 1, g2pts + 64, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
+  B2_LAUNCH(ctx, bls_g2_prepare, 1, 64, 0, st, (const Affine<F2>*)w.q2, (const uint8_t*)nullptr, (size_t)2, w.lines);
+  const uint32_t h_offs[2] = {0, 2};
+  B2_CUDA(ctx, cudaMemcpyAsync(w.offs, h_offs, 8, cudaMemcpyHostToDevice, st));
+  B2_TRY(pairing_run(ctx, w.P, w.lines, 2, w.pst, 2, w.offs, 1, w.f, w.res, w.sts, st));
+  uint8_t h_res = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(&h_res, w.res, 1, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  *valid = h_res ? 1 : 0;
+  return B200ZK_OK;
+}
+
 }  // namespace
 }  // namespace b200zk
 
@@ -420,29 +473,20 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   if (!ctx || !valid || (n && (!blobs || !commitments || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: null argument");
   NvtxRange nvtx("b200zk:kzg_verify_cell_proof_batch");
   DeviceGuard guard(ctx);
-  const BasesEntry* g1 = find_bases(ctx, g1_setup, Group::Bls12G1, "kzg_verify_cell_proof_batch: unknown G1 setup handle");
-  if (!g1) return B200ZK_ERR_INVALID_ARG;
-  if (g1->n != kN) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G1 setup must hold FIELD_ELEMENTS_PER_BLOB = 4096 points");
-  const BasesEntry* e = nullptr;
-  B2_TRY(kzg_g2_setup(ctx, g2_setup, what, &e));
-  if (e->n < 65) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cell_proof_batch: the G2 setup must hold at least 65 points ([tau^64]2 is point 64)");
+  const BasesEntry *g1 = nullptr, *e = nullptr;
+  B2_TRY(cell_setups(ctx, g1_setup, g2_setup, what, &g1, &e));
   if (!n) { *valid = 1; return B200ZK_OK; }
   const size_t m = kCells * n;  // cells and proofs
   cudaStream_t st = ctx->stream;
-  uint8_t *d_blobs, *cells, *in, *pt_st, *rbe, *pst, *res, *sts;
+  uint8_t *d_blobs, *cells, *in, *pt_st, *rbe;
   void *weights, *partial, *s_proof, *s_lin, *s_setup;
-  Affine<Fp381>*pts, *P;
-  Affine<F2>* q2;
-  XYZZ<Fp381>* parts;
-  BlsLine* lines;
-  F12* f;
-  uint32_t* offs;
+  Affine<Fp381>* pts;
+  CellTail tail;
   B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
     d_blobs = c.take<uint8_t>(kBlob * n); cells = c.take<uint8_t>(kExt * n); in = c.take<uint8_t>(48 * (n + m));
     pts = c.take<Affine<Fp381>>(n + m); pt_st = c.take<uint8_t>(n + m); rbe = c.take<uint8_t>(32);
     weights = c.take<uint4>(2 * 65); partial = c.take<uint4>(2 * 64 * n); s_proof = c.take<uint4>(2 * m); s_lin = c.take<uint4>(2 * (n + m));
-    s_setup = c.take<uint4>(2 * kN); parts = c.take<XYZZ<Fp381>>(3); q2 = c.take<Affine<F2>>(2); lines = c.take<BlsLine>(2 * kLines);
-    P = c.take<Affine<Fp381>>(2); pst = c.take<uint8_t>(2); f = c.take<F12>(2); offs = c.take<uint32_t>(2); res = c.take<uint8_t>(1); sts = c.take<uint8_t>(1);
+    s_setup = c.take<uint4>(2 * kN); tail.take(c);
   }));
   char msg[160];
   // 1. every blob element < r (c-kzg blob_to_polynomial inside compute_cells): an error, not a false
@@ -489,22 +533,92 @@ int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint6
   //    [sum r^k I_k(tau)]1 over the Lagrange setup; 6. one 2-pair check against (G2, [tau^64]2)
   B2_CUDA(ctx, cudaMemcpyAsync(rbe, h_r, 32, cudaMemcpyHostToDevice, st));
   B2_TRY(kzg_cell_scalars_run(ctx, d_blobs, n, rbe, weights, partial, s_proof, s_lin, s_setup, st));
-  B2_TRY(msm_run_bls(ctx, pts + n, s_proof, m, 0, st, parts));
-  B2_TRY(msm_run_bls(ctx, pts, s_lin, n + m, 0, st, parts + 1));
-  B2_TRY(msm_run_bls(ctx, g1->d.p, s_setup, kN, 0, st, parts + 2, g1->table_c, g1->n));
-  B2_LAUNCH(ctx, kzg_cell_fold, 1, 32, 0, st, (const XYZZ<Fp381>*)parts, P, pst);
-  const Affine<F2>* g2pts = (const Affine<F2>*)e->d.p;
-  B2_CUDA(ctx, cudaMemcpyAsync(q2, g2pts, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
-  B2_CUDA(ctx, cudaMemcpyAsync(q2 + 1, g2pts + 64, sizeof(Affine<F2>), cudaMemcpyDeviceToDevice, st));
-  B2_LAUNCH(ctx, bls_g2_prepare, 1, 64, 0, st, (const Affine<F2>*)q2, (const uint8_t*)nullptr, (size_t)2, lines);
-  const uint32_t h_offs[2] = {0, 2};
-  B2_CUDA(ctx, cudaMemcpyAsync(offs, h_offs, 8, cudaMemcpyHostToDevice, st));
-  B2_TRY(pairing_run(ctx, P, lines, 2, pst, 2, offs, 1, f, res, sts, st));
-  uint8_t h_res = 0;
-  B2_CUDA(ctx, cudaMemcpyAsync(&h_res, res, 1, cudaMemcpyDeviceToHost, st));
+  return cell_check_tail(ctx, *g1, *e, pts, n, m, s_proof, s_lin, s_setup, tail, st, valid);
+}
+
+
+int b200zk_kzg_verify_cells(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const uint8_t* commitments, const uint64_t* cell_indices,
+                            const uint8_t* cells, const uint8_t* proofs, size_t n, int* valid) {
+  static const char* what = "kzg_verify_cells";
+  constexpr size_t kCell = kBatchCellBytes, kElems = kBatchCellN;
+  if (!ctx || !valid || (n && (!commitments || !cell_indices || !cells || !proofs))) return fail(ctx, B200ZK_ERR_INVALID_ARG, "kzg_verify_cells: null argument");
+  NvtxRange nvtx("b200zk:kzg_verify_cells");
+  DeviceGuard guard(ctx);
+  const BasesEntry *g1 = nullptr, *e = nullptr;
+  B2_TRY(cell_setups(ctx, g1_setup, g2_setup, what, &g1, &e));
+  if (!n) { *valid = 1; return B200ZK_OK; }
+  char msg[192];
+  // 1. cell indices < 128, then the deduplicated commitments and the groupings by commitment and by cell index (host)
+  CellBatch b;
+  const size_t bad_index = cell_batch_build(commitments, cell_indices, n, &b);
+  if (bad_index < n) {
+    snprintf(msg, sizeof msg, "%s: cell %zu: index %llu is not below 128", what, bad_index, (unsigned long long)cell_indices[bad_index]);
+    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+  }
+  const size_t u = b.unique.size(), n_cols = b.columns.size();
+  std::vector<uint8_t> h_commit(48 * u);
+  for (size_t i = 0; i < u; ++i) memcpy(&h_commit[48 * i], commitments + 48 * (size_t)b.unique[i], 48);
+  // meta: idx (n) | commit_off (u + 1) | by_commit (n) | column_off (n_cols + 1) | by_column (n) | columns (n_cols)
+  std::vector<uint32_t> meta;
+  meta.reserve(3 * n + u + 2 * n_cols + 2);
+  for (size_t k = 0; k < n; ++k) meta.push_back((uint32_t)cell_indices[k]);
+  for (const std::vector<uint32_t>* v : {&b.commit_off, &b.by_commit, &b.column_off, &b.by_column, &b.columns}) meta.insert(meta.end(), v->begin(), v->end());
+  cudaStream_t st = ctx->stream;
+  uint8_t *in, *d_cells, *pt_st, *rbe;
+  uint32_t* d_meta;
+  unsigned long long* d_bad;
+  void *rpow, *partial, *s_proof, *s_lin, *s_setup;
+  Affine<Fp381>* pts;
+  CellTail tail;
+  B2_TRY(carve(ctx, ctx->ws_pairing, [&](Carve& c) {
+    in = c.take<uint8_t>(48 * (u + n)); d_cells = c.take<uint8_t>(kCell * n); d_meta = c.take<uint32_t>(meta.size()); d_bad = c.take<unsigned long long>(1);
+    pts = c.take<Affine<Fp381>>(u + n); pt_st = c.take<uint8_t>(u + n); rbe = c.take<uint8_t>(32);
+    rpow = c.take<uint4>(2 * n); partial = c.take<uint4>(2 * kElems * n_cols); s_proof = c.take<uint4>(2 * n); s_lin = c.take<uint4>(2 * (u + n));
+    s_setup = c.take<uint4>(2 * 4096); tail.take(c);
+  }));
+  VCellsMeta vm;
+  vm.n = n; vm.n_commit = u; vm.n_cols = n_cols;
+  vm.idx = d_meta; vm.commit_off = vm.idx + n; vm.by_commit = vm.commit_off + u + 1;
+  vm.column_off = vm.by_commit + n; vm.by_column = vm.column_off + n_cols + 1; vm.columns = vm.by_column + n;
+  // 2. enqueue the inputs, the decompression and subgroup checks of the deduplicated commitments and the proofs
+  //    (c-kzg validate_kzg_g1), and the range check of every cell element
+  const unsigned long long h_bad = kElems * n;
+  B2_CUDA(ctx, cudaMemcpyAsync(in, h_commit.data(), 48 * u, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(in + 48 * u, proofs, 48 * n, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(d_meta, meta.data(), 4 * meta.size(), cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(d_bad, &h_bad, 8, cudaMemcpyHostToDevice, st));
+  // every copy before the first kernel: a copy from pageable memory queued behind the subgroup checks would hold the
+  // host until they finish, and the hash with it
+  B2_CUDA(ctx, cudaMemcpyAsync(d_cells, cells, kCell * n, cudaMemcpyHostToDevice, st));
+  B2_LAUNCH(ctx, bls_g1_decode_subgroup, (unsigned)((u + n + 63) / 64), 64, 0, st, (const uint8_t*)in, u + n, pts, pt_st);
+  B2_TRY(bls_scalars_check_enqueue(ctx, d_cells, kElems * n, true, st, d_bad));
+  // 3. while they run: r = compute_verify_cell_kzg_proof_batch_challenge over the caller's buffers (host SHA-256)
+  uint8_t h_r[32];
+  cell_batch_challenge(b, commitments, cell_indices, cells, proofs, h_r);
+  // 4. the statuses, in the spec's order: the deduplicated commitments, the cell elements, the proofs
+  std::vector<uint8_t> h_st(u + n);
+  unsigned long long h_bad_out = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(h_st.data(), pt_st, u + n, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&h_bad_out, d_bad, 8, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  *valid = h_res ? 1 : 0;
-  return B200ZK_OK;
+  auto point_error = [&](size_t p) {
+    if (p < u) snprintf(msg, sizeof msg, "%s: the commitment of cell %u ", what, b.unique[p]);
+    else snprintf(msg, sizeof msg, "%s: the proof of cell %zu ", what, p - u);
+    const std::string text = std::string(msg) + (h_st[p] == B200ZK_ERR_NOT_IN_FIELD ? "has a coordinate >= p" : "has malformed flag bits, is not on the curve or not in the order-r subgroup");
+    return fail(ctx, h_st[p], text.c_str());
+  };
+  for (size_t p = 0; p < u; ++p)
+    if (h_st[p]) return point_error(p);
+  if (h_bad_out < kElems * n) {
+    snprintf(msg, sizeof msg, "%s: cell %llu, element %llu is >= the BLS12-381 group order", what, h_bad_out / kElems, h_bad_out % kElems);
+    return fail(ctx, B200ZK_ERR_NOT_IN_FIELD, msg);
+  }
+  for (size_t p = u; p < u + n; ++p)
+    if (h_st[p]) return point_error(p);
+  // 5. the scalars on the device (r^k, the commitment weights, the per-column interpolation); 6. the shared tail
+  B2_CUDA(ctx, cudaMemcpyAsync(rbe, h_r, 32, cudaMemcpyHostToDevice, st));
+  B2_TRY(kzg_vcells_scalars_run(ctx, d_cells, vm, rbe, rpow, partial, s_proof, s_lin, s_setup, st));
+  return cell_check_tail(ctx, *g1, *e, pts, u, n, s_proof, s_lin, s_setup, tail, st, valid);
 }
 
 }  // extern "C"

@@ -390,6 +390,8 @@ int msm_encode_bls(b200zk_ctx* ctx, const void* d_partials, size_t count, uint32
 int bls_points_to_native(b200zk_ctx* ctx, const void* d_in, void* d_native, size_t n, bool compressed, cudaStream_t st);
 // first index of a 32-byte scalar (big-endian, or little-endian limbs) >= the BLS12-381 group order among n, or n
 int bls_scalars_check(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big_endian, cudaStream_t st, size_t* bad_index);
+// the same check enqueued on st without a synchronisation: *d_bad, set to n by the caller, ends as the first such index
+int bls_scalars_check_enqueue(b200zk_ctx* ctx, const void* d_scalars, size_t n, bool big_endian, cudaStream_t st, unsigned long long* d_bad);
 int msm_precompute_g1(b200zk_ctx* ctx, const void* d_bases, size_t n, uint32_t c, void* d_table, cudaStream_t st);
 int msm_precompute_g2(b200zk_ctx* ctx, const void* d_bases, size_t n, uint32_t c, void* d_table, cudaStream_t st);
 uint32_t precompute_window(size_t n);
@@ -419,10 +421,9 @@ int groth16_assemble_zk_dev(b200zk_ctx* ctx, const void* d_partials, size_t coun
 int bn254_g1_add_batch(b200zk_ctx* ctx, const uint8_t* a, const uint8_t* b, size_t count, uint8_t* out, uint8_t* status);
 int bn254_g1_mul_batch(b200zk_ctx* ctx, const uint8_t* points, const uint8_t* scalars, size_t count, uint8_t* out, uint8_t* status);
 int bn254_pairing_check_batch(b200zk_ctx* ctx, const uint8_t* pairs, const uint32_t* pair_offsets, size_t count, uint8_t* result, uint8_t* status);
-// EIP-4844 (bls381.cu): the Fiat-Shamir challenge of one blob, the digest-to-field reduction, and y = p(z) of n blobs on the
-// device (the quotient goes to d_q, n x 4096 x 32 bytes of scratch)
+// EIP-4844 (bls381.cu): the Fiat-Shamir challenge of one blob, and y = p(z) of n blobs on the device (the quotient goes to
+// d_q, n x 4096 x 32 bytes of scratch).  The digest-to-field reduction, hash_to_bls_field, is in cell_batch.h.
 void kzg_challenge(const uint8_t* blob, const uint8_t commitment[48], uint8_t z_be[32]);
-void hash_to_bls_field(const uint8_t digest[32], uint8_t out_be[32]);
 int kzg_eval_run(b200zk_ctx* ctx, const uint8_t* d_blobs, const uint8_t* d_z, size_t n, void* d_q, uint8_t* d_y, cudaStream_t st);
 // the setup handle of a KZG call: a BLS12-381 G1 handle of exactly 4096 points, else status 4 naming `what`
 int kzg_setup(b200zk_ctx* ctx, uint64_t handle, const char* what, BasesEntry** e);
@@ -436,6 +437,21 @@ int kzg_msms(b200zk_ctx* ctx, const BasesEntry& e, const uint8_t* scalars, size_
 int kzg_cells_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, uint8_t* d_cells, cudaStream_t st);
 int kzg_cell_scalars_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, const uint8_t* d_r_be, void* d_weights, void* d_partial,
                          void* d_s_proof, void* d_s_lin, void* d_s_setup, cudaStream_t st);
+// The same scalars for n arbitrary cells (b200zk_kzg_verify_cells, cells n x 2048 bytes big-endian, checked < r), from the
+// host's groupings (cell_batch.h) on the device: s_proof (n) = r^k; s_lin (n_commit + n) = each deduplicated commitment's
+// sum of r^k over its cells, then r^k h_k^64; s_setup (4096) as above.  Scratch: rpow n x 32 bytes, partial n_cols x 64
+// x 32 bytes
+struct VCellsMeta {
+  size_t n = 0, n_commit = 0, n_cols = 0;
+  const uint32_t* idx = nullptr;         // n: the cell index of each cell
+  const uint32_t* commit_off = nullptr;  // n_commit + 1, into by_commit (n)
+  const uint32_t* by_commit = nullptr;
+  const uint32_t* column_off = nullptr;  // n_cols + 1, into by_column (n); columns (n_cols): the cell indices that occur
+  const uint32_t* by_column = nullptr;
+  const uint32_t* columns = nullptr;
+};
+int kzg_vcells_scalars_run(b200zk_ctx* ctx, const uint8_t* d_cells, const VCellsMeta& m, const uint8_t* d_r_be, void* d_rpow, void* d_partial,
+                           void* d_s_proof, void* d_s_lin, void* d_s_setup, cudaStream_t st);
 
 // every element of n_blobs big-endian blobs, and of the n_extra z values right behind them, < r; else status 2 naming
 // `what` and the first offending blob and element (or z)

@@ -176,6 +176,70 @@ __global__ void __launch_bounds__(256) kzg_cells_scalars(const void* __restrict_
   store_fe(s_lin, k, Fr381::from_mont(Fr381::mul(rq, tw_at(tw, kCellN * brp7((uint32_t)(q % kCells))))));
 }
 
+// ---- the same check over arbitrary cells (b200zk_kzg_verify_cells) ---------------------------------------------------
+// Cell k carries its own commitment (index i_k among the deduplicated ones) and cell index c_k.  The interpolant of a
+// cell on its coset h_c <w_64> comes from its values alone: its values at h_c w_64^brp6(t) are y[t], so the inverse NTT
+// of size 64 (bit-reversed in, natural out) gives g(Y) = I(h_c Y), and I's coefficient j is g_j h_c^-j / 64.  Cells that
+// share a cell index share the coset, so A = sum_k r^k I_k is one such interpolation per cell index c that occurs, of
+// agg_c = sum_(k: c_k = c) r^k y_k, and its coefficients go through kzg_cells_interp_eval like the per-blob shares above.
+
+// one thread per cell: rpow[k] = r^k (Montgomery); s_proof[k] = r^k and s_lin[n_commit + k] = r^k h_(c_k)^64 (canonical)
+__global__ void __launch_bounds__(256) kzg_vcells_powers(const uint8_t* __restrict__ r_be, const void* __restrict__ tw, const uint32_t* __restrict__ idx,
+                                                          size_t n, size_t n_commit, void* __restrict__ rpow, void* __restrict__ s_proof, void* __restrict__ s_lin) {
+  const size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint32_t e[8] = {(uint32_t)k, (uint32_t)((uint64_t)k >> 32), 0, 0, 0, 0, 0, 0};
+  const Fr381 rk = Fr381::pow(Fr381::to_mont(load_be32(r_be)), e);
+  store_fe(rpow, k, rk);
+  store_fe(s_proof, k, Fr381::from_mont(rk));
+  store_fe(s_lin, n_commit + k, Fr381::from_mont(Fr381::mul(rk, tw_at(tw, kCellN * brp7(idx[k])))));
+}
+
+// one thread per deduplicated commitment i: s_lin[i] = sum r^k over its cells (by_commit[off[i] .. off[i + 1]))
+__global__ void __launch_bounds__(256) kzg_vcells_weights(const uint32_t* __restrict__ off, const uint32_t* __restrict__ by_commit, size_t n_commit,
+                                                           const void* __restrict__ s_proof, void* __restrict__ s_lin) {
+  const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (i >= n_commit) return;
+  Fr381 w = Fr381::zero();
+#pragma unroll 1
+  for (uint32_t q = off[i]; q < off[i + 1]; ++q) w = Fr381::add(w, load_fe_nc<Fr381>(s_proof, by_commit[q]));
+  store_fe(s_lin, i, w);
+}
+
+// One CTA per 64 of the cell indices that occur (columns[q], q < n_cols; cells by_column[off[q] .. off[q + 1])):
+// partial[64 q + j] = coefficient j of the interpolant of agg_q on its coset (canonical), the layout of kzg_cells_interp
+__global__ void __launch_bounds__(kThreads, 1) kzg_vcells_columns(const uint8_t* __restrict__ cells, const void* __restrict__ rpow,
+                                                                 const uint32_t* __restrict__ off, const uint32_t* __restrict__ by_column,
+                                                                 const uint32_t* __restrict__ columns, size_t n_cols, const void* __restrict__ tw,
+                                                                 void* __restrict__ partial) {
+  extern __shared__ uint4 cells_smem[];
+  const size_t first = (size_t)kCellN * blockIdx.x;
+  for (uint32_t e = threadIdx.x; e < kN; e += kThreads) {
+    const size_t q = first + e / kCellN;
+    Fr381 acc = Fr381::zero();
+    if (q < n_cols) {
+#pragma unroll 1
+      for (uint32_t s = off[q]; s < off[q + 1]; ++s) {
+        const uint32_t k = by_column[s];
+        acc = Fr381::add(acc, Fr381::mul(load_be32(cells + kCellN * 32 * (size_t)k + 32 * (e % kCellN)), load_fe_nc<Fr381>(rpow, k)));
+      }
+    }
+    store_fe(cells_smem, e, acc);
+  }
+  __syncthreads();
+  ntt_inverse_brp(cells_smem, tw, kCellN);
+  Fr381 inv64 = tw_at(tw, kExtN);  // 1/4096, doubled six times
+#pragma unroll 1
+  for (int k = 0; k < 6; ++k) inv64 = Fr381::dbl(inv64);
+  for (uint32_t e = threadIdx.x; e < kN; e += kThreads) {
+    const size_t q = first + e / kCellN;
+    if (q >= n_cols) break;
+    const uint32_t j = e % kCellN;
+    const Fr381 unshift = Fr381::mul(tw_at(tw, (kExtN - brp7(columns[q]) * j) & (kExtN - 1)), inv64);
+    store_fe(partial, first * kCellN + e, Fr381::mul(load_fe<Fr381>(cells_smem, e), unshift));
+  }
+}
+
 // ---- cell proofs by FK20 (c-kzg compute_cells_and_kzg_proofs) --------------------------------------------------------
 // pi_k = [q_k(tau)]1, q_k = (p - I_k) / (X^64 - s_k), is sum_(m=1..63) s_k^(m-1) T_m with the Toeplitz sums
 //   T_m = sum_(i <= 4095 - 64 m) c_(i + 64 m) [tau^i]1 = sum_b sum_(a <= 63 - m) C_b[a + m] S_b[a],
@@ -466,6 +530,7 @@ int cells_tw(b200zk_ctx* ctx, cudaStream_t st, const void** tw) {
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_cells_interp_eval, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_fk20_columns, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColSmem));
     B2_CUDA(ctx, cudaFuncSetAttribute(kzg_recover_blob, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
+    B2_CUDA(ctx, cudaFuncSetAttribute(kzg_vcells_columns, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
     ctx->attr_kzg_cells = true;
   }
   return B200ZK_OK;
@@ -532,6 +597,18 @@ int kzg_cell_scalars_run(b200zk_ctx* ctx, const uint8_t* d_blobs, size_t n, cons
   B2_LAUNCH(ctx, kzg_cells_interp, (unsigned)n, kThreads, kSmem, st, d_blobs, tw, (const void*)d_weights, d_partial);
   B2_LAUNCH(ctx, kzg_cells_interp_eval, 1, kThreads, kSmem, st, (const void*)d_partial, n, tw, d_s_setup);
   B2_LAUNCH(ctx, kzg_cells_scalars, (unsigned)(((kCells + 1) * n + 255) / 256), 256, 0, st, tw, (const void*)d_weights, n, d_s_proof, d_s_lin);
+  return B200ZK_OK;
+}
+
+int kzg_vcells_scalars_run(b200zk_ctx* ctx, const uint8_t* d_cells, const VCellsMeta& m, const uint8_t* d_r_be, void* d_rpow, void* d_partial,
+                           void* d_s_proof, void* d_s_lin, void* d_s_setup, cudaStream_t st) {
+  const void* tw = nullptr;
+  B2_TRY(cells_tw(ctx, st, &tw));
+  B2_LAUNCH(ctx, kzg_vcells_powers, (unsigned)((m.n + 255) / 256), 256, 0, st, d_r_be, tw, m.idx, m.n, m.n_commit, d_rpow, d_s_proof, d_s_lin);
+  B2_LAUNCH(ctx, kzg_vcells_weights, (unsigned)((m.n_commit + 255) / 256), 256, 0, st, m.commit_off, m.by_commit, m.n_commit, (const void*)d_s_proof, d_s_lin);
+  B2_LAUNCH(ctx, kzg_vcells_columns, (unsigned)((m.n_cols + kCellN - 1) / kCellN), kThreads, kSmem, st, d_cells, (const void*)d_rpow, m.column_off,
+            m.by_column, m.columns, m.n_cols, tw, d_partial);
+  B2_LAUNCH(ctx, kzg_cells_interp_eval, 1, kThreads, kSmem, st, (const void*)d_partial, m.n_cols, tw, d_s_setup);
   return B200ZK_OK;
 }
 

@@ -26,7 +26,10 @@ points ([tau^64]2 is point 64).  `blob_to_commitment_and_cell_proofs` (kzg.rs:27
 calls per blob for wrapper version 1) computes the commitment and the 128 cell proofs by FK20 on the device
 (`b200zk_kzg_blob_to_commitment_and_cell_proofs`); it needs `g1_monomial`, the setup's 4096 points [tau^i]1.
 `recover_cells_and_kzg_proofs` rebuilds all 128 cells and their proofs from any half of a blob's cells on the device
-(`b200zk_kzg_recover_cells_and_cell_proofs`), with the same `g1_monomial`.
+(`b200zk_kzg_recover_cells_and_cell_proofs`), with the same `g1_monomial`.  `verify_cells` is c-kzg's general
+`verify_cell_kzg_proof_batch(commitments, cell_indices, cells, proofs)` over any cells without their blobs, such as a
+data column or the cells about to be recovered (`b200zk_kzg_verify_cells`); it needs the same setup as the whole-blob
+check.
 """
 from __future__ import annotations
 
@@ -291,6 +294,22 @@ class KzgSettings:
             raise ValueError("a blob is 131072 bytes, a commitment and a proof 48 bytes")
         try:
             return self.ctx.kzg_verify_cell_proof_batch(self.handle, h, b"".join(blobs), b"".join(commitments), b"".join(cell_proofs))
+        except B200Error as e:
+            if e.status in (2, 3):
+                raise ValueError(str(e)) from e
+            raise
+
+    def verify_cells(self, commitments, cell_indices, cells, proofs) -> bool:
+        """c-kzg verify_cell_kzg_proof_batch(commitments, cell_indices, cells, proofs): one answer for any cells, each with
+        its own 48-byte commitment, cell index, 2048-byte cell and 48-byte proof; cells may repeat and share commitments.
+        ValueError on malformed input: an index >= 128, an element >= r, an invalid commitment or proof."""
+        h = self._verifier()
+        if not len(commitments) == len(cell_indices) == len(cells) == len(proofs):
+            raise ValueError("commitments, cell_indices, cells and proofs differ in length")
+        if any(len(c) != 48 for c in commitments) or any(len(c) != BYTES_PER_CELL for c in cells) or any(len(p) != 48 for p in proofs):
+            raise ValueError("a commitment and a proof are 48 bytes, a cell 2048 bytes")
+        try:
+            return self.ctx.kzg_verify_cells(self.handle, h, b"".join(commitments), list(cell_indices), b"".join(cells), b"".join(proofs))
         except B200Error as e:
             if e.status in (2, 3):
                 raise ValueError(str(e)) from e

@@ -543,6 +543,30 @@ int b200zk_kzg_recover_cells_and_cell_proofs(b200zk_ctx* ctx, uint64_t g1_monomi
 int b200zk_kzg_verify_cell_proof_batch(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const uint8_t* blobs,
                                        const uint8_t* commitments /* 48 n */, const uint8_t* proofs /* 128 x 48 n */, size_t n_blobs,
                                        int* valid);
+/* c-kzg verify_cell_kzg_proof_batch over any n_cells cells, each with its own commitment and cell index and no blob: a
+ * data column, a node's custody or sampling columns, or the cells about to go to b200zk_kzg_recover_cells_and_cell_proofs
+ * (recovery only checks its cells against one another, not against a commitment).  Cell k is commitments + 48 k,
+ * cell_indices[k], cells + 2048 k (64 big-endian elements) and proofs + 48 k (compressed G1).  Cells may repeat, indices
+ * may come in any order, and any number of cells may share a commitment.  One answer, *valid = 1 or 0, exactly as the
+ * consensus-specs verify_cell_kzg_proof_batch / _impl: the commitments are deduplicated in order of first occurrence,
+ * cell k gets the index i_k of its commitment among them, and
+ *   e(sum r^k pi_k, [tau^64]2) = e(sum_i w_i C_i - [sum r^k I_k(tau)]1 + sum r^k h_k^64 pi_k, [1]2),  w_i = sum_(k: i_k = i) r^k
+ * with I_k the interpolation polynomial of cell k on the coset h_k <w_64> of its index and r the spec's
+ * compute_verify_cell_kzg_proof_batch_challenge: SHA-256 of "RCKZGCBATCH__V1_", the sizes (4096, 64, the number of
+ * deduplicated commitments, n_cells as u64 big-endian), the deduplicated commitments, then per cell its commitment index
+ * and cell index (u64 big-endian), its 2048 bytes and its proof, reduced mod r.
+ * g1_setup and g2_setup: the two handles of b200zk_kzg_verify_cell_proof_batch, with the same rules (status 4 otherwise).
+ * Bad input is an error and *valid is not written.  Every check runs before any MSM, in this order, and the first
+ * failure is returned with b200zk_last_error naming the cell (for a commitment, the first cell that uses it):
+ *   1. a cell index >= 128: 2;
+ *   2. each deduplicated commitment, in order: a coordinate >= p: 2; bad flag bits, off the curve or outside the
+ *      order-r subgroup: 3 (the identity is valid);
+ *   3. a cell element >= r: 2 (the first in cell order);
+ *   4. each proof, in cell order: as the commitments.
+ * Null pointers with n_cells > 0 return 4.  n_cells = 0 returns 0 with *valid = 1. */
+int b200zk_kzg_verify_cells(b200zk_ctx* ctx, uint64_t g1_setup, uint64_t g2_setup, const uint8_t* commitments /* 48 n */,
+                            const uint64_t* cell_indices /* n */, const uint8_t* cells /* 2048 n */, const uint8_t* proofs /* 48 n */,
+                            size_t n_cells, int* valid);
 
 /* ---- EIP-2537 G1/G2 addition and multi-scalar multiplication -------------------------------------------------------
  * The Prague precompiles 0x0b-0x0e, `count` independent items per call, HOST buffers:

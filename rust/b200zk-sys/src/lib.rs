@@ -153,6 +153,7 @@ unsafe extern "C" {
     pub fn b200zk_kzg_blob_to_commitment_and_cell_proofs(ctx: *mut b200zk_ctx, g1_lagrange: u64, g1_monomial: u64, blobs: *const u8, n_blobs: usize, commitments: *mut u8, proofs: *mut u8) -> c_int;
     pub fn b200zk_kzg_verify_cell_proof_batch(ctx: *mut b200zk_ctx, g1_setup: u64, g2_setup: u64, blobs: *const u8, commitments: *const u8, proofs: *const u8, n_blobs: usize, valid: *mut c_int) -> c_int;
     pub fn b200zk_kzg_recover_cells_and_cell_proofs(ctx: *mut b200zk_ctx, g1_monomial: u64, cell_offsets: *const u32, cell_indices: *const u64, cells: *const u8, n_blobs: usize, cells_out: *mut u8, proofs_out: *mut u8) -> c_int;
+    pub fn b200zk_kzg_verify_cells(ctx: *mut b200zk_ctx, g1_setup: u64, g2_setup: u64, commitments: *const u8, cell_indices: *const u64, cells: *const u8, proofs: *const u8, n_cells: usize, valid: *mut c_int) -> c_int;
     pub fn b200zk_bls12_381_g1_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g2_add_batch(ctx: *mut b200zk_ctx, a: *const u8, b: *const u8, count: usize, out: *mut u8, status: *mut u8) -> c_int;
     pub fn b200zk_bls12_381_g1_msm_batch(ctx: *mut b200zk_ctx, pairs: *const u8, pair_offsets: *const u32, count: usize, out: *mut u8, status: *mut u8) -> c_int;

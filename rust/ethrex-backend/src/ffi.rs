@@ -761,6 +761,26 @@ impl B200zk {
         check(self, status)?;
         Ok(valid == 1)
     }
+
+    /// c-kzg `verify_cell_kzg_proof_batch(commitments, cell_indices, cells, proofs)` over any n cells without their blobs
+    /// (a data column, custody or sampling columns, the cells about to be recovered): 48 bytes of commitment, one index,
+    /// 2048 bytes of cell and 48 bytes of proof per cell.  One answer; malformed input is an error.  The handles are those
+    /// of `kzg_verify_cell_proof_batch`.
+    pub fn kzg_verify_cells(&mut self, g1_setup: u64, g2_setup: u64, commitments: &[u8], cell_indices: &[u64], cells: &[u8], proofs: &[u8]) -> Result<bool, BackendError> {
+        const CELL: usize = 64 * 32;
+        let n = cell_indices.len();
+        if commitments.len() != 48 * n || cells.len() != CELL * n || proofs.len() != 48 * n {
+            return Err(BackendError::serialization("kzg_verify_cells: need 48 + 2048 + 48 bytes and one index per cell"));
+        }
+        let mut valid: core::ffi::c_int = 0;
+        // SAFETY: every input holds n cells' worth of its items; `valid` is a valid out pointer.
+        let status = unsafe {
+            sys::b200zk_kzg_verify_cells(self.ctx.as_ptr(), g1_setup, g2_setup, commitments.as_ptr(), cell_indices.as_ptr(), cells.as_ptr(), proofs.as_ptr(), n,
+                                         &mut valid)
+        };
+        check(self, status)?;
+        Ok(valid == 1)
+    }
 }
 
 impl Drop for B200zk {
