@@ -83,6 +83,7 @@ SIGNATURES = {
     "b200zk_groth16_zkey_free": (_int, [_ctx, _u64]),
     "b200zk_groth16_zkey_info": (_int, [_ctx, _u64, C.POINTER(_u32), C.POINTER(_u32), C.POINTER(_u32), _vp, _sz]),
     "b200zk_groth16_zkey_prove": (_int, [_ctx, _u64, _vp, _sz, _vp, _vp, _vp, _vp]),
+    "b200zk_groth16_verify_batch": (_int, [_ctx, _vp, _sz, _vp, _vp, _sz, _vp, _vp, C.POINTER(_int)]),
     "b200zk_plonk_zkey_load": (_int, [_ctx, _vp, _sz, _int, C.POINTER(_u64)]),
     "b200zk_plonk_zkey_free": (_int, [_ctx, _u64]),
     "b200zk_plonk_zkey_info": (_int, [_ctx, _u64, C.POINTER(_u32), C.POINTER(_u32), C.POINTER(_u32), _vp, _sz]),

@@ -170,6 +170,25 @@ class Context:
                                                           count, res, st), "bn254_pairing_check_batch")
         return list(res.raw[:count]), list(st.raw[:count])
 
+    def groth16_verify_batch(self, vk: bytes, proofs, public_inputs):
+        """b200zk_groth16_verify_batch: proofs (count x 256 bytes A | B | C) against one verifying key (alpha1 | beta2 |
+        gamma2 | delta2 | IC, the layout of groth16_zkey_info), public_inputs count x n_pub 32-byte big-endian values (each
+        argument a list of items or their concatenation) -> ([valid bool], [status], batch_ok)"""
+        proofs = proofs if isinstance(proofs, (bytes, bytearray, memoryview)) else b"".join(proofs)
+        public_inputs = public_inputs if isinstance(public_inputs, (bytes, bytearray, memoryview)) else b"".join(public_inputs)
+        if len(vk) < 512 or (len(vk) - 448) % 64:
+            raise B200Error.serialization(f"b200zk_groth16_verify_batch vk: {len(vk)} bytes is not 448 + 64 (n_pub + 1)")
+        if len(proofs) % 256:
+            raise B200Error.serialization(f"b200zk_groth16_verify_batch proofs: {len(proofs)} bytes is not a whole number of 256-byte proofs")
+        n_pub, count = (len(vk) - 448) // 64 - 1, len(proofs) // 256
+        _need(public_inputs, 32 * n_pub * count, "b200zk_groth16_verify_batch public_inputs")
+        valid, st = C.create_string_buffer(max(1, count)), C.create_string_buffer(max(1, count))
+        ok = C.c_int(-1)
+        bufs = [_host_ptr(b) if len(b) else (None, None) for b in (vk, proofs, public_inputs)]
+        self._check(F.lib.b200zk_groth16_verify_batch(self._h, bufs[0][0], len(vk), bufs[1][0], bufs[2][0], count, valid, st, C.byref(ok)),
+                    "b200zk_groth16_verify_batch")
+        return [v == 1 for v in valid.raw[:count]], list(st.raw[:count]), ok.value == 1
+
     # ------------------------------------------------------------------ host-buffer entry points
     def g1_msm(self, points, scalars, n: int, flags: int = 0) -> bytes:
         return self._msm_host(F.lib.b200zk_g1_msm, 64, points, scalars, n, flags)

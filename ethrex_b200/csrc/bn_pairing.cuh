@@ -1,6 +1,6 @@
 // bn_pairing.cuh -- the stages of the BN254 ate pairing: the affine line function, the Miller loop and the final
-// exponentiation.  pairing.cu builds the ecPairing kernels on them; tests/csrc/pairing_conformance.cu runs each stage
-// alone.  See pairing.cu for the algorithm.
+// exponentiation, and the EIP-196/197 point decoding.  pairing.cu builds the ecPairing kernels on them, groth16_verify.cu
+// the batched Groth16 check; tests/csrc/pairing_conformance.cu runs each stage alone.  See pairing.cu for the algorithm.
 // Internal linkage (anonymous namespace, __constant__ tables): the build has no -rdc, so each translation unit that
 // includes this header holds its own copy.
 #pragma once
@@ -55,6 +55,11 @@ __device__ __noinline__ Fq12 miller_ate(const Affine<Fq2>& q, const Affine<Fq>& 
   return f;
 }
 
+// the Miller value of one pair of decoded points: 1 when either is the identity (the pair contributes nothing)
+B2_D Fq12 miller_pair(const Affine<Fq>& p, const Affine<Fq2>& q) {
+  return (p.is_inf() || q.is_inf()) ? Fq12::one() : miller_ate(q, p);
+}
+
 __device__ __noinline__ Fq12 final_exponentiate(const Fq12& f) {
   Fq12 b = Fq12::mul(Fq12::conj(f), Fq12::inv(f));  // f^(p^6 - 1)
   Fq12 acc = Fq12::one();
@@ -63,6 +68,35 @@ __device__ __noinline__ Fq12 final_exponentiate(const Fq12& f) {
     if ((kFinalExp[i >> 5] >> (i & 31)) & 1) acc = Fq12::mul(acc, b);
   }
   return acc;
+}
+
+// ---- decoding with the precompile's error order: field range first, then the curve ---------------------------
+// a 32-byte big-endian value as limbs of F (not reduced); *in_range = value < the modulus
+template <class F> B2_D F load_be(const uint8_t* in, bool* in_range) {
+  F v;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const uint8_t* b = in + 4 * (7 - k);
+    v.v[k] = ((uint32_t)b[0] << 24) | ((uint32_t)b[1] << 16) | ((uint32_t)b[2] << 8) | (uint32_t)b[3];
+  }
+  F m = F::modulus(), t;
+  *in_range = detail::sub8(t.v, v.v, m.v) != 0;
+  return v;
+}
+// 0 ok, 2 coordinate >= p, 3 not on the curve
+B2_D uint32_t decode_g1(const uint8_t* be, Affine<Fq>* out) {
+  bool okx, oky;
+  Fq x = load_be<Fq>(be, &okx), y = load_be<Fq>(be + 32, &oky);
+  if (!(okx && oky)) return B200ZK_ERR_NOT_IN_FIELD;
+  *out = {Fq::to_mont(x), Fq::to_mont(y)};
+  return affine_on_curve(*out) ? 0u : (uint32_t)B200ZK_ERR_NOT_ON_CURVE;
+}
+B2_D uint32_t decode_g2(const uint8_t* be, Affine<Fq2>* out) {
+  bool ok[4];
+  Fq xi = load_be<Fq>(be, &ok[0]), xr = load_be<Fq>(be + 32, &ok[1]), yi = load_be<Fq>(be + 64, &ok[2]), yr = load_be<Fq>(be + 96, &ok[3]);
+  if (!(ok[0] && ok[1] && ok[2] && ok[3])) return B200ZK_ERR_NOT_IN_FIELD;
+  *out = {{Fq::to_mont(xr), Fq::to_mont(xi)}, {Fq::to_mont(yr), Fq::to_mont(yi)}};
+  return affine_on_curve(*out) ? 0u : (uint32_t)B200ZK_ERR_NOT_ON_CURVE;
 }
 
 }  // namespace

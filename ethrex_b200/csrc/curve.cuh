@@ -120,10 +120,10 @@ template <class F> B2_HD Affine<F> xyzz_to_affine(const XYZZ<F>& p) {
   return {F::mul(p.x, zz_inv), F::mul(p.y, zzz_inv)};
 }
 
-// k * P, k = 256-bit little-endian limbs (double-and-add, MSB first).  Setup / utility use only.
-template <class F> B2_HD XYZZ<F> xyzz_scalar_mul(const uint32_t* k, const Affine<F>& p) {
+// k * P, k = `bits`-bit little-endian limbs (double-and-add, MSB first).  Setup / utility use only.
+template <class F> B2_HD XYZZ<F> xyzz_scalar_mul(const uint32_t* k, const Affine<F>& p, int bits = 256) {
   XYZZ<F> acc = XYZZ<F>::identity();
-  for (int i = 255; i >= 0; --i) {
+  for (int i = bits - 1; i >= 0; --i) {
     acc = xyzz_dbl(acc);
     if ((k[i >> 5] >> (i & 31)) & 1) xyzz_add_mixed(acc, p.x, p.y);
   }

@@ -20,39 +20,12 @@
 namespace b200zk {
 namespace {
 
-// ---- decoding with the precompile's error order: field range first, then the curve ---------------------------
-B2_D Fq load_be_fq(const uint8_t* in, bool* in_range) {
-  Fq v;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const uint8_t* b = in + 4 * (7 - k);
-    v.v[k] = ((uint32_t)b[0] << 24) | ((uint32_t)b[1] << 16) | ((uint32_t)b[2] << 8) | (uint32_t)b[3];
-  }
-  Fq m = Fq::modulus(), t;
-  *in_range = detail::sub8(t.v, v.v, m.v) != 0;
-  return v;
-}
 B2_D void store_be_fq(uint8_t* out, const Fq& canonical) {
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     uint32_t w = canonical.v[7 - k];
     out[4 * k] = (uint8_t)(w >> 24); out[4 * k + 1] = (uint8_t)(w >> 16); out[4 * k + 2] = (uint8_t)(w >> 8); out[4 * k + 3] = (uint8_t)w;
   }
-}
-// 0 ok, 2 coordinate >= p, 3 not on the curve
-B2_D uint32_t decode_g1(const uint8_t* be, Affine<Fq>* out) {
-  bool okx, oky;
-  Fq x = load_be_fq(be, &okx), y = load_be_fq(be + 32, &oky);
-  if (!(okx && oky)) return B200ZK_ERR_NOT_IN_FIELD;
-  *out = {Fq::to_mont(x), Fq::to_mont(y)};
-  return affine_on_curve(*out) ? 0u : (uint32_t)B200ZK_ERR_NOT_ON_CURVE;
-}
-B2_D uint32_t decode_g2(const uint8_t* be, Affine<Fq2>* out) {
-  bool ok[4];
-  Fq xi = load_be_fq(be, &ok[0]), xr = load_be_fq(be + 32, &ok[1]), yi = load_be_fq(be + 64, &ok[2]), yr = load_be_fq(be + 96, &ok[3]);
-  if (!(ok[0] && ok[1] && ok[2] && ok[3])) return B200ZK_ERR_NOT_IN_FIELD;
-  *out = {{Fq::to_mont(xr), Fq::to_mont(xi)}, {Fq::to_mont(yr), Fq::to_mont(yi)}};
-  return affine_on_curve(*out) ? 0u : (uint32_t)B200ZK_ERR_NOT_ON_CURVE;
 }
 B2_D void encode_g1(uint8_t* out, const Affine<Fq>& p) {
   store_be_fq(out, Fq::from_mont(p.x));
@@ -108,9 +81,7 @@ __global__ void __launch_bounds__(32) pairing_miller(const uint8_t* pairs, size_
   uint32_t sp = decode_g1(pairs + 192 * i, &p), sq = decode_g2(pairs + 192 * i + 64, &q);
   uint32_t s = (sp == B200ZK_ERR_NOT_IN_FIELD || sq == B200ZK_ERR_NOT_IN_FIELD) ? (uint32_t)B200ZK_ERR_NOT_IN_FIELD : (sp ? sp : sq);
   if (!s && !q.is_inf() && !in_subgroup<FrCfg::mod>(q)) s = B200ZK_ERR_NOT_ON_CURVE;  // G1 has cofactor 1: on the curve = in the group
-  Fq12 r = Fq12::one();
-  if (!s && !p.is_inf() && !q.is_inf()) r = miller_ate(q, p);
-  f[i] = r;
+  f[i] = s ? Fq12::one() : miller_pair(p, q);
   pair_status[i] = (uint8_t)s;
 }
 

@@ -26,6 +26,7 @@ import secrets
 from dataclasses import dataclass, field
 
 from . import _ffi as F
+from .errors import B200Error
 
 R_MOD = 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001
 COSET_GEN = 5  # ark/gnark multiplicative generator of Fr
@@ -139,12 +140,12 @@ class Groth16ZkProver(Groth16Prover):
 
 
 class Groth16Verifier:
-    """Groth16 verification on the device, many proofs per launch: what `ProverBackend::verify` does off-chain
+    """Groth16 verification on the device, many proofs per call: what `ProverBackend::verify` does off-chain
     (/root/reference/crates/prover/src/backend/mod.rs:116-117) and what the on-chain verifier contracts compute
     (/root/reference/crates/l2/contracts/src/l1/OnChainProposer.sol:365-388) --
         e(-A, B) * e(alpha, beta) * e(IC_0 + sum x_i IC_i, gamma) * e(C, delta) == 1
-    through b200zk_bn254_pairing_check_batch; the public-input combination is a small G1 MSM through the host entry
-    point.  All points are EIP-196/197 byte strings."""
+    `verify_batch` checks a whole batch with one pairing product (b200zk_groth16_verify_batch); `calldata` gives one
+    proof's ecpairing input for b200zk_bn254_pairing_check_batch.  All points are EIP-196/197 byte strings."""
     P_MOD = 0x30644E72E131A029B85045B68181585D97816A916871CA8D3C208C16D87CFD47
 
     def __init__(self, ctx, alpha_g1: bytes, beta_g2: bytes, gamma_g2: bytes, delta_g2: bytes, ic):
@@ -161,12 +162,19 @@ class Groth16Verifier:
             return None
         return g1 if (x == 0 and y == 0) else g1[:32] + (self.P_MOD - y).to_bytes(32, "big")
 
-    def calldata(self, proof: bytes, public_inputs):
-        """ecpairing calldata of the verification equation, or None when the proof / inputs are not canonically encoded
-        (a public input outside [0, r) is rejected, not reduced: x and x + r must not verify alike)."""
+    def _check_sizes(self, proof: bytes, public_inputs):
         if len(proof) != 256 or len(public_inputs) != len(self.ic) - 1:
             raise ValueError("proof must be 256 bytes and carry one public input per IC point after the first")
-        if any((not isinstance(x, int)) or x < 0 or x >= R_MOD for x in public_inputs):
+
+    @staticmethod
+    def _canonical_inputs(public_inputs) -> bool:
+        """a public input outside [0, r) is rejected, not reduced: x and x + r must not verify alike"""
+        return all(isinstance(x, int) and 0 <= x < R_MOD for x in public_inputs)
+
+    def calldata(self, proof: bytes, public_inputs):
+        """ecpairing calldata of the verification equation, or None when the proof / inputs are not canonically encoded"""
+        self._check_sizes(proof, public_inputs)
+        if not self._canonical_inputs(public_inputs):
             return None
         a, b, c = proof[:64], proof[64:192], proof[192:]
         neg_a = self._neg(a)
@@ -177,18 +185,25 @@ class Groth16Verifier:
         return neg_a + b + self.alpha_g1 + self.beta_g2 + vk_x + self.gamma_g2 + c + self.delta_g2
 
     def verify_batch(self, proofs, public_inputs):
-        """-> list of booleans; a proof with a malformed point (status != 0) or a non-canonical encoding is False."""
-        cds = [self.calldata(p, x) for p, x in zip(proofs, public_inputs)]
-        live = [cd for cd in cds if cd is not None]
-        res, st = self.ctx.bn254_pairing_check_batch(live) if live else ([], [])
-        it = iter(zip(res, st))
-        out = []
-        for cd in cds:
-            if cd is None:
-                out.append(False)
-            else:
-                r, s = next(it)
-                out.append(bool(r) and s == 0)
+        """-> list of booleans, one call of b200zk_groth16_verify_batch for the batch.  A proof with a malformed point or
+        a public input outside [0, r) is False; a verifying key the device refuses makes every proof False."""
+        items = list(zip(proofs, public_inputs))
+        for p, x in items:
+            self._check_sizes(p, x)
+        live = [i for i, (_, x) in enumerate(items) if self._canonical_inputs(x)]
+        out = [False] * len(items)
+        if not live:
+            return out
+        vk = self.alpha_g1 + self.beta_g2 + self.gamma_g2 + self.delta_g2 + b"".join(self.ic)
+        xs = b"".join(int(v).to_bytes(32, "big") for i in live for v in items[i][1])
+        try:
+            valid, _, _ = self.ctx.groth16_verify_batch(vk, b"".join(bytes(items[i][0]) for i in live), xs)
+        except B200Error as e:
+            if e.status in (F.ERR_NOT_IN_FIELD, F.ERR_NOT_ON_CURVE):
+                return out
+            raise
+        for i, v in zip(live, valid):
+            out[i] = v
         return out
 
     def verify(self, proof: bytes, public_inputs) -> bool:

@@ -345,6 +345,33 @@ int b200zk_groth16_zkey_info(b200zk_ctx* ctx, uint64_t key, uint32_t* n_vars, ui
 int b200zk_groth16_zkey_prove(b200zk_ctx* ctx, uint64_t key, const void* wtns, size_t len, const uint8_t r[32], const uint8_t s[32],
                               void* stream, uint8_t proof[256]);
 
+/* ---- Groth16 batch verification: `count` proofs against one verifying key, one pairing product for the batch ---------
+ * vk: the layout b200zk_groth16_zkey_info returns, alpha1 (64) | beta2 (128) | gamma2 (128) | delta2 (128) | IC (64 (n_pub
+ * + 1)), EIP-196/197 bytes (G2 as x_im | x_re | y_im | y_re); n_pub = (vk_len - 448) / 64 - 1.  A vk_len not of that form
+ * is B200ZK_ERR_INVALID_ARG.  A vk coordinate >= p fails the call with B200ZK_ERR_NOT_IN_FIELD, a point off its curve or a
+ * beta2 / gamma2 / delta2 outside the order-r subgroup with B200ZK_ERR_NOT_ON_CURVE (a range error anywhere in the key
+ * outranks a curve error); b200zk_last_error names the element.  Nothing is written on failure.
+ * proofs: count x 256 bytes A | B | C, as b200zk_groth16_prove returns them.  public_inputs: count x n_pub x 32 bytes,
+ * big-endian (may be NULL when n_pub = 0).
+ * Per proof, as the ecPairing precompile orders its errors: status[i] = 2 when a coordinate of A, B or C is >= p or a public
+ * input is >= r; else 3 when A or C is off the curve, or B off the twist or outside the order-r subgroup; else 0.  (0,0)
+ * is the identity and allowed.  valid[i] = 1 when status[i] = 0 and the proof satisfies
+ *   e(A, B) = e(alpha1, beta2) e(IC_0 + sum_j x_j IC_j, gamma2) e(C, delta2).
+ * A malformed proof (status != 0) is left out of the batch: it never changes another proof's verdict.
+ * The well-formed proofs are checked together with random coefficients rho_i:
+ *   prod_i e(-rho_i A_i, B_i) e((sum rho_i) alpha1, beta2) e(sum_j s_j IC_j, gamma2) e(sum rho_i C_i, delta2) = 1,
+ *   s_0 = sum_i rho_i, s_j = sum_i rho_i x_ij.
+ * When that holds every well-formed proof is valid (*batch_ok = 1).  Otherwise each is decided by its own 4-pair check on
+ * the device (*batch_ok = 0).  batch_ok may be NULL.
+ * The coefficients are Fiat-Shamir, so the call is deterministic and needs no randomness from the caller:
+ *   D = SHA-256("b200zk-groth16-batch-v1" (23 ASCII bytes) | vk | count as u64 big-endian | proofs | public_inputs)
+ *   rho_i = the first 16 bytes of SHA-256(D | i as u64 big-endian) read big-endian, or 1 if those bytes are all zero.
+ * Every input byte enters D, malformed proofs included.  count = 0 returns B200ZK_OK and writes nothing.  At most two host
+ * synchronisations. */
+int b200zk_groth16_verify_batch(b200zk_ctx* ctx, const uint8_t* vk, size_t vk_len, const uint8_t* proofs /* count*256 */,
+                                const uint8_t* public_inputs /* count*n_pub*32 */, size_t count, uint8_t* valid /* count */,
+                                uint8_t* status /* count */, int* batch_ok /* may be NULL */);
+
 /* ---- PLONK from circom artifacts: a snarkjs PLONK .zkey loaded once, each .wtns witness proved in one call ------------
  * snarkjs 0.7's PLONK (plonk_setup.js, zkey_utils.js readHeaderPlonk, plonk_prove.js, plonk_verify.js): the proof system the
  * same circom witness feeds without a per-circuit ceremony.  Same container and .wtns as the Groth16 zkey above; the .wtns

@@ -108,6 +108,7 @@ unsafe extern "C" {
     pub fn b200zk_groth16_zkey_free(ctx: *mut b200zk_ctx, key: u64) -> c_int;
     pub fn b200zk_groth16_zkey_info(ctx: *mut b200zk_ctx, key: u64, n_vars: *mut u32, n_public: *mut u32, log_n: *mut u32, vk: *mut u8, vk_len: usize) -> c_int;
     pub fn b200zk_groth16_zkey_prove(ctx: *mut b200zk_ctx, key: u64, wtns: *const c_void, len: usize, r: *const u8, s: *const u8, stream: *mut c_void, proof: *mut u8) -> c_int;
+    pub fn b200zk_groth16_verify_batch(ctx: *mut b200zk_ctx, vk: *const u8, vk_len: usize, proofs: *const u8, public_inputs: *const u8, count: usize, valid: *mut u8, status: *mut u8, batch_ok: *mut c_int) -> c_int;
     // PLONK from circom artifacts: a snarkjs 0.7 PLONK .zkey loaded once, each .wtns witness proved in one call
     pub fn b200zk_plonk_zkey_load(ctx: *mut b200zk_ctx, zkey: *const c_void, len: usize, precompute: c_int, key: *mut u64) -> c_int;
     pub fn b200zk_plonk_zkey_free(ctx: *mut b200zk_ctx, key: u64) -> c_int;

@@ -245,6 +245,27 @@ impl B200zk {
         Ok(proof)
     }
 
+    /// Verifies `proofs` (256 bytes A | B | C each) against one verifying key `vk` (the layout `groth16_zkey_info` returns,
+    /// 448 + 64 (n_pub + 1) bytes) with one pairing product for the batch; `public_inputs` holds n_pub 32-byte big-endian
+    /// values per proof.  One verdict per proof: a malformed proof is false, and never changes another proof's verdict.
+    pub fn groth16_verify_batch(&mut self, vk: &[u8], proofs: &[u8], public_inputs: &[u8]) -> Result<Vec<bool>, BackendError> {
+        if vk.len() < 512 || (vk.len() - 448) % 64 != 0 || proofs.len() % 256 != 0 {
+            return Err(BackendError::serialization("groth16_verify_batch: vk must be 448 + 64 (n_pub + 1) bytes and each proof 256 bytes"));
+        }
+        let (n_pub, count) = ((vk.len() - 448) / 64 - 1, proofs.len() / 256);
+        if public_inputs.len() != 32 * n_pub * count {
+            return Err(BackendError::serialization("groth16_verify_batch: need n_pub 32-byte public inputs per proof"));
+        }
+        let (mut valid, mut status) = (vec![0u8; count], vec![0u8; count]);
+        // SAFETY: every input holds `count` proofs' worth of its items, the outputs hold `count` bytes; NULL batch_ok is allowed.
+        let status_rc = unsafe {
+            sys::b200zk_groth16_verify_batch(self.ctx.as_ptr(), vk.as_ptr(), vk.len(), proofs.as_ptr(), public_inputs.as_ptr(), count, valid.as_mut_ptr(),
+                                             status.as_mut_ptr(), std::ptr::null_mut())
+        };
+        check(self, status_rc)?;
+        Ok(valid.iter().map(|&v| v == 1).collect())
+    }
+
     /// Loads a snarkjs 0.7 PLONK proving key (the bytes of a PLONK `.zkey`) into HBM: PTau as resident bases (window tables
     /// with `precompute`), the selector and permutation polynomials on the domain and on the quotient's coset.  Returns
     /// the key handle for `plonk_zkey_prove`; Groth16 handles are not accepted there, nor PLONK handles by the Groth16 calls.
